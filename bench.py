@@ -4,10 +4,12 @@ iterations per second on the 4-camera x 400-frame
 LENSMODEL_SPLINED_STEREOGRAPHIC_order=3_Nx=30_Ny=20_fov_x_deg=170 synthetic
 calibration (BASELINE config 3).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 3]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 3] [--dump-outputs DIR]
 
 A "step" is one complete solve of the problem from the same seed. Prints ONE JSON
 line (rank 0). See DESIGN.md "Measurement" for what every field means.
+--dump-outputs DIR writes what the last timed step computed as DIR/<name>.npy (float64);
+the inputs are seeded, so two builds can be compared output for output.
 
   value   iterations/s with the problem resident in HBM: Problem.reset() + Problem.optimize(),
           timed on the device with CUDA events inside the library (info.ms_total)
@@ -37,7 +39,7 @@ UNIT = "iterations/s"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -102,7 +104,7 @@ def describe(config, kw):
                 Nobservations_board=int(kw["observations_board"].shape[0]),
                 pixel_noise=0.3, seed="truth perturbed (mrcal_b200/synthetic.py, default_rng(0))",
                 l2="working set per iteration (Jacobian strips 146 MB x2 + per-item Gram blocks + panels) exceeds the "
-                   "126 MB L2; additionally a 256 MB buffer is written between timed steps")
+                   "50 MB L2 of an H100; additionally a 256 MB buffer is written between timed steps")
 
 
 def cpu_reference_run(kw, iterations):
@@ -188,6 +190,25 @@ def measure_fp64_peak():
     return 2.0 * n ** 3 / (best * 1e-3) / 1e12
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(outdir, sol, last):
+    """What a caller of the timed path receives after its last step: the state and residuals Problem.download()
+    returns (b_packed, x, the unpacked solution, the outlier flags in observations_board) and the solve's scalar
+    results, one float64 .npy per name."""
+    arrays = {k: np.ascontiguousarray(v, np.float64) for k, v in sol.items() if isinstance(v, np.ndarray) and v.size}
+    for k in ("rms_reproj_error__pixels", "Niterations", "Noutliers_board", "Noutliers_triangulated_point",
+              "norm2_x_initial", "norm2_x_final"):
+        arrays[k] = np.array([last[k]], np.float64)
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise RuntimeError(f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT_BYTES} byte limit")
+    os.makedirs(outdir, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(outdir, k + ".npy"), a)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -200,6 +221,8 @@ def main():
     ap.add_argument("--profile", action="store_true",
                     help="run under a profiler: only the device-resident steps (no e2e leg, no CPU baseline, no DGEMM peak "
                          "measurement); the numbers printed are not bench values")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="after the timed steps, write the outputs of the last one as DIR/<name>.npy (rank 0)")
     ap.add_argument("--max-iterations", type=int, default=300,
                     help="cap on trust-region iterations per solve (300 = the reference's; smaller only for profiling runs)")
     args = ap.parse_args()
@@ -280,6 +303,8 @@ def main():
         infos.append(one_step())
     barrier()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, P.download(into_inputs=False), infos[-1])
 
     ms = np.array([i["ms_total"] for i in infos])
     its = np.array([i["Niterations"] for i in infos])
@@ -361,14 +386,6 @@ def main():
         return 0
 
     ###### roofline of the dominant kernel family
-    # DRAM traffic per launch of the kernels named below, from the committed ncu capture (null if absent)
-    traffic = {}
-    for name in ("r02_dram_traffic.json", "r01c_dram_traffic.json"):
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", name)))
-            break
-        except Exception:
-            pass
     last = infos[-1]
     n_c = last["Nreduced"]
     roofline = None
@@ -379,7 +396,6 @@ def main():
         achieved = flops / per_fact_s / 1e12
         roofline = {"bound": "tensor", "kernel": "reduced-system Cholesky: chol_spine_kernel (persistent, DMMA; chol_dataflow.cu)",
                     "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                    "traffic": traffic.get("chol_spine_kernel", traffic.get("chol_dataflow_kernel")), "traffic_unit": "bytes per launch (ncu dram read+write)",
                     "flops_per_launch": flops, "n_reduced": n_c,
                     "peak_source": "cuBLAS DGEMM 8192^3 (torch.matmul fp64) measured in this run: MEASURED_PEAKS.json has no fp64 entry"}
     except Exception as e:   # pragma: no cover
@@ -389,13 +405,13 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         hbm = peaks["hbm_gbs"]; hbm_src = "MEASURED_PEAKS.json hbm_gbs (of measured)"
     except Exception:
-        hbm = 6650.0; hbm_src = "fallback 6.65 TB/s (of fallback)"
+        hbm = 3350.0; hbm_src = "H100 SXM data sheet 3.35 TB/s (not measured)"
     ms_cb = P.time_callback(20, True)
     ncorners = kw_local["observations_board"].shape[0] * kw_local["observations_board"].shape[1] * kw_local["observations_board"].shape[2]
     bytes_cb = 24 * ncorners + 8 * P.Nstate + 8 * P.Nmeasurements + 12 * P.N_j_nonzero + 4 * (P.Nmeasurements + 1)
     fill = {"bound": "hbm", "kernel": "eval_boards_kernel (residual + Jacobian fill)", "achieved": bytes_cb / (ms_cb * 1e-3) / 1e9,
             "peak": hbm, "unit": "GB/s", "frac": bytes_cb / (ms_cb * 1e-3) / 1e9 / hbm, "bytes_per_launch": bytes_cb,
-            "ms_per_launch": ms_cb, "peak_source": hbm_src, "traffic": traffic.get("eval_boards_kernel")}
+            "ms_per_launch": ms_cb, "peak_source": hbm_src}
 
     # the assembly + Schur phase (SURVEY.md 8d): flops = sum_rows nnz(nnz+1) [JtJ] + sum_groups 6 k(k+1) [Schur, k = shared unknowns the
     # group touches]; bytes = the Jacobian read once (12 B per nonzero) + the residuals. Both rooflines are given; the phase is
@@ -427,10 +443,7 @@ def main():
                     "achieved": (bytes_asm / per_asm_s / 1e9) if bound == "hbm" else (flops_asm / per_asm_s / 1e12),
                     "peak": hbm if bound == "hbm" else roofline["peak"], "unit": "GB/s" if bound == "hbm" else "TFLOP/s",
                     "frac": (t_bytes if bound == "hbm" else t_flops) / per_asm_s,
-                    "frac_hbm": t_bytes / per_asm_s, "frac_fp64_tensor": (t_flops / per_asm_s) if t_flops else None,
-                    "traffic": (sum(traffic[k] for k in ("fused_boards_kernel", "groups_panels_kernel", "schur_tiles_kernel") if k in traffic)
-                                if "schur_tiles_kernel" in traffic else None),
-                    "traffic_note": "ncu dram read+write per launch: fused_boards_kernel + groups_panels_kernel + schur_tiles_kernel"}
+                    "frac_hbm": t_bytes / per_asm_s, "frac_fp64_tensor": (t_flops / per_asm_s) if t_flops else None}
     except Exception as e:   # pragma: no cover
         assembly = {"error": str(e)}
 

@@ -1,4 +1,4 @@
-// mrcal_b200: C-ABI of the B200-native implementation of mrcal's calibration
+// mrcal_b200: C-ABI of the H100-native implementation of mrcal's calibration
 // solve (the optimizer_callback residual/Jacobian evaluator and the
 // trust-region normal-equations solve).
 //
@@ -376,7 +376,7 @@ mrcal_stats_t mrcal_optimize(double* b_packed_final, int buffer_size_b_packed_fi
 ////////////////////////////////////////////////////////////////////////////////
 
 // Version / build introspection. The string names the arch the kernels were
-// compiled for ("sm_100a")
+// compiled for ("sm_90a")
 const char* mrcal_b200_version(void);
 // Number of usable CUDA devices; 0 (never an error) when there is no GPU
 int mrcal_b200_device_count(void);

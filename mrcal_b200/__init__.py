@@ -1,4 +1,4 @@
-"""mrcal_b200: a B200-native (sm_100a CUDA) implementation of mrcal's
+"""mrcal_b200: an H100-native (sm_90a CUDA) implementation of mrcal's
 calibration solve -- the optimizer_callback residual/Jacobian evaluator and the
 trust-region normal-equations solve -- behind mrcal's own Python API for that
 path. See DESIGN.md and INTEGRATION.md at the repository root."""

@@ -10,7 +10,7 @@ keyword arguments, return values and error behaviour (mrcal-pywrap.c:890-937,
     lensmodel_num_params(), lensmodel_metadata_and_config(),
     knots_for_splined_models(), supported_lensmodels(), CHOLMOD_factorization
 
-Everything numeric happens in libmrcal_b200.so (CUDA, sm_100a). This module only
+Everything numeric happens in libmrcal_b200.so (CUDA, sm_90a). This module only
 marshals arguments, the way mrcal-pywrap.c does for the reference.
 """
 import ctypes as C

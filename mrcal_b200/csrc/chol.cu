@@ -257,7 +257,7 @@ static bool syrk_update(double* A, int ld, int n, int c0, int c1, int k0, int k1
     if(c1 <= c0 || n <= c0) return true;
     // big tiles when they fill the chip twice over, small tiles otherwise
     const long nt128 = (long)((c1 - c0 + 127) / 128) * ((n - c0 + 127) / 128);
-    if(nt128 >= 2 * 148)
+    if(nt128 >= 2L * device_sm_count())
     {
         dim3 grid((c1 - c0 + 127) / 128, (n - c0 + 127) / 128);
         syrk_dmma_kernel<128><<<grid, 256, kSyrkSmem, s>>>(A, ld, n, c0, c1, k0, k1);

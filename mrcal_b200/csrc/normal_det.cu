@@ -360,8 +360,8 @@ tile_plan_kernel(NormalBuffers N, int nblk, int ns_per_item, int ns_per_group, i
             n_groups += cnt;
         }
     }
-    // what the tile costs one CTA (measured: ~1 us per item of phase A, ~0.27 us per group of phase S), cut into parts of
-    // ns_per_part each: the kernel ends when its longest CTA does
+    // what the tile costs one CTA (a cost model: ns_per_item per item of phase A, ns_per_group per group of phase S), cut
+    // into parts of ns_per_part each: the kernel ends when its longest CTA does
     const long cost = (long)n_items * ns_per_item + (long)n_groups * ns_per_group;
     int parts = (int)((cost + ns_per_part - 1) / ns_per_part);
     parts = min(kMaxParts, max(1, parts));
@@ -623,8 +623,8 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
         fence_proxy_async();
         __syncthreads();
         // rows 6 i .. 6 i + 5 of the K panel <- group i of the chunk: ONE bulk copy (TMA) per group and side -- the panels
-        // are contiguous in Ypan and carry the row padding of the shared-memory layout; a bulk copy has a fixed cost of
-        // some 45 cycles in the copy engine, whatever its size -- issued by one thread each, all counted on the buffer's
+        // are contiguous in Ypan and carry the row padding of the shared-memory layout; a bulk copy has a fixed cost in the
+        // copy engine, whatever its size -- issued by one thread each, all counted on the buffer's
         // mbarrier. No thread spends instructions on moving the data
         static_assert(kYld == TLD, "the panels of Ypan are copied as they are");
         const int sides = diag ? 1 : 2;

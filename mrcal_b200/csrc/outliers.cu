@@ -25,7 +25,10 @@ bool comm_active();
 bool comm_allreduce_sum(double* d_buf, size_t count, cudaStream_t s);
 
 constexpr double kOutlierK0 = 4.0, kOutlierK1 = 5.0;
-constexpr int kOutlierBlocks = 592;   // 4 x 148
+// Fixed, not derived from the SM count: the number of partial sums sets the order of the additions, and so
+// the bits of the result, which must not depend on the device. 592 blocks of 256 threads are resident at once
+// on a 132-SM H100 (8 per SM), so the count costs no second wave
+constexpr int kOutlierBlocks = 592;
 
 // acc layout (doubles)
 enum { OA_SUMSQ = 0, OA_NINL_B, OA_NOUT_B, OA_NINL_T, OA_NOUT_T, OA_FOUND, OA_NEW_B, OA_NEW_T, OA_N };

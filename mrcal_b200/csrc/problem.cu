@@ -63,6 +63,19 @@ static bool pack_seed_host(mrcal_b200_problem* P, std::vector<double>* b,
     return true;
 }
 
+int device_sm_count()
+{
+    static int cached[kMaxDevices] = {};
+    int dev = 0;
+    if(cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) { cudaGetLastError(); return 0; }
+    if(cached[dev] == 0 && cudaDeviceGetAttribute(&cached[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    {
+        cudaGetLastError();
+        cached[dev] = 0;
+    }
+    return cached[dev];
+}
+
 bool problem_evaluate(mrcal_b200_problem* P, int which, bool with_jacobian, bool with_rowptr)
 {
     return launch_evaluate(P->dp, P->op[which], with_jacobian, with_rowptr ? P->d_rowptr : nullptr, P->stream, &P->launches);
@@ -72,7 +85,7 @@ bool problem_evaluate(mrcal_b200_problem* P, int which, bool with_jacobian, bool
 
 using namespace mb200;
 
-extern "C" const char* mrcal_b200_version(void) { return "mrcal_b200 0.1 (sm_100a)"; }
+extern "C" const char* mrcal_b200_version(void) { return "mrcal_b200 0.1 (sm_90a)"; }
 extern "C" const char* mrcal_b200_last_error(void) { return get_error(); }
 extern "C" int mrcal_b200_device_count(void)
 {

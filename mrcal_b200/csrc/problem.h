@@ -19,6 +19,9 @@ namespace mb200 {
 
 constexpr int kMaxDevices = 64;   // per-device one-time kernel configuration flags
 
+// SMs of the current device (cached per device); 0 if it cannot be queried
+int device_sm_count();
+
 // Read-only description handed to every kernel BY VALUE (lives in the constant
 // bank; ~300 bytes). All pointers are device pointers.
 struct DevProblem

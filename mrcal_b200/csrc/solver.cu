@@ -279,7 +279,7 @@ static bool count_negative_weights(mrcal_b200_problem* P, int* count)
     const long n = (long)L.d.Nobs_board * L.d.W * L.d.H;
     int* d_cnt = ws->N.stat + 2;
     MB200_CUDA_CHECK(cudaMemsetAsync(d_cnt, 0, sizeof(int), P->stream));
-    count_negative_kernel<<<296, 256, 0, P->stream>>>(P->d_pool_board, n, d_cnt);
+    count_negative_kernel<<<2 * std::max(1, device_sm_count()), 256, 0, P->stream>>>(P->d_pool_board, n, d_cnt);
     P->launches++;
     MB200_CUDA_CHECK(cudaMemcpyAsync(ws->h_info + 2, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, P->stream));
     MB200_CUDA_CHECK(cudaStreamSynchronize(P->stream));
@@ -607,7 +607,7 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
             // nothing of them: they run on a second stream, UNDER the factorization (whose spine leaves the machine mostly
             // idle). The price: whether the Cauchy point already leaves the trust region -- and the Gauss-Newton step is
             // unnecessary -- is only known afterwards, so every new operating point is factored; the rare unnecessary
-            // factorization (the first few steps of a solve) costs less than ~50 us on the critical path of every step
+            // factorization (the first few steps of a solve) costs less than those sums on the critical path of every step
             const bool overlap = N.s_side[0] != nullptr && getenv("MRCAL_B200_NO_OVERLAP") == nullptr;
             if(!have_cauchy)
             {
@@ -620,15 +620,16 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
                     MB200_CUDA_CHECK(cudaStreamWaitEvent(sc, N.ev_fork, 0));
                 }
                 dots_kernel<<<3, 1024, 0, sc>>>(N.g_full, nullptr, e0, e1, Nstate, ws->scal + 0);
+                const int nsm = std::max(1, device_sm_count());
                 if(N.fused)
                 {
                     // |J g|^2: the board rows from the observations' blocks, the others from their stored rows
                     if(!launch_quadform_boards(P->dp, N, N.g_full, N.qf_part, ws->scal + 10, sc, nl)) return false;
                     if(Nrows_mine > P->dp.m_point0)
-                        jv_kernel<<<148 * 4, 256, 0, sc>>>(P->d_rowptr, cur.Jcol, cur.Jval, N.g_full, cur.x, P->dp.m_point0, Nrows_mine, ws->scal + 9);
+                        jv_kernel<<<nsm * 4, 256, 0, sc>>>(P->d_rowptr, cur.Jcol, cur.Jval, N.g_full, cur.x, P->dp.m_point0, Nrows_mine, ws->scal + 9);
                 }
                 else
-                    jv_kernel<<<148 * 16, 256, 0, sc>>>(P->d_rowptr, cur.Jcol, cur.Jval, N.g_full, cur.x, 0, Nrows_mine, ws->scal + 9);
+                    jv_kernel<<<nsm * 16, 256, 0, sc>>>(P->d_rowptr, cur.Jcol, cur.Jval, N.g_full, cur.x, 0, Nrows_mine, ws->scal + 9);
                 *nl += 2;
                 if(overlap) MB200_CUDA_CHECK(cudaEventRecord(N.ev_join[0], sc));
                 // eliminated-range dots and the row sums are per-rank partial sums. Sharded: they wait for the partial sums

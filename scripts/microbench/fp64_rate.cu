@@ -1,5 +1,5 @@
 // Microbenchmark: sustained FP64 throughput of the vector pipe (DFMA) and of the
-// tensor pipe (DMMA.8x8x4) on this GPU. Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o fp64_rate fp64_rate.cu
+// tensor pipe (DMMA.8x8x4) on this GPU. Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_rate fp64_rate.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

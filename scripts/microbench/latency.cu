@@ -1,5 +1,5 @@
 // Dependent-issue latencies (SM cycles) of the instructions on the pivot chain of potrf_block.cuh.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/latency latency.cu && /tmp/latency
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o latency latency.cu && ./latency
 #include <cstdio>
 #include <cuda_runtime.h>
 constexpr int N = 512;

@@ -10,13 +10,13 @@ sys.path.insert(0, os.path.dirname(__file__))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 @pytest.fixture(scope="session")
 def ref():
-    """The compiled reference (oracle/_ref). Built in the dev container; travels to the GPU box."""
+    """The compiled reference (oracle/_ref), built by build() where the reference tree is readable."""
     from oracle import ref as _ref
     if not _ref.available():
-        pytest.skip("oracle/_ref/libmrcal_ref.so not built (needs /root/reference: make -C oracle ref)")
+        pytest.skip("oracle/_ref/libmrcal_ref.so not built (needs the reference tree: make -C oracle ref)")
     return _ref
