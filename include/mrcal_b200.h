@@ -528,6 +528,19 @@ int mrcal_b200_problem_triangulated_outliers(mrcal_b200_problem_t* problem, int*
    the reference refuses (uncertainty.c:944-989). */
 bool mrcal_b200_problem_drt_cross_reprojection__dbpacked(mrcal_b200_problem_t* problem, int icam_intrinsics, double* K /* [6][Nstate] */);
 
+/* Projection uncertainty, as mrcal.projection_uncertainty(what='covariance') computes it (mrcal/model_analysis.py:1192-1517):
+   Var(q) [N][2][2] of the projections of the camera-frame points p_cam [N] by camera icam_intrinsics, propagated from
+   the noise of the pixel observations through the solve, at the problem's current state. method: one of the enum
+   below (the reference's 'mean-pcam', 'cross-reprojection-rrp-Jfp', 'cross-reprojection-ccp'). atinfinity: the
+   points are directions; only the rotations propagate. observed_pixel_uncertainty <= 0: estimated from the residuals
+   (model_analysis.py:491-556); the value used is returned in *sigma_used (may be NULL). Evaluation, factorization,
+   the dF/db rows, the solves and the reductions all run on the device; only Var comes back. Refuses what the
+   reference refuses, and sharded problems. False + mrcal_b200_last_error() on refusal or failure */
+enum { MRCAL_B200_UNCERTAINTY_MEAN_PCAM = 0, MRCAL_B200_UNCERTAINTY_RRP_JFP, MRCAL_B200_UNCERTAINTY_CCP };
+bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* problem, int icam_intrinsics, int method,
+                                               bool atinfinity, const mrcal_point3_t* p_cam, int N,
+                                               double observed_pixel_uncertainty, double* Var, double* sigma_used);
+
 // Timing hook for benchmarks: run N cost-function evaluations (residuals +
 // Jacobian) at the current state back to back, return the mean device time per
 // evaluation in milliseconds (CUDA events on the library's stream); <0 on error

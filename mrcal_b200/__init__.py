@@ -3,7 +3,8 @@ calibration solve -- the optimizer_callback residual/Jacobian evaluator and the
 trust-region normal-equations solve -- behind mrcal's own Python API for that
 path. See DESIGN.md and INTEGRATION.md at the repository root."""
 from .api import (  # noqa: F401
-    optimize, optimizer_callback, drt_cross_reprojection__dbpacked, Problem, CHOLMOD_factorization,
+    optimize, optimizer_callback, drt_cross_reprojection__dbpacked, projection_uncertainty, worst_direction_stdev,
+    Problem, CHOLMOD_factorization,
     lensmodel_num_params, supported_lensmodels, lensmodel_metadata_and_config, knots_for_splined_models,
     state_index_intrinsics, state_index_extrinsics, state_index_frames, state_index_points,
     state_index_calobject_warp,

@@ -328,6 +328,51 @@ def drt_cross_reprojection__dbpacked(icam_intrinsics=-1, **kwargs):
         P.close()
 
 
+_UNCERTAINTY_METHODS = {"mean-pcam": 0, "cross-reprojection-rrp-Jfp": 1, "cross-reprojection-ccp": 2}   # mrcal_b200.h
+
+
+def worst_direction_stdev(cov):
+    """sqrt of the larger eigenvalue of each 2x2 covariance (..., 2, 2), in closed form"""
+    cov = np.asarray(cov, np.float64)
+    a, b, c = cov[..., 0, 0], cov[..., 0, 1], cov[..., 1, 1]
+    return np.sqrt((a + c) / 2. + np.sqrt(((a - c) / 2.) ** 2 + b * b))
+
+
+def projection_uncertainty(p_cam, model, *, method="cross-reprojection-ccp", atinfinity=False, what="covariance",
+                           observed_pixel_uncertainty=None):
+    """The uncertainty of the projection of the camera-frame points p_cam (..., 3) by the camera of `model`, propagated
+    from the noise of the calibration's pixel observations, as mrcal.projection_uncertainty() computes it
+    (mrcal/model_analysis.py:1192-1517). The model must carry optimization_inputs; its own (possibly edited)
+    extrinsics are not used. what='covariance' returns (..., 2, 2); 'worstdirection-stdev' and 'rms-stdev' return
+    (...). observed_pixel_uncertainty=None estimates it from the residuals at the solution."""
+    known_methods = set(_UNCERTAINTY_METHODS)
+    if method not in known_methods:
+        raise RuntimeError(f"Unknown uncertainty method: '{method}'. I know about {known_methods}")
+    what_known = {"covariance", "worstdirection-stdev", "rms-stdev"}
+    if what not in what_known:
+        raise RuntimeError(f"'what' kwarg must be in {what_known}, but got '{what}'")
+    icam_intrinsics = model.icam_intrinsics()
+    optimization_inputs = model.optimization_inputs()
+    if optimization_inputs is None:
+        raise RuntimeError("optimization_inputs are unavailable in this model. Uncertainty cannot be computed")
+    _require_gpu()
+    p = np.asarray(p_cam, np.float64)
+    if p.shape[-1:] != (3,):
+        raise RuntimeError(f"p_cam must have shape (...,3); got {p.shape}")
+    P = Problem(**optimization_inputs)
+    try:
+        Var, _ = P.projection_uncertainty(p.reshape(-1, 3), icam_intrinsics, method=method, atinfinity=atinfinity,
+                                          observed_pixel_uncertainty=observed_pixel_uncertainty)
+    finally:
+        P.close()
+    Var = Var.reshape(p.shape[:-1] + (2, 2))
+    if what == "covariance":
+        return Var
+    if what == "worstdirection-stdev":
+        return worst_direction_stdev(Var)
+    return np.sqrt((Var[..., 0, 0] + Var[..., 1, 1]) / 2.)
+
+
 def optimizer_callback(no_jacobian=False, no_factorization=False, **kwargs):
     """One evaluation of the cost function at the given seed.
 
@@ -514,6 +559,27 @@ class Problem:
         if not lib.mrcal_b200_problem_drt_cross_reprojection__dbpacked(self._h, int(icam_intrinsics), _ptr(K)):
             raise RuntimeError("_mrcal_drt_cross_reprojection__dbpacked() failed: " + _capi.last_error())
         return K
+
+    def projection_uncertainty(self, p_cam, icam_intrinsics, method="cross-reprojection-ccp", atinfinity=False,
+                               observed_pixel_uncertainty=None):
+        """(Var, sigma): the raw (N,2,2) covariances of the projections of the points p_cam (N,3) by camera
+        icam_intrinsics at the problem's current state, and the observed-pixel uncertainty used (estimated from the
+        residuals if None). Everything but the reshaping runs on the device (csrc/uncertainty.cu)"""
+        if method not in _UNCERTAINTY_METHODS:
+            raise RuntimeError(f"Unknown uncertainty method: '{method}'. I know about {set(_UNCERTAINTY_METHODS)}")
+        p = np.ascontiguousarray(p_cam, np.float64)
+        if p.ndim != 2 or p.shape[1] != 3:
+            raise RuntimeError(f"p_cam must have shape (N,3); got {p.shape}")
+        Var = np.zeros((p.shape[0], 2, 2))
+        sigma = C.c_double(0.)
+        s = -1.0 if observed_pixel_uncertainty is None else float(observed_pixel_uncertainty)
+        if observed_pixel_uncertainty is not None and not s > 0:
+            raise RuntimeError("observed_pixel_uncertainty must be > 0 (or None to estimate it)")
+        if not lib.mrcal_b200_problem_projection_uncertainty(self._h, int(icam_intrinsics), _UNCERTAINTY_METHODS[method],
+                                                            bool(atinfinity), _ptr(p), p.shape[0], s, _ptr(Var),
+                                                            C.byref(sigma)):
+            raise RuntimeError("projection_uncertainty: " + _capi.last_error())
+        return Var, sigma.value
 
     def callback(self, jacobian=True):
         b = np.zeros(self.Nstate)

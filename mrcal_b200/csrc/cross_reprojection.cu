@@ -283,12 +283,9 @@ __global__ void cross_solve_kernel(const double* __restrict__ JJ, double* __rest
 }
 
 }  // namespace
-}  // namespace mb200
-using namespace mb200;
 
-// K_out: [6][Nstate] (host), zero outside the extrinsics / frames / points / calobject_warp columns. The Jacobian is
-// evaluated at the problem's current state (as mrcal.drt_cross_reprojection__dbpacked() does, mrcal-pywrap.c:1931-1990)
-extern "C" bool mrcal_b200_problem_drt_cross_reprojection__dbpacked(mrcal_b200_problem_t* P, int icam_intrinsics, double* K_out)
+// K into d_K (device, [6][Nstate]), zero outside the extrinsics / frames / points / calobject_warp columns
+bool cross_reprojection_K(mrcal_b200_problem* P, int icam_intrinsics, bool evaluate, double* d_K)
 {
     const Layout& L = P->L;
     const DevProblem& dp = P->dp;
@@ -317,15 +314,17 @@ extern "C" bool mrcal_b200_problem_drt_cross_reprojection__dbpacked(mrcal_b200_p
     }
     if(dp.Ntri > 0) { set_error("drt_cross_reprojection__dbpacked: triangulated points are not supported (nor are they by the reference)"); return false; }
     cudaStream_t s = P->stream;
-    if(!problem_evaluate(P, P->cur, true, false)) return false;
+    if(evaluate && !problem_evaluate(P, P->cur, true, false)) return false;
     const int Nobs = dp.Nobs_board + dp.Nobs_point, Nstate = L.Nstate;
     if(Nobs == 0) { set_error("no observations"); return false; }
     DeviceArena tmp;
     ObsOut* obs = nullptr;
-    double *K = nullptr, *JJ = nullptr;
+    double* JJ = nullptr;
     int* info = nullptr;
-    if(!tmp.alloc(&obs, (size_t)Nobs) || !tmp.alloc(&K, (size_t)6 * Nstate, true) || !tmp.alloc(&JJ, 21, true) || !tmp.alloc(&info, 1, true))
+    if(!tmp.alloc(&obs, (size_t)Nobs) || !tmp.alloc(&JJ, 21, true) || !tmp.alloc(&info, 1, true))
         return false;
+    double* K = d_K;
+    MB200_CUDA_CHECK(cudaMemsetAsync(K, 0, (size_t)6 * Nstate * sizeof(double), s));
     const EvalBuffers& op = P->op[P->cur];
     cross_observations_kernel<<<(Nobs * 32 + 127) / 128, 128, 0, s>>>(dp, op.p, op.Jval, icam_intrinsics, obs);
     if(dp.i_extr0 >= 0 && dp.Ncam_e > 0 && icam_intrinsics >= 0)
@@ -346,8 +345,23 @@ extern "C" bool mrcal_b200_problem_drt_cross_reprojection__dbpacked(mrcal_b200_p
     int h_info = 0;
     MB200_CUDA_CHECK(cudaGetLastError());
     MB200_CUDA_CHECK(cudaMemcpyAsync(&h_info, info, sizeof(int), cudaMemcpyDeviceToHost, s));
-    MB200_CUDA_CHECK(cudaMemcpyAsync(K_out, K, (size_t)6 * Nstate * sizeof(double), cudaMemcpyDeviceToHost, s));
     MB200_CUDA_CHECK(cudaStreamSynchronize(s));
     if(h_info != 0) { set_error("Singular Jcross_t Jcross!"); return false; }
+    return true;
+}
+
+}  // namespace mb200
+using namespace mb200;
+
+// K_out: [6][Nstate] (host), zero outside the extrinsics / frames / points / calobject_warp columns. The Jacobian is
+// evaluated at the problem's current state (as mrcal.drt_cross_reprojection__dbpacked() does, mrcal-pywrap.c:1931-1990)
+extern "C" bool mrcal_b200_problem_drt_cross_reprojection__dbpacked(mrcal_b200_problem_t* P, int icam_intrinsics, double* K_out)
+{
+    DeviceArena tmp;
+    double* K = nullptr;
+    if(!tmp.alloc(&K, (size_t)6 * P->L.Nstate)) return false;
+    if(!cross_reprojection_K(P, icam_intrinsics, true, K)) return false;
+    MB200_CUDA_CHECK(cudaMemcpyAsync(K_out, K, (size_t)6 * P->L.Nstate * sizeof(double), cudaMemcpyDeviceToHost, P->stream));
+    MB200_CUDA_CHECK(cudaStreamSynchronize(P->stream));
     return true;
 }

@@ -132,22 +132,30 @@ __global__ void csr_mtm_final_kernel(const double* __restrict__ partial, int Nx,
     out[e] = s;
 }
 
+// The stable transpose (CSC) of a device CSR matrix: column c's entries in row order at [tp[c], tp[c+1]), with their
+// positions in the CSR arrays (tsrc) and their rows (trow). The arrays are allocated from `arena`
+bool csr_stable_transpose(const int* p, const int* col, int Nrows, int nnz, int Ncols, DeviceArena& arena,
+                          int** tp, int** tsrc, int** trow, cudaStream_t s)
+{
+    DeviceArena tmp;
+    int *rows = nullptr, *hist = nullptr;
+    if(!arena.alloc(tp, (size_t)Ncols + 1, true) || !arena.alloc(tsrc, nnz) || !arena.alloc(trow, nnz) ||
+       !tmp.alloc(&rows, nnz) || !tmp.alloc(&hist, (size_t)kTChunks * Ncols, true))
+        return false;
+    if(Nrows > 0) csr_expand_rows_kernel<<<(Nrows + 255) / 256, 256, 0, s>>>(p, Nrows, rows);
+    csr_chunk_hist_kernel<<<(kTChunks + 127) / 128, 128, 0, s>>>(col, nnz, Ncols, hist);
+    csr_chunk_scan_kernel<<<(Ncols + 127) / 128, 128, 0, s>>>(Ncols, hist, *tp);
+    csr_colptr_scan_kernel<<<1, 32, 0, s>>>(Ncols, *tp);
+    csr_chunk_fill_kernel<<<(kTChunks + 127) / 128, 128, 0, s>>>(col, rows, nnz, Ncols, hist, *tp, *tsrc, *trow);
+    MB200_CUDA_CHECK(cudaGetLastError());
+    MB200_CUDA_CHECK(cudaStreamSynchronize(s));   // tmp goes out of scope
+    return true;
+}
+
 static bool build_transpose(mrcal_b200_csr* J)
 {
     if(J->have_t) return true;
-    cudaStream_t s = J->stream;
-    DeviceArena tmp;
-    int *rows = nullptr, *hist = nullptr;
-    if(!J->arena.alloc(&J->tp, (size_t)J->Ncols + 1, true) || !J->arena.alloc(&J->tsrc, J->nnz) || !J->arena.alloc(&J->trow, J->nnz) ||
-       !tmp.alloc(&rows, J->nnz) || !tmp.alloc(&hist, (size_t)kTChunks * J->Ncols, true))
-        return false;
-    if(J->Nrows > 0) csr_expand_rows_kernel<<<(J->Nrows + 255) / 256, 256, 0, s>>>(J->p, J->Nrows, rows);
-    csr_chunk_hist_kernel<<<(kTChunks + 127) / 128, 128, 0, s>>>(J->i, J->nnz, J->Ncols, hist);
-    csr_chunk_scan_kernel<<<(J->Ncols + 127) / 128, 128, 0, s>>>(J->Ncols, hist, J->tp);
-    csr_colptr_scan_kernel<<<1, 32, 0, s>>>(J->Ncols, J->tp);
-    csr_chunk_fill_kernel<<<(kTChunks + 127) / 128, 128, 0, s>>>(J->i, rows, J->nnz, J->Ncols, hist, J->tp, J->tsrc, J->trow);
-    MB200_CUDA_CHECK(cudaGetLastError());
-    MB200_CUDA_CHECK(cudaStreamSynchronize(s));   // tmp goes out of scope
+    if(!csr_stable_transpose(J->p, J->i, J->Nrows, J->nnz, J->Ncols, J->arena, &J->tp, &J->tsrc, &J->trow, J->stream)) return false;
     J->have_t = true;
     return true;
 }

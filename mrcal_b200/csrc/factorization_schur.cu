@@ -354,6 +354,62 @@ __global__ void rank_inactive_kernel(NormalBuffers N, int* __restrict__ ia_rank)
     for(int r = 0; r < N.n_r; r++) ia_rank[r] = N.cidx[r] < 0 ? k++ : -1;
 }
 
+// Builds the structured factor of P at its current state into F (F->P is set by the caller; F does not own P here).
+// False, with the reason in the error string, if P is sharded or JtJ is not positive definite. The device problem's
+// solver workspace holds L_S and the panels afterwards (they are what the next solver iteration overwrites)
+bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F, bool* other_path)
+{
+    if(other_path) *other_path = false;
+    if(comm_active() || P->sharded) { set_error("structured factorization: not available for sharded problems"); return false; }
+    if(!solver_build_workspace(P)) return false;
+    SolverWorkspace* ws = P->ws.get();
+    NormalBuffers& N = ws->N;
+    cudaStream_t s = P->stream;
+    int nl = 0;
+    if(!problem_evaluate(P, P->cur, true, true) ||
+       !normal_assemble(P->dp, N, P->op[P->cur], P->d_rowptr, 0., s, &nl)) return false;
+    if(!N.det)
+    {
+        if(other_path) *other_path = true;
+        set_error("structured factorization: this problem takes the other assembly path");
+        return false;
+    }
+    int h_info[2] = {0, 0}, h_bad = 0;
+    if(N.n_c > 0 && !chol_factor(N.S, N.ldS, N.n_c, ws->invL, N.info + 1, s, &nl, &ws->chol)) return false;
+    clear_aug_rows_kernel<<<(N.ldS + 255) / 256, 256, 0, s>>>(N, N.n_c, ws->invL);
+    int* d_bad = nullptr;
+    F->arena.release();
+    if(!F->arena.alloc(&F->ia_L, 3 * (size_t)(N.n_r > 0 ? N.n_r : 1), true) || !F->arena.alloc(&F->ia_first, 2 * (size_t)(N.n_r > 0 ? N.n_r : 1), true) ||
+       !F->arena.alloc(&F->minmax, 2) || !F->arena.alloc(&d_bad, 1, true)) return false;
+    if(N.n_r > 0)
+    {
+        inactive_blocks_kernel<<<(N.n_r + 255) / 256, 256, 0, s>>>(P->dp, N, P->op[P->cur].Jval, F->ia_L, F->ia_first, d_bad);
+        rank_inactive_kernel<<<1, 32, 0, s>>>(N, F->ia_first + N.n_r);
+    }
+    if(cudaMemcpyAsync(h_info, N.info, sizeof(h_info), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+       cudaMemcpyAsync(&h_bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
+       cudaStreamSynchronize(s) != cudaSuccess)
+    { set_error("structured factorization: device failure"); return false; }
+    if(h_info[0] != 0 || h_info[1] != 0 || h_bad != 0) { set_error("JtJ is not positive definite"); return false; }
+    F->n = P->L.Nstate;
+    F->Nelim = N.e1 - N.e0;
+    return true;
+}
+
+// L_D z = b / L_D' x = z and L_I z = b / L_I' x = z on pieces laid out as schur_factorization_solve() lays them out
+void schur_groups_tri(const mrcal_b200_factorization* F, double* Bf, int Nrhs, bool forward, cudaStream_t s)
+{
+    const NormalBuffers& N = F->P->ws->N;
+    const long gr = (long)Nrhs * N.Ngroups;
+    if(gr > 0) groups_tri_kernel<<<(unsigned)((gr + 127) / 128), 128, 0, s>>>(N, Bf, F->Nelim, Nrhs, forward);
+}
+void schur_inactive_tri(const mrcal_b200_factorization* F, double* Bi, int Nrhs, bool forward, cudaStream_t s)
+{
+    const NormalBuffers& N = F->P->ws->N;
+    const long ir = (long)Nrhs * N.n_r;
+    if(N.n_r > N.n_c) inactive_tri_kernel<<<(unsigned)((ir + 255) / 256), 256, 0, s>>>(N, F->ia_L, F->ia_first, Bi, Nrhs, forward);
+}
+
 }  // namespace mb200
 using namespace mb200;
 
@@ -366,38 +422,12 @@ extern "C" mrcal_b200_factorization_t* mrcal_b200_factorization_create_from_last
     if(P == nullptr) { set_error("no mrcal_optimizer_callback() problem to factor"); return nullptr; }
     std::unique_ptr<mrcal_b200_factorization> F(new mrcal_b200_factorization());
     F->P = P;
-    auto fail = [&](const char* why) -> mrcal_b200_factorization_t*
+    if(!schur_factor_build(P, F.get()))
     {
-        set_error("%s", why);
+        const std::string why = get_error();
         schur_factorization_release(F.get());
+        set_error("%s", why.c_str());
         return nullptr;
-    };
-    if(comm_active() || P->sharded) return fail("structured factorization: not available for sharded problems");
-    if(!solver_build_workspace(P)) { schur_factorization_release(F.get()); return nullptr; }
-    SolverWorkspace* ws = P->ws.get();
-    NormalBuffers& N = ws->N;
-    cudaStream_t s = P->stream;
-    int nl = 0;
-    if(!problem_evaluate(P, P->cur, true, true) ||
-       !normal_assemble(P->dp, N, P->op[P->cur], P->d_rowptr, 0., s, &nl)) { schur_factorization_release(F.get()); return nullptr; }
-    if(!N.det) return fail("structured factorization: this problem takes the other assembly path");
-    int h_info[2] = {0, 0}, h_bad = 0;
-    if(N.n_c > 0 && !chol_factor(N.S, N.ldS, N.n_c, ws->invL, N.info + 1, s, &nl, &ws->chol)) { schur_factorization_release(F.get()); return nullptr; }
-    clear_aug_rows_kernel<<<(N.ldS + 255) / 256, 256, 0, s>>>(N, N.n_c, ws->invL);
-    int* d_bad = nullptr;
-    if(!F->arena.alloc(&F->ia_L, 3 * (size_t)(N.n_r > 0 ? N.n_r : 1), true) || !F->arena.alloc(&F->ia_first, 2 * (size_t)(N.n_r > 0 ? N.n_r : 1), true) ||
-       !F->arena.alloc(&F->minmax, 2) || !F->arena.alloc(&d_bad, 1, true)) { schur_factorization_release(F.get()); return nullptr; }
-    if(N.n_r > 0)
-    {
-        inactive_blocks_kernel<<<(N.n_r + 255) / 256, 256, 0, s>>>(P->dp, N, P->op[P->cur].Jval, F->ia_L, F->ia_first, d_bad);
-        rank_inactive_kernel<<<1, 32, 0, s>>>(N, F->ia_first + N.n_r);
     }
-    if(cudaMemcpyAsync(h_info, N.info, sizeof(h_info), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-       cudaMemcpyAsync(&h_bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, s) != cudaSuccess ||
-       cudaStreamSynchronize(s) != cudaSuccess)
-        return fail("structured factorization: device failure");
-    if(h_info[0] != 0 || h_info[1] != 0 || h_bad != 0) return fail("JtJ is not positive definite");
-    F->n = P->L.Nstate;
-    F->Nelim = N.e1 - N.e0;
     return F.release();
 }

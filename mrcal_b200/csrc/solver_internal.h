@@ -67,4 +67,14 @@ namespace mb200 {
 bool schur_factorization_solve(mrcal_b200_factorization* F, double* out, const double* bt, int Nrhs, int sys);
 double schur_factorization_rcond(mrcal_b200_factorization* F);
 void schur_factorization_release(mrcal_b200_factorization* F);
+// other_path (may be NULL): set when the failure is that this problem's reduced system is assembled without the panels
+bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F, bool* other_path = nullptr);
+// csr_ops.cu
+bool csr_stable_transpose(const int* p, const int* col, int Nrows, int nnz, int Ncols, DeviceArena& arena,
+                          int** tp, int** tsrc, int** trow, cudaStream_t s);
+void schur_groups_tri(const mrcal_b200_factorization* F, double* Bf, int Nrhs, bool forward, cudaStream_t s);
+void schur_inactive_tri(const mrcal_b200_factorization* F, double* Bi, int Nrhs, bool forward, cudaStream_t s);
+// cross_reprojection.cu: K = drt/db_packed (6 x Nstate, row-major) into device memory; evaluate: evaluate the
+// Jacobian at the current state first (false: the caller just did)
+bool cross_reprojection_K(mrcal_b200_problem* P, int icam_intrinsics, bool evaluate, double* d_K);
 }  // namespace mb200
