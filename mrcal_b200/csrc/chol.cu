@@ -230,6 +230,28 @@ syrk_dmma_kernel(double* __restrict__ A, int ld, int n, int c0, int c1, int k0, 
     }
 }
 
+__global__ void fill_words_kernel(WordFill f)
+{
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
+    for(int k = 0; k < f.count; k++)
+    {
+        unsigned* p = f.p[k];
+        const unsigned v = f.v[k];
+        for(long long i = t; i < f.n[k]; i += stride) p[i] = v;
+    }
+}
+
+bool fill_words(const WordFill& f, cudaStream_t s)
+{
+    if(f.count == 0) return true;
+    long long widest = 0;
+    for(int k = 0; k < f.count; k++) widest = f.n[k] > widest ? f.n[k] : widest;
+    const long long blocks = (widest + 255) / 256;
+    fill_words_kernel<<<(unsigned)(blocks < 1 ? 1 : (blocks > 512 ? 512 : blocks)), 256, 0, s>>>(f);
+    MB200_CUDA_CHECK(cudaGetLastError());
+    return true;
+}
+
 static const size_t kSyrkSmem = (size_t)2 * STAGES * BM * LDS * sizeof(double);   // TILE = 128; half of it for TILE = 64
 static const size_t kBlockSmem = (size_t)2 * NB * (NB + 1) * sizeof(double);   // trsm
 static const size_t kPotrfSmem = sizeof(PotrfSmem);

@@ -7,6 +7,23 @@ namespace mb200 {
 constexpr int kCholBlock = 64;
 inline int chol_padded(int n) { return ((n + kCholBlock - 1) / kCholBlock) * kCholBlock; }
 
+// Up to 8 device ranges of 32-bit words, each set to one value, in ONE launch (fill_words, chol.cu). The trust-region
+// step clears its flags, counters and accumulators a few words at a time; one cudaMemsetAsync per buffer costs a launch
+// gap each on the step's critical path
+struct WordFill
+{
+    unsigned* p[8];
+    long long n[8];
+    unsigned v[8];
+    int count = 0;
+    void add(void* ptr, size_t bytes, unsigned value = 0u)
+    {
+        if(bytes == 0) return;
+        p[count] = (unsigned*)ptr; n[count] = (long long)(bytes / 4); v[count] = value; count++;
+    }
+};
+bool fill_words(const WordFill& f, cudaStream_t s);
+
 // Scratch of the persistent kernels (tile flags, the solution slots of the backward substitution): one per
 // owner of a factorization, so that two factorizations in flight never share flags
 struct CholScratch { int* flags = nullptr; double* xbuf = nullptr; };

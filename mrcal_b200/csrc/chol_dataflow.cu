@@ -659,17 +659,20 @@ bool chol_factor_dataflow(double* A, int npad, int nreal, double* invL, int* d_i
     if(!cfg || !sc) { set_error("the persistent Cholesky kernel is not available on this device"); return false; }
     int nb = npad / T;
     const int ntiles = 1 + (nb - 1) * nb / 2;   // tasks: see the kernel
-    MB200_CUDA_CHECK(cudaMemsetAsync(d_info, 0, sizeof(int), s));
-    MB200_CUDA_CHECK(cudaMemsetAsync(sc->flags, 0, (size_t)(nb * (nb + 1) / 2) * sizeof(int), s));   // one flag per tile of the lower triangle
-    MB200_CUDA_CHECK(cudaMemsetAsync(sc->flags + kMaxTiles, 0, sizeof(int), s));
     int ld = npad;
     int* flags = sc->flags;
     int* abort_flag = sc->flags + kMaxTiles;
     static const bool no_spine = getenv("MRCAL_B200_CHOL_NO_SPINE") != nullptr;
-    if(!no_spine && nb >= 3 && cfg->num_sms >= 2)
+    const bool spine = !no_spine && nb >= 3 && cfg->num_sms >= 2;
+    // d_info, one flag per tile of the lower triangle, the abort flag and (spine) the spine's nb counters behind it
+    WordFill clear;
+    clear.add(d_info, sizeof(int));
+    clear.add(sc->flags, (size_t)(nb * (nb + 1) / 2) * sizeof(int));
+    clear.add(abort_flag, (size_t)(1 + (spine ? nb : 0)) * sizeof(int));
+    if(!fill_words(clear, s)) return false;
+    if(spine)
     {
         int* pre = sc->flags + kMaxTiles + 1;
-        MB200_CUDA_CHECK(cudaMemsetAsync(pre, 0, (size_t)nb * sizeof(int), s));
         long long* stamps = g_debug_stamps;
         void* args[] = {&A, &ld, &nb, &nreal, &invL, &d_info, &flags, &pre, &abort_flag, &d_run_if, &stamps};
         const int nhelper_tasks = (nb - 1) * nb / 2 - 1;
@@ -692,9 +695,11 @@ bool chol_solve_backward_dataflow(const double* L, int npad, const double* invL,
     CholScratch* sc = scratch_or_default(scratch);
     if(!cfg || !sc) { set_error("the persistent Cholesky kernel is not available on this device"); return false; }
     int nb = npad / T, ld = npad;
-    MB200_CUDA_CHECK(cudaMemsetAsync(sc->xbuf, 0xff, (size_t)nb * T * sizeof(double), s));
-    MB200_CUDA_CHECK(cudaMemsetAsync(sc->flags + kMaxTiles, 0, sizeof(int), s));
     int* abort_flag = sc->flags + kMaxTiles;
+    WordFill clear;   // the solution slots to all-ones bytes (not yet written), the abort flag to 0
+    clear.add(sc->xbuf, (size_t)nb * T * sizeof(double), 0xffffffffu);
+    clear.add(abort_flag, sizeof(int));
+    if(!fill_words(clear, s)) return false;
     double* xbuf = sc->xbuf;
     void* args[] = {&L, &ld, &nb, &invL, &B, &xbuf, &abort_flag, &d_info, &d_run_if};
     const int grid = nb < cfg->num_sms ? nb : cfg->num_sms;

@@ -897,7 +897,7 @@ __global__ void marks_unstage_kernel(int* __restrict__ active, int n_r, double* 
 }
 
 bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, cudaStream_t s, int* nlaunch, bool boards_done,
-                    double* rider, bool* rider_summed)
+                    double* rider, bool* rider_summed, bool copy_sizes)
 {
     if(rider_summed) *rider_summed = false;
     if(!configure_kernels()) return false;
@@ -934,16 +934,22 @@ bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& o
     compact_scan_kernel<<<1, 1024, 0, s>>>(N);
     (*nlaunch)++;
     if(N.det_available && !N.fused && !normal_det_item_offsets(dp, N, s, nlaunch)) return false;
-    MB200_CUDA_CHECK(cudaMemcpyAsync(N.h_stat, N.stat, 4 * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if(copy_sizes) MB200_CUDA_CHECK(cudaMemcpyAsync(N.h_stat, N.stat, 4 * sizeof(int), cudaMemcpyDeviceToHost, s));
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;
 }
 
+void normal_marks_to_clear(const NormalBuffers& N, WordFill* f)
+{
+    f->add(N.active, (size_t)(N.n_r > 0 ? N.n_r : 1) * sizeof(int));
+    f->add(N.stat, 4 * sizeof(int));
+}
+
 bool normal_clear_marks(NormalBuffers& N, cudaStream_t s)
 {
-    MB200_CUDA_CHECK(cudaMemsetAsync(N.active, 0, (size_t)(N.n_r > 0 ? N.n_r : 1) * sizeof(int), s));
-    MB200_CUDA_CHECK(cudaMemsetAsync(N.stat, 0, 4 * sizeof(int), s));
-    return true;
+    WordFill f;
+    normal_marks_to_clear(N, &f);
+    return fill_words(f, s);
 }
 
 // After the stream was synchronised: take over what normal_prepare() found
@@ -1019,7 +1025,7 @@ bool normal_assemble(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& 
 
 // Pass 2: Gram matrices, Schur elimination, regularization, right-hand side: S, g', J'x
 bool normal_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
-                   double lambda, cudaStream_t s, int* nlaunch, bool boards_done)
+                   double lambda, cudaStream_t s, int* nlaunch, bool boards_done, double* also_clear, int also_clear_n)
 {
     const size_t lmap_bytes = ((size_t)dp.Nintr_state * sizeof(short) + 7) / 8 * 8;
     const size_t ccol_bytes = ((size_t)N.cap * sizeof(int) + 7) / 8 * 8;
@@ -1028,8 +1034,13 @@ bool normal_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op
     const int ncols_pad = ((max_ntot + 1 + 7) / 8) * 8;
     if(Nwi == 0) N.det = false;
     if(!N.det) N.ldS = chol_padded(N.n_c + 1) > N.ldS_max ? N.ldS_max : chol_padded(N.n_c + 1);
-    MB200_CUDA_CHECK(cudaMemsetAsync(N.g_full, 0, (size_t)dp.Nstate * sizeof(double), s));
-    MB200_CUDA_CHECK(cudaMemsetAsync(N.info, 0, sizeof(int), s));
+    // every accumulator and counter of the assembly (and the caller's scalars) zeroed in one launch
+    WordFill clear;
+    clear.add(N.g_full, (size_t)dp.Nstate * sizeof(double));
+    clear.add(N.info, sizeof(int));
+    if(also_clear) clear.add(also_clear, (size_t)also_clear_n * sizeof(double));
+    if(N.det) normal_det_to_clear(N, &clear);
+    if(!fill_words(clear, s)) return false;
 
     if(N.det)
     {

@@ -1,6 +1,7 @@
 // Internal: normal-equation assembly + Schur elimination (normal.cu)
 #pragma once
 #include "problem.h"
+#include "chol.h"
 
 namespace mb200 {
 
@@ -81,12 +82,15 @@ struct NormalBuffers
 
 // The same in pieces, for a caller that wants to pick its own moment to wait for the device:
 // prepare (device work + an async copy of the sizes) -> [synchronise the stream] -> adopt_sizes -> finish
+// (copy_sizes = false: the caller copies stat[] to h_stat itself, together with its own scalars)
 bool normal_clear_marks(NormalBuffers& N, cudaStream_t s);
+void normal_marks_to_clear(const NormalBuffers& N, WordFill* f);   // the same buffers, into the caller's fill
 bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, cudaStream_t s, int* nlaunch, bool boards_done,
-                    double* rider = nullptr, bool* rider_summed = nullptr);
+                    double* rider = nullptr, bool* rider_summed = nullptr, bool copy_sizes = true);
 bool normal_adopt_sizes(NormalBuffers& N);
+// also_clear: n doubles of the caller's that are zeroed with the assembly's own accumulators (one launch)
 bool normal_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
-                   double lambda, cudaStream_t s, int* nlaunch, bool boards_done);
+                   double lambda, cudaStream_t s, int* nlaunch, bool boards_done, double* also_clear = nullptr, int also_clear_n = 0);
 // fused_eval.cu
 bool launch_fused_boards(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& out, double* norm_part, cudaStream_t s, int* nlaunch);
 bool launch_quadform_boards(const DevProblem& dp, const NormalBuffers& N, const double* g_full, double* part, double* out, cudaStream_t s, int* nlaunch);
@@ -110,6 +114,7 @@ bool normal_expand_step(const DevProblem& dp, const NormalBuffers& N, const Eval
 bool normal_det_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
                        double lambda, cudaStream_t s, int* nlaunch);
 bool normal_det_item_prepare(const DevProblem& dp, NormalBuffers& N, cudaStream_t s, int* nlaunch);   // after the compaction
+void normal_det_to_clear(const NormalBuffers& N, WordFill* f);   // before item_prepare: what it and det_finish expect zeroed
 bool normal_det_item_offsets(const DevProblem& dp, NormalBuffers& N, cudaStream_t s, int* nlaunch);   // before it
 size_t normal_det_part_scratch_doubles(int nblk_max);
 int normal_det_part_arrive_ints(int nblk_max);

@@ -30,6 +30,7 @@
 // sparse JtJ (call site mrcal.c:6435).
 #include "normal_items.cuh"
 #include "chol.h"
+#include "chol.h"
 
 namespace mb200 {
 
@@ -910,12 +911,19 @@ bool normal_det_item_offsets(const DevProblem& dp, NormalBuffers& N, cudaStream_
     return true;
 }
 
+// What the stages below expect cleared when they start: the presence bitmaps and the tiles' arrival counters
+void normal_det_to_clear(const NormalBuffers& N, WordFill* f)
+{
+    const int nblk = N.ldS / TB;
+    f->add(N.wi_present, (size_t)nblk * N.wwords * sizeof(unsigned));
+    if(N.Ngroups > 0) f->add(N.grp_present, (size_t)nblk * N.gwords * sizeof(unsigned));
+    f->add(N.part_arrive, (size_t)(nblk * (nblk + 1) / 2) * sizeof(int));
+}
+
 bool normal_det_item_prepare(const DevProblem& dp, NormalBuffers& N, cudaStream_t s, int* nlaunch)
 {
     const int Nwi = dp.Nobs_board + dp.Nobs_point;
     const int nblk = N.ldS / TB;
-    MB200_CUDA_CHECK(cudaMemsetAsync(N.wi_present, 0, (size_t)nblk * N.wwords * sizeof(unsigned), s));
-    if(N.Ngroups > 0) MB200_CUDA_CHECK(cudaMemsetAsync(N.grp_present, 0, (size_t)nblk * N.gwords * sizeof(unsigned), s));
     if(Nwi > 0)
     {
         item_prepare_kernel<<<(Nwi * 32 + 255) / 256, 256, 0, s>>>(N, Nwi, N.n_c, nblk);
@@ -955,9 +963,8 @@ bool normal_det_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers
     }
     const bool sharded = comm_active();
     if(sharded && N.S_packed == nullptr) { set_error("internal error: sharded solve without the packed tile buffer"); return false; }
-    // part_arrive: [ntiles] arrival counters | the plan | the CTA list (+ its length)
+    // part_arrive: [ntiles] arrival counters (cleared with normal_det_to_clear) | the plan | the CTA list (+ its length)
     const int ntiles_max = N.nblk_max * (N.nblk_max + 1) / 2;
-    MB200_CUDA_CHECK(cudaMemsetAsync(N.part_arrive, 0, (size_t)ntiles * sizeof(int), s));
     int* plan = N.part_arrive + ntiles_max;
     int* cta = plan + (size_t)kPlanInts * ntiles_max;
     static const int ns_per_item = env_int("MRCAL_B200_TILE_NS_PER_ITEM", 1000), ns_per_group = env_int("MRCAL_B200_TILE_NS_PER_GROUP", 270),

@@ -263,6 +263,8 @@ static bool build_workspace(mrcal_b200_problem* P)
     MB200_CUDA_CHECK(cudaMallocHost(&ws->h_info, 16 * sizeof(int)));
     N.h_stat = ws->h_info + 4;
     ws->h_ictl = ws->h_info + 8;
+    MB200_CUDA_CHECK(cudaHostGetDevicePointer((void**)&ws->h_scal_dev, ws->h_scal, 0));
+    MB200_CUDA_CHECK(cudaHostGetDevicePointer((void**)&ws->h_info_dev, ws->h_info, 0));
     if(!chol_scratch_create(&ws->chol)) return false;
     MB200_CUDA_CHECK(cudaMemcpyAsync(N.grp_ptr, ptr.data(), ptr.size() * sizeof(int), cudaMemcpyHostToDevice, P->stream));
     if(!items.empty())
@@ -399,6 +401,23 @@ __global__ void select_step_kernel(double* __restrict__ scal, const int* __restr
     scal[SC_EXPECTED] = -2. * x_Js - Js2;
 }
 
+// Everything the host looks at after a step, straight into its pinned mirrors in one launch (one stream operation
+// instead of a device-to-device and four device-to-host copies): the scalars, with |x|^2 of the trial point in slot 22,
+// the factorization codes, the sizes normal_prepare() found, the control flags. h_info: [0..1] info, [4..7] stat,
+// [8..9] ictl (the layout of the SolverWorkspace mirrors)
+__global__ void read_back_kernel(double* __restrict__ scal, const double* __restrict__ norm2, const int* __restrict__ info,
+                                 const int* __restrict__ stat, const int* __restrict__ ictl, double* __restrict__ h_scal,
+                                 int* __restrict__ h_info)
+{
+    const int i = threadIdx.x;
+    const double n2 = *norm2;
+    if(i < SC_N) h_scal[i] = i == 22 ? n2 : scal[i];
+    if(i == 22) scal[22] = n2;
+    if(i < 2) h_info[i] = info[i];
+    if(i < 4) h_info[4 + i] = stat[i];
+    if(i < 2) h_info[8 + i] = ictl[i];
+}
+
 // step = cg g + cn gn ; p_new = p + step, with cg, cn read on the device
 __global__ void combine_step_dev_kernel(int n, const double* __restrict__ scal, const double* __restrict__ g, const double* __restrict__ gn,
                                         const double* __restrict__ p, double* __restrict__ step, double* __restrict__ p_new)
@@ -511,8 +530,10 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
         {
             // boards: residuals and normal-equation blocks in one pass, no Jacobian; the rest (points, regularization) as usual
             const EvalBuffers& o = P->op[which];
-            MB200_CUDA_CHECK(cudaMemsetAsync(o.norm2, 0, sizeof(double), s));
-            if(!normal_clear_marks(N, s) || !launch_unpack_state(P->dp, o.p, s, nl) ||
+            WordFill clear;   // the cost and the marks of the columns, in one launch
+            clear.add(o.norm2, sizeof(double));
+            normal_marks_to_clear(N, &clear);
+            if(!fill_words(clear, s) || !launch_unpack_state(P->dp, o.p, s, nl) ||
                !launch_fused_boards(P->dp, N, o, N.norm_part, s, nl) ||
                !launch_evaluate(P->dp, o, true, nullptr, s, nl, false)) return false;
         }
@@ -520,8 +541,9 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
         T->spans[0].push_back({a, T->mark()});
         info->Nevaluations++;
         const int b = T->mark();
-        // (sharded: the cost of this evaluation is summed over the ranks in the collective that unites the active sets)
-        if(!normal_prepare(P->dp, N, P->op[which], s, nl, N.fused, P->op[which].norm2, &norm2_summed)) return false;
+        // (sharded: the cost of this evaluation is summed over the ranks in the collective that unites the active sets.
+        // Not sharded: the sizes reach the host with the step's scalars, in read_back)
+        if(!normal_prepare(P->dp, N, P->op[which], s, nl, N.fused, P->op[which].norm2, &norm2_summed, comm_active())) return false;
         T->spans[1].push_back({b, T->mark()});
         return true;
     };
@@ -529,16 +551,28 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
     {
         if(!N.selfchecked && !solver_selfcheck(P, which, *lambda)) return false;
         const int a = T->mark();
-        if(!normal_finish(P->dp, N, P->op[which], P->d_rowptr, *lambda, s, nl, N.fused)) return false;
+        // (the scalars of the Cauchy step that follows are cleared with the assembly's accumulators)
+        if(!normal_finish(P->dp, N, P->op[which], P->d_rowptr, *lambda, s, nl, N.fused, ws->scal, 32)) return false;
         T->spans[1].push_back({a, T->mark()});
         return true;
     };
-    // ONE device -> host read per iteration: the scalars, the control flags, the factorization codes
-    auto read_back = [&]() -> bool
+    // ONE device -> host read per iteration: the scalars (|x|^2 of the evaluation at op[which] in slot 22), the control
+    // flags, the factorization codes, the sizes of the next reduced system
+    auto read_back = [&](int which) -> bool
     {
-        MB200_CUDA_CHECK(cudaMemcpyAsync(ws->h_scal, ws->scal, SC_N * sizeof(double), cudaMemcpyDeviceToHost, s));
-        MB200_CUDA_CHECK(cudaMemcpyAsync(ws->h_info, N.info, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
-        MB200_CUDA_CHECK(cudaMemcpyAsync(ws->h_ictl, ws->ictl, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+        if(comm_active())
+        {
+            // (sharded: |x|^2 is summed over the ranks in place, in scal[22])
+            MB200_CUDA_CHECK(cudaMemcpyAsync(ws->h_scal, ws->scal, SC_N * sizeof(double), cudaMemcpyDeviceToHost, s));
+            MB200_CUDA_CHECK(cudaMemcpyAsync(ws->h_info, N.info, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+            MB200_CUDA_CHECK(cudaMemcpyAsync(ws->h_ictl, ws->ictl, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+        }
+        else
+        {
+            read_back_kernel<<<1, 64, 0, s>>>(ws->scal, P->op[which].norm2, N.info, N.stat, ws->ictl, ws->h_scal_dev, ws->h_info_dev);
+            (*nl)++;
+            MB200_CUDA_CHECK(cudaGetLastError());
+        }
         MB200_CUDA_CHECK(cudaStreamSynchronize(s));
         info->Nsyncs++;
         return normal_adopt_sizes(N);   // n_c, widest item: from the prepare() that ran last
@@ -563,9 +597,12 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
         for(int attempt = 0; attempt < 2; attempt++)
         {
             if(!evaluate(which)) return false;
-            MB200_CUDA_CHECK(cudaMemcpyAsync(ws->scal + 22, P->op[which].norm2, sizeof(double), cudaMemcpyDeviceToDevice, s));
-            if(comm_active() && !norm2_summed && !comm_allreduce_sum(ws->scal + 22, 1, s)) return false;
-            if(!read_back()) return false;
+            if(comm_active())
+            {
+                MB200_CUDA_CHECK(cudaMemcpyAsync(ws->scal + 22, P->op[which].norm2, sizeof(double), cudaMemcpyDeviceToDevice, s));
+                if(!norm2_summed && !comm_allreduce_sum(ws->scal + 22, 1, s)) return false;
+            }
+            if(!read_back(which)) return false;
             if(!(N.fused && N.h_stat[3] != 0)) return true;
             fprintf(stderr, "mrcal_b200: an observation touches more control points than the fused evaluation handles: "
                             "continuing with the stored-Jacobian path\n");
@@ -611,7 +648,7 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
             const bool overlap = N.s_side[0] != nullptr && getenv("MRCAL_B200_NO_OVERLAP") == nullptr;
             if(!have_cauchy)
             {
-                MB200_CUDA_CHECK(cudaMemsetAsync(ws->scal, 0, 32 * sizeof(double), s));
+                // (scal[0..31] were cleared by the assembly, which always comes right before)
                 cudaStream_t sc = s;
                 if(overlap)
                 {

@@ -22,6 +22,8 @@ struct SolverWorkspace
     int*    h_info = nullptr;     // pinned
     int*    ictl = nullptr;       // [8] device control flags of the step logic
     int*    h_ictl = nullptr;     // pinned
+    double* h_scal_dev = nullptr; // the device's addresses of the pinned mirrors (read_back_kernel writes them directly)
+    int*    h_info_dev = nullptr;
     CholScratch chol;             // this workspace's own flags of the persistent factorization kernels
     std::vector<cudaEvent_t> ev;
     ~SolverWorkspace()
