@@ -541,6 +541,34 @@ bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* problem, in
                                                bool atinfinity, const mrcal_point3_t* p_cam, int N,
                                                double observed_pixel_uncertainty, double* Var, double* sigma_used);
 
+/* The transformation implied by two cameras' intrinsics, as mrcal.implied_Rt10__from_unprojections() fits it
+   (mrcal/model_analysis.py:27-395): Rt10 [4][3] (R then t; t = 0 if atinfinity) minimizing the huber-robust sum over the
+   points (m, i) in the focus region (|q0[i] - focus_center|^2 < focus_radius^2) of (w[m][i] th2)^2, th2 = 2 (1 -
+   cos(angle between R p0[m][i] + t and v1[i])). p0 [M][N]: unit vectors if atinfinity, else points; v1 [N]: unit
+   vectors; weights [M][N] or NULL for 1. Points with a non-finite p0, v1 or weight are ignored. One CTA on the device
+   runs the whole fit. False + mrcal_b200_last_error() on refusal ("Focus region contained too few points": fewer than
+   3) or failure */
+bool mrcal_b200_implied_Rt10__from_unprojections(double* Rt10, const mrcal_point2_t* q0, int N, const mrcal_point3_t* p0,
+                                                 int M, const mrcal_point3_t* v1, const double* weights, bool atinfinity,
+                                                 const double* focus_center, double focus_radius);
+
+/* The projection difference of Nmodels >= 2 camera models over a grid, as mrcal.projection_diff() computes it after
+   its unprojection (mrcal/model_analysis.py:1520-1928). q0 [N]: the grid; v [Nmodels][N]: its unit rays unprojected
+   by each model; distance [Nd], or NULL for infinity (Nd = 1); lensmodels [Nmodels] and their intrinsics, concatenated
+   in model order. If fit_Rt10, Rt10 [Nmodels-1][4][3] is fitted for each pair (0, k) as
+   mrcal_b200_implied_Rt10__from_unprojections() does, with p0 = v[0] * distance, v1 = v[k] and, if uncertainties
+   [Nmodels][Nd][N] (worst-direction stdev of each model's projection of v[k] * distance) is given, the weights
+   (1/(u_0 u_k))^2; all pairs in one launch. Otherwise Rt10 is read. Then q_k = project_k(R_k v[0] distance + t_k):
+   with 2 models difflen [Nd][N] = |q_1 - q0| and diff [Nd][N][2] = q_1 - q0 (may be NULL); with more, difflen =
+   sqrt(mean_k |q_k - q0|^2). Each grid-sized array crosses the bus once each way. False + mrcal_b200_last_error() on
+   refusal or failure */
+bool mrcal_b200_projection_diff(double* Rt10, double* difflen, double* diff,
+                                const mrcal_point2_t* q0, int N, const mrcal_point3_t* v, int Nmodels,
+                                const double* distance, int Nd,
+                                const mrcal_lensmodel_t* lensmodels, const double* intrinsics,
+                                const double* uncertainties, const double* focus_center, double focus_radius,
+                                bool fit_Rt10);
+
 // Timing hook for benchmarks: run N cost-function evaluations (residuals +
 // Jacobian) at the current state back to back, return the mean device time per
 // evaluation in milliseconds (CUDA events on the library's stream); <0 on error

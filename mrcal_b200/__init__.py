@@ -4,6 +4,7 @@ trust-region normal-equations solve -- behind mrcal's own Python API for that
 path. See DESIGN.md and INTEGRATION.md at the repository root."""
 from .api import (  # noqa: F401
     optimize, optimizer_callback, drt_cross_reprojection__dbpacked, projection_uncertainty, worst_direction_stdev,
+    sample_imager, sample_imager_unproject, implied_Rt10__from_unprojections, projection_diff,
     Problem, CHOLMOD_factorization,
     lensmodel_num_params, supported_lensmodels, lensmodel_metadata_and_config, knots_for_splined_models,
     state_index_intrinsics, state_index_extrinsics, state_index_frames, state_index_points,

@@ -111,6 +111,7 @@ EXPORTED_SYMBOLS = (
     "mrcal_b200_problem_triangulated_outliers",
     "mrcal_b200_problem_drt_cross_reprojection__dbpacked",
     "mrcal_b200_problem_projection_uncertainty",
+    "mrcal_b200_implied_Rt10__from_unprojections", "mrcal_b200_projection_diff",
     "mrcal_b200_nccl_get_unique_id", "mrcal_b200_nccl_comm_init", "mrcal_b200_nccl_comm_destroy",
     "mrcal_b200_problem_set_sharding",
     "mrcal_b200_factorization_create", "mrcal_b200_factorization_destroy",
@@ -155,6 +156,13 @@ lib.mrcal_b200_problem_drt_cross_reprojection__dbpacked.argtypes = [C.c_void_p, 
 lib.mrcal_b200_problem_projection_uncertainty.restype = C.c_bool
 lib.mrcal_b200_problem_projection_uncertainty.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_bool, C.c_void_p, C.c_int,
                                                            C.c_double, C.c_void_p, C.c_void_p]
+lib.mrcal_b200_implied_Rt10__from_unprojections.restype = C.c_bool
+lib.mrcal_b200_implied_Rt10__from_unprojections.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                                             C.c_void_p, C.c_void_p, C.c_bool, C.c_void_p, C.c_double]
+lib.mrcal_b200_projection_diff.restype = C.c_bool
+lib.mrcal_b200_projection_diff.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                           C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_double, C.c_bool]
 lib.mrcal_b200_factorization_create_from_last_callback.restype = C.c_void_p
 lib.mrcal_b200_csr_create.restype = C.c_void_p
 lib.mrcal_b200_csr_destroy.restype = None

@@ -15,6 +15,8 @@ marshals arguments, the way mrcal-pywrap.c does for the reference.
 """
 import ctypes as C
 import os
+import re
+import sys
 
 import numpy as np
 import scipy.sparse
@@ -371,6 +373,174 @@ def projection_uncertainty(p_cam, model, *, method="cross-reprojection-ccp", ati
     if what == "worstdirection-stdev":
         return worst_direction_stdev(Var)
     return np.sqrt((Var[..., 0, 0] + Var[..., 1, 1]) / 2.)
+
+
+####################################################################################################
+# comparing camera models (mrcal/utils.py:268-450, mrcal/model_analysis.py:27-395, 1520-1928)
+####################################################################################################
+def sample_imager(gridn_width, gridn_height, imager_width, imager_height):
+    """A regular grid over the imager, shape (gridn_height, gridn_width, 2) of (x, y): [0,0] is (0,0), [-1,-1] is
+    (W-1, H-1). gridn_height=None keeps the grid square-ish: int(round(H/W*gridn_width))"""
+    if gridn_height is None:
+        gridn_height = int(round(imager_height / imager_width * gridn_width))
+    w = np.linspace(0, imager_width - 1, gridn_width)
+    h = np.linspace(0, imager_height - 1, gridn_height)
+    return np.ascontiguousarray(np.stack(np.meshgrid(w, h), axis=-1))
+
+
+def sample_imager_unproject(gridn_width, gridn_height, imager_width, imager_height, lensmodel, intrinsics_data,
+                            normalize=False):
+    """(v, q): the grid of sample_imager() and its unprojection. One camera (lensmodel a string): v (Nh, Nw, 3). A
+    list or tuple of lens models: v (Ncameras, Nh, Nw, 3), each camera unprojecting the same grid"""
+    q = sample_imager(gridn_width, gridn_height, imager_width, imager_height)
+
+    def unp(lm, intr):
+        v = unproject(q, lm, intr)
+        return v / np.linalg.norm(v, axis=-1)[..., None] if normalize else v
+    if isinstance(lensmodel, (list, tuple)):
+        return np.array([unp(lensmodel[i], intrinsics_data[i]) for i in range(len(lensmodel))]), q
+    return unp(lensmodel, intrinsics_data), q
+
+
+def _as_points(a, n, name):
+    a = np.ascontiguousarray(a, np.float64)
+    if a.ndim == 0 or a.shape[-1] != n:
+        raise RuntimeError(f"{name} must have shape (...,{n}); got {a.shape}")
+    return a
+
+
+def implied_Rt10__from_unprojections(q0, p0, v1, *, weights=None, atinfinity=True, focus_center=(0., 0.),
+                                     focus_radius=1.0e8):
+    """The Rt transformation (4,3) from camera 0 to camera 1 that best lines up the unprojections p0 (..., Nh, Nw, 3)
+    of camera 0 (unit vectors at infinity, else points) with the unit vectors v1 (Nh, Nw, 3) of camera 1 over the grid
+    q0 (Nh, Nw, 2), as mrcal.implied_Rt10__from_unprojections() fits it. Leading dimensions of p0 and weights
+    (..., Nh, Nw) are fitted together. atinfinity fits a rotation only (t = 0). Only grid points strictly within
+    focus_radius of focus_center are used; non-finite rays and weights are ignored. The fit runs on the device
+    (csrc/diff.cu)"""
+    _require_gpu()
+    q0 = _as_points(q0, 2, "q0").reshape(-1, 2)
+    N = q0.shape[0]
+    p0 = _as_points(p0, 3, "p0")
+    v1 = _as_points(v1, 3, "v1").reshape(-1, 3)
+    if v1.shape[0] != N or N == 0 or p0.size % (3 * N):
+        raise RuntimeError(f"q0, p0, v1 must describe the same grid; got shapes {q0.shape}, {p0.shape}, {v1.shape}")
+    p0 = p0.reshape(-1, N, 3)
+    M = p0.shape[0]
+    if weights is not None:
+        weights = np.ascontiguousarray(weights, np.float64)
+        if weights.size != M * N:
+            raise RuntimeError(f"weights must have the shape of p0 without its last dimension; got {weights.shape}")
+    fc = np.ascontiguousarray(focus_center, np.float64).reshape(2)
+    Rt = np.zeros((4, 3))
+    if not lib.mrcal_b200_implied_Rt10__from_unprojections(_ptr(Rt), _ptr(q0), N, _ptr(p0), M, _ptr(v1),
+                                                           _ptr(weights) if weights is not None else None,
+                                                           bool(atinfinity), _ptr(fc), float(focus_radius)):
+        raise RuntimeError(_capi.last_error())
+    return Rt
+
+
+def _compose_Rt(A, B):
+    return np.vstack((A[:3] @ B[:3], A[:3] @ B[3] + A[3]))
+
+
+def _identity_Rt():
+    return np.vstack((np.eye(3), np.zeros(3)))
+
+
+def projection_diff(models, *, implied_Rt10=None, gridn_width=60, gridn_height=None, intrinsics_only=False,
+                    distance=None, use_uncertainties=True, focus_center=None, focus_radius=-1.):
+    """The difference in projection between camera models, as mrcal.projection_diff() computes it. Returns
+    (difflen, diff, q0, Rt10): difflen (..., Nh, Nw) the length of the projection difference (2 models) or
+    sqrt(mean_k |q_k - q0|^2) over models 1..N-1 (more); diff (..., Nh, Nw, 2) or None for more than 2 models; q0 the
+    grid (Nh, Nw, 2); Rt10 (4,3), or (Nmodels-1, 4, 3), the transformations from camera 0 to each other camera. An
+    iterable distance adds a leading dimension. Rt10 is implied_Rt10 if given, the identity if intrinsics_only, the
+    models' relative extrinsics if focus_radius == 0, and otherwise fitted, weighted by the projection uncertainties
+    if use_uncertainties and the models carry optimization_inputs. The fit and the reprojections run on the device
+    (csrc/diff.cu), all pairs of models in one call"""
+    if len(models) < 2:
+        raise RuntimeError("At least 2 models are required to compute the diff")
+    if len(models) > 2 and implied_Rt10 is not None:
+        raise RuntimeError("A given implied_Rt10 is currently supported ONLY if exactly 2 models are being compared")
+    try:
+        len(distance)
+        distance_is_iterable = True
+    except TypeError:
+        distance_is_iterable = False
+    atinfinity = distance is None
+    dist = np.ones(1) if atinfinity else np.ascontiguousarray(np.atleast_1d(np.array(distance, np.float64)).ravel())
+
+    imagersizes = np.array([m.imagersize() for m in models])
+    if np.linalg.norm(np.std(imagersizes, axis=-2)) != 0:
+        raise RuntimeError(f"The diff function needs all the imager dimensions to match. Instead got {imagersizes}")
+    W, H = imagersizes[0]
+    lensmodels = [m.intrinsics()[0] for m in models]
+    intrinsics_data = [m.intrinsics()[1] for m in models]
+    # noncentral models (model_analysis.py:1759-1772)
+    for i in range(len(models)):
+        if lensmodel_metadata_and_config(lensmodels[i])["noncentral"] and not \
+           (re.match("LENSMODEL_CAHVORE_", lensmodels[i]) and np.sum(intrinsics_data[i][-3:] ** 2) < 1e-12):
+            if not atinfinity:
+                raise RuntimeError(f"Model {i} is noncentral, so I can only evaluate the diff at infinity")
+            if re.match("LENSMODEL_CAHVORE_", lensmodels[i]):
+                if use_uncertainties:
+                    raise RuntimeError("I have a noncentral model. No usable uncertainties for those yet")
+                intrinsics_data[i][-3:] = 0   # a copy: centralize CAHVORE
+            else:
+                raise RuntimeError("I have a non-CAHVORE noncentral model. This isn't supported yet")
+
+    v, q0 = sample_imager_unproject(gridn_width, gridn_height, W, H, lensmodels, intrinsics_data, normalize=True)
+    Nmodels, Nd = len(models), dist.size
+
+    uncertainties = None
+    if use_uncertainties and not intrinsics_only and focus_radius != 0 and implied_Rt10 is None:
+        try:
+            uncertainties = np.array([projection_uncertainty(v[i] * dist[:, None, None, None], models[i],
+                                                             atinfinity=atinfinity, what="worstdirection-stdev")
+                                      for i in range(Nmodels)])
+        except Exception as e:
+            print("WARNING: projection_diff() was asked to use uncertainties, but they aren't available/couldn't be "
+                  f"computed. Falling back on the region-based-only logic. Caught exception: {e}", file=sys.stderr)
+    if focus_center is None:
+        focus_center = ((W - 1.) / 2., (H - 1.) / 2.)
+    if focus_radius < 0:
+        focus_radius = float(max(W, H) * 100.) if uncertainties is not None else float(min(W, H) / 6.)
+
+    fit = False
+    if implied_Rt10 is not None:
+        Rt10 = np.array(implied_Rt10, np.float64).reshape(1, 4, 3)
+    elif intrinsics_only:
+        Rt10 = np.array([_identity_Rt()] * (Nmodels - 1))
+    elif focus_radius == 0:
+        Rt10 = np.array([_compose_Rt(models[k].Rt_cam_ref(), models[0].Rt_ref_cam()) for k in range(1, Nmodels)])
+    else:
+        Rt10 = np.zeros((Nmodels - 1, 4, 3))
+        fit = True
+
+    lms = (_capi.Lensmodel * Nmodels)(*[_lensmodel(lm) for lm in lensmodels])
+    intr = np.ascontiguousarray(np.concatenate(intrinsics_data), np.float64)
+    vv = np.ascontiguousarray(v.reshape(Nmodels, -1, 3))
+    qq = q0.reshape(-1, 2)
+    N = qq.shape[0]
+    difflen = np.zeros((Nd, N))
+    diff = np.zeros((Nd, N, 2)) if Nmodels == 2 else None
+    fc = np.ascontiguousarray(focus_center, np.float64).reshape(2)
+    U = np.ascontiguousarray(uncertainties.reshape(Nmodels, Nd, N)) if uncertainties is not None and fit else None
+    if not lib.mrcal_b200_projection_diff(_ptr(Rt10), _ptr(difflen), _ptr(diff) if diff is not None else None,
+                                          _ptr(qq), N, _ptr(vv), Nmodels, None if atinfinity else _ptr(dist), Nd,
+                                          lms, _ptr(intr), _ptr(U) if U is not None else None, _ptr(fc),
+                                          float(focus_radius), fit):
+        raise RuntimeError(_capi.last_error())
+
+    difflen = difflen.reshape((Nd,) + q0.shape[:2])
+    if diff is not None:
+        diff = diff.reshape((Nd,) + q0.shape)
+    if not distance_is_iterable:
+        difflen = difflen[0]
+        if diff is not None:
+            diff = diff[0]
+    if implied_Rt10 is not None:
+        return difflen, diff, q0, implied_Rt10
+    return difflen, diff, q0, (Rt10[0] if Nmodels == 2 else Rt10)
 
 
 def optimizer_callback(no_jacobian=False, no_factorization=False, **kwargs):

@@ -210,6 +210,14 @@ class cameramodel:
             return self.rt_cam_ref(invert_rt(rt))
         return invert_rt(self._rt_cam_ref)
 
+    def Rt_cam_ref(self):
+        """The pose as a (4,3) Rt transformation: R on top, t in the last row"""
+        return np.vstack((_R_from_r(self._rt_cam_ref[:3]), self._rt_cam_ref[3:]))
+
+    def Rt_ref_cam(self):
+        rt = self.rt_ref_cam()
+        return np.vstack((_R_from_r(rt[:3]), rt[3:]))
+
     extrinsics_rt_fromref = rt_cam_ref
     extrinsics_rt_toref = rt_ref_cam
 

@@ -12,29 +12,11 @@
 
 #include "common.h"
 #include "device_math.cuh"
+#include "lens_dispatch.cuh"
 #include "problem.h"
 
 namespace mb200 {
-
-bool spline_segments_per_u(double* out, const mrcal_lensmodel_t* lm);   // layout.cpp
-int lens_kind_of(const mrcal_lensmodel_t* lm);                          // problem.cu
-
 namespace {
-
-struct LensArgs { const double* intr; int Nx, Ny; double segments_per_u, cfg; };
-
-template <int KIND>
-__device__ __forceinline__ void project_any(double q[2], double dq_dp[2][3], const double* p, const LensArgs& a)
-{
-    if constexpr(LensTraits<KIND>::SPLINED)
-    {
-        double wx[4], wy[4], upd[2];
-        int ivar0;
-        project_splined<LensTraits<KIND>::RUN>(q, dq_dp, wx, wy, &ivar0, upd, p, a.intr, a.Nx, a.Ny, a.segments_per_u);
-    }
-    else
-        project_parametric<KIND>(q, dq_dp, nullptr, p, a.intr, a.cfg);
-}
 
 // dq_di: dense (N,2,Nintr), zeroed by the caller, or NULL. The layout of mrcal.c:2936-2992: the core (dq/df
 // on its own axis only, dq/dc = I), then the distortions -- dense for the parametric models, the RUN x RUN touched
@@ -170,25 +152,16 @@ bool run(bool unproject, double* out, double* dq_dp, double* dq_di, const double
     if(kind < 0) { set_error("this lens model has no CUDA implementation"); return false; }
     const int Nintr = mrcal_lensmodel_num_params(lensmodel);
     if(N <= 0) return true;
-    LensArgs a = {};
-    if(kind == LENS_SPLINED3 || kind == LENS_SPLINED2)
-    {
-        a.Nx = lensmodel->LENSMODEL_SPLINED_STEREOGRAPHIC__config.Nx;
-        a.Ny = lensmodel->LENSMODEL_SPLINED_STEREOGRAPHIC__config.Ny;
-        if(!spline_segments_per_u(&a.segments_per_u, lensmodel)) return false;
-    }
-    if(kind == LENS_CAHVORE)
-    {
-        a.cfg = lensmodel->LENSMODEL_CAHVORE__config.linearity;
-        if(unproject)
-            for(int i = Nintr - 3; i < Nintr; i++)
-                if(intrinsics[i] != 0.)
-                {
-                    // the reference's rule (mrcal.c:3203-3214)
-                    set_error("unproject() currently only works with a central projection. So I cannot unproject(CAHVORE,E!=0)");
-                    return false;
-                }
-    }
+    LensArgs a;
+    if(!lens_args_setup(&a, kind, lensmodel)) return false;
+    if(kind == LENS_CAHVORE && unproject)
+        for(int i = Nintr - 3; i < Nintr; i++)
+            if(intrinsics[i] != 0.)
+            {
+                // the reference's rule (mrcal.c:3203-3214)
+                set_error("unproject() currently only works with a central projection. So I cannot unproject(CAHVORE,E!=0)");
+                return false;
+            }
     Scratch S;
     const size_t nin = (size_t)N * (unproject ? 2 : 3), nout = (size_t)N * (unproject ? 3 : 2);
     MB200_CUDA_CHECK(cudaMalloc(&S.d_intr, Nintr * sizeof(double)));
@@ -205,17 +178,13 @@ bool run(bool unproject, double* out, double* dq_dp, double* dq_di, const double
     a.intr = S.d_intr;
     const mrcal_lensmodel_metadata_t meta = mrcal_lensmodel_metadata(lensmodel);
     const int threads = 128, blocks = (N + threads - 1) / threads;
-#define MB200_LENS_CASE(K) \
-    case K: if(unproject) unproject_kernel<K><<<blocks, threads>>>(a, S.d_in, N, S.d_out, meta.can_project_behind_camera); \
-            else          project_kernel<K><<<blocks, threads>>>(a, S.d_in, N, S.d_out, S.d_grad, S.d_gi, Nintr); break;
-    switch(kind)
+    const bool ok = dispatch_lens_kind(kind, [&](auto k)
     {
-        MB200_LENS_CASE(LENS_PINHOLE) MB200_LENS_CASE(LENS_STEREOGRAPHIC) MB200_LENS_CASE(LENS_LONLAT) MB200_LENS_CASE(LENS_LATLON)
-        MB200_LENS_CASE(LENS_OPENCV4) MB200_LENS_CASE(LENS_OPENCV5) MB200_LENS_CASE(LENS_OPENCV8) MB200_LENS_CASE(LENS_OPENCV12)
-        MB200_LENS_CASE(LENS_SPLINED3) MB200_LENS_CASE(LENS_SPLINED2) MB200_LENS_CASE(LENS_CAHVOR) MB200_LENS_CASE(LENS_CAHVORE)
-    default: set_error("lens model kind %d has no CUDA implementation", kind); return false;
-    }
-#undef MB200_LENS_CASE
+        constexpr int K = decltype(k)::value;
+        if(unproject) unproject_kernel<K><<<blocks, threads>>>(a, S.d_in, N, S.d_out, meta.can_project_behind_camera);
+        else          project_kernel<K><<<blocks, threads>>>(a, S.d_in, N, S.d_out, S.d_grad, S.d_gi, Nintr);
+    });
+    if(!ok) return false;
     MB200_CUDA_CHECK(cudaGetLastError());
     MB200_CUDA_CHECK(cudaMemcpy(out, S.d_out, nout * sizeof(double), cudaMemcpyDeviceToHost));
     if(dq_dp) MB200_CUDA_CHECK(cudaMemcpy(dq_dp, S.d_grad, (size_t)N * 6 * sizeof(double), cudaMemcpyDeviceToHost));
