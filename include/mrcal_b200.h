@@ -504,6 +504,11 @@ bool mrcal_b200_problem_optimize(mrcal_b200_problem_t* problem,
 // valid; g_reduced [n_reduced]; g_full [Nstate] = J'x. Any output may be NULL
 bool mrcal_b200_problem_reduced_system(mrcal_b200_problem_t* problem, double lambda, int* n_reduced,
                                        double* S_out, double* g_reduced, double* g_full);
+// The same, with the board observations' blocks from the fused evaluation (the
+// path mrcal_b200_problem_optimize() takes for splined models with the core
+// locked) instead of the stored Jacobian. False if this problem does not take it
+bool mrcal_b200_problem_reduced_system_fused(mrcal_b200_problem_t* problem, double lambda, int* n_reduced,
+                                             double* S_out, double* g_reduced, double* g_full);
 
 // Copy results to the host: the packed state, the residuals, the unpacked
 // solution and the (possibly outlier-marked) board observation pool. Any may be NULL

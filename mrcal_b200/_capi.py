@@ -106,7 +106,7 @@ EXPORTED_SYMBOLS = (
     "mrcal_b200_problem_num_states", "mrcal_b200_problem_num_measurements",
     "mrcal_b200_problem_num_j_nonzero", "mrcal_b200_problem_reset", "mrcal_b200_problem_upload",
     "mrcal_b200_problem_callback", "mrcal_b200_problem_optimize", "mrcal_b200_problem_download",
-    "mrcal_b200_problem_reduced_system",
+    "mrcal_b200_problem_reduced_system", "mrcal_b200_problem_reduced_system_fused",
     "mrcal_b200_problem_time_callback",
     "mrcal_b200_problem_triangulated_outliers",
     "mrcal_b200_problem_drt_cross_reprojection__dbpacked",
@@ -137,7 +137,7 @@ for _n in ["mrcal_lensmodel_from_name", "mrcal_lensmodel_name", "mrcal_knots_for
            "mrcal_corresponding_icam_extrinsics", "mrcal_optimizer_callback",
            "mrcal_b200_problem_reset", "mrcal_b200_problem_upload", "mrcal_b200_problem_callback",
            "mrcal_b200_problem_optimize", "mrcal_b200_problem_download", "mrcal_b200_problem_reduced_system",
-           "mrcal_b200_nccl_get_unique_id", "mrcal_b200_nccl_comm_init", "mrcal_b200_problem_set_sharding",
+           "mrcal_b200_problem_reduced_system_fused", "mrcal_b200_nccl_get_unique_id", "mrcal_b200_nccl_comm_init", "mrcal_b200_problem_set_sharding",
            "mrcal_b200_factorization_solve_xt_JtJ_bt", "mrcal_b200_factorization_solve_sys", "mrcal_project", "mrcal_unproject"]:
     getattr(lib, _n).restype = C.c_bool
 lib.mrcal_lensmodel_metadata.restype = Metadata

@@ -801,15 +801,18 @@ class Problem:
         return dict(b_packed=b, x=x, intrinsics=intr, rt_cam_ref=rtc, rt_ref_frame=rtf, points=pts,
                     calobject_warp=warp, observations_board=obs)
 
-    def reduced_system(self, lambda_=0.0):
-        """(S, g_reduced, g_full): the Schur-reduced normal equations at the current state (introspection)."""
+    def reduced_system(self, lambda_=0.0, fused=False):
+        """(S, g_reduced, g_full): the Schur-reduced normal equations at the current state (introspection).
+        fused: the board observations' blocks come from the fused evaluation that optimize() uses for splined models
+        with the core locked, not from the stored Jacobian (RuntimeError if this problem does not take that path)."""
+        fn = lib.mrcal_b200_problem_reduced_system_fused if fused else lib.mrcal_b200_problem_reduced_system
         n = C.c_int(0)
-        if not lib.mrcal_b200_problem_reduced_system(self._h, C.c_double(lambda_), C.byref(n), None, None, None):
+        if not fn(self._h, C.c_double(lambda_), C.byref(n), None, None, None):
             raise RuntimeError(_capi.last_error())
         S = np.zeros((n.value, n.value))
         g = np.zeros(n.value)
         gf = np.zeros(self.Nstate)
-        if not lib.mrcal_b200_problem_reduced_system(self._h, C.c_double(lambda_), C.byref(n), _ptr(S), _ptr(g), _ptr(gf)):
+        if not fn(self._h, C.c_double(lambda_), C.byref(n), _ptr(S), _ptr(g), _ptr(gf)):
             raise RuntimeError(_capi.last_error())
         S = np.tril(S) + np.tril(S, -1).T
         return S, g, gf

@@ -19,8 +19,8 @@
 //      two dense products Dk'[Dk | Gx Gy ex ey] on the fp64 tensor pipe (DMMA 8x8x4) -- a quarter of the flops of
 //      the Gram matrix over the full row width that normal.cu's kernel computes from the stored Jacobian
 //   3. geometry x geometry (14 x 14) and J'x over the geometry: plain FMAs
-//   4. the blocks go out in the layout normal_det.cu consumes (A lower triangle over the local columns in state
-//      order, rows nsh, nsh+1 = -J'x; B, D, gf)
+//   4. the blocks go out in the layout normal_det.cu consumes: A in the compact layout (normal.h, kCompactSlot: fx^2,
+//      fy^2, M = Dk'Dk once, the geometry rows, -J'x once), and B, D, gf
 //
 // Replaces, for this path: the board loop of optimizer_callback() (mrcal.c:4604-4900), libdogleg's Jt*x and what
 // CHOLMOD's A*A' does with those rows.
@@ -33,7 +33,7 @@ namespace {
 
 constexpr int FLDK = 68;    // row stride of Dk [K][<=64 knots]: 4 (mod 16), conflict-free DMMA fragment loads
 constexpr int FLDG = 36;    // row stride of G  [K][32]
-constexpr int FMAXK = 64;   // most knots of one observation's patch that are touched
+constexpr int FMAXK = kCompactMaxKnots;   // most knots of one observation's patch that are touched
 constexpr int FMAXPATCH = 400;   // bounding box of the patch (knots)
 
 struct FusedGeom { double Rf[9], dRf[27], tf[3], Rc[9], dRc[27], tc[3]; };
@@ -243,7 +243,13 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
         }
         if(tid < ncam)  { const int r = N.reduced_index(P.i_extr0 + 6 * icam_e + tid); cols[2 * nk + tid] = r; N.active[r] = 1; }
         if(tid < nwarp) { const int r = N.reduced_index(P.i_warp0 + tid); cols[2 * nk + ncam + tid] = r; N.active[r] = 1; }
-        if(tid == 0) { N.wi_nsh[w_item] = nsh; atomicMax(&N.stat[1], nsh + 6); }
+        if(tid == 0)
+        {
+            N.wi_nsh[w_item] = nsh;
+            N.wi_lda[w_item] = ~nk;   // the compact layout, at this observation's fixed slot
+            N.wi_Aoff[w_item] = (long long)w_item * kCompactSlot;
+            atomicMax(&N.stat[1], nsh + 6);
+        }
     }
     // ---- Dk
     if(have)
@@ -263,8 +269,8 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
     const int g = lane >> 2, t = lane & 3;
     const int ksteps = K >> 2;
     const double fx = intr[0], fy = intr[1];
-    double* Aw = N.wi_A + N.wi_Aoff[w_item];
-    const int lda = N.wi_lda[w_item];
+    double* Aw = N.wi_A + (size_t)w_item * kCompactSlot;
+    if(tid == 0) { Aw[0] = fx * fx; Aw[1] = fy * fy; }
     for(int q0 = warp; q0 < ntiles; q0 += 16)
     {
         int ti[4], tj[4];
@@ -306,18 +312,13 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
             const int k1 = 8 * ti[u] + g;
             if(sym[u])
             {
-                // M[k1][k2], k2 = 8 tj + 2t + h: the x surface gets fx^2 M, the y surface fy^2 M, nothing across.
-                // Local columns are interleaved (knot k: 2k on the x surface, 2k+1 on the y surface), lower triangle
+                // M[k1][k2], k2 = 8 tj + 2t + h, lower triangle: once (the readers scale it by fx^2 and fy^2)
 #pragma unroll
                 for(int h = 0; h < 2; h++)
                 {
                     const int k2 = 8 * tj[u] + 2 * t + h;
                     if(k1 >= nk || k2 > k1) continue;
-                    const double m = acc[u][h];
-                    Aw[(size_t)(2 * k1) * lda + 2 * k2] = fx * fx * m;
-                    Aw[(size_t)(2 * k1 + 1) * lda + 2 * k2 + 1] = fy * fy * m;
-                    Aw[(size_t)(2 * k1 + 1) * lda + 2 * k2] = 0.;
-                    if(k2 < k1) Aw[(size_t)(2 * k1) * lda + 2 * k2 + 1] = 0.;
+                    Aw[2 + k1 * (k1 + 1) / 2 + k2] = acc[u][h];
                 }
             }
             else if(k1 < FMAXK)
@@ -354,6 +355,7 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
     // ---- 4. the rest of the item's blocks. Local geometry column l (after the 2 nk knot columns) -> G column
     auto gcol = [&](int l) { return l < ncam ? l : 12 + (l - ncam); };
     const int ngeo = ncam + nwarp;
+    double* Ag = Aw + compact_geo0(nk);
     // geometry rows of A: [geom l][knot (k,s)] = f_s C[k][gcol(l) + 14 s];  [geom l][geom l2 <= l] = GG
     for(int e = tid; e < ngeo * (2 * nk + ngeo); e += 128)
     {
@@ -366,16 +368,15 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
             if(l2 > l) continue;
             v = GG[gcol(l) * 14 + gcol(l2)];
         }
-        Aw[(size_t)(2 * nk + l) * lda + c] = v;
+        Ag[(size_t)l * nsh + c] = v;
     }
-    // rows nsh, nsh+1: -J'x over the shared columns
+    // -J'x over the shared columns
     for(int c = tid; c < nsh; c += 128)
     {
         double v;
         if(c < 2 * nk) { const int k = c >> 1, sfc = c & 1; v = (sfc ? fy : fx) * Cs[k * 33 + 28 + sfc]; }
         else v = GG[196 + gcol(c - 2 * nk)];
-        Aw[(size_t)nsh * lda + c] = -v;
-        Aw[(size_t)(nsh + 1) * lda + c] = -v;
+        Ag[(size_t)ngeo * nsh + c] = -v;
     }
     // the frame: B [6][cap], D, gf
     {
@@ -409,15 +410,19 @@ sum_norm_partials_kernel(const double* __restrict__ part, int n, double* __restr
 }
 
 // |J g|^2 over the board rows from the blocks: g_w' [A B'; B D] g_w per observation. part[w] = that. One CTA per item, one
-// entry of the lower triangle of A per thread and step (all loads independent); the per-thread sums are added in a fixed tree
+// entry of the lower triangle of A per thread and step (all loads independent); the per-thread sums are added in a fixed tree.
+// A is in the compact layout (normal.h); each entry is formed as the full layout holds it, the zeros across the two
+// surfaces included
 __global__ void __launch_bounds__(128)
 quadform_items_kernel(DevProblem P, NormalBuffers N, const double* __restrict__ g_full, int Nitems, double* __restrict__ part)
 {
     __shared__ double s_g[168];
     __shared__ double s_red[128];
     const int w = blockIdx.x, tid = threadIdx.x;
-    const int nsh = N.wi_nsh[w], lda = N.wi_lda[w];
+    const int nsh = N.wi_nsh[w], nk = ~N.wi_lda[w];
     const double* A = N.wi_A + N.wi_Aoff[w];
+    const double* Ag = A + compact_geo0(nk);
+    const double fx2 = A[0], fy2 = A[1];
     const int* cols = N.wi_cols + (size_t)w * N.cap;
     const int iframe = P.obs_board[3 * w + 2];
     for(int i = tid; i < nsh; i += 128) s_g[i] = g_full[N.state_index(cols[i])];
@@ -431,7 +436,11 @@ quadform_items_kernel(DevProblem P, NormalBuffers N, const double* __restrict__ 
         while(i * (i + 1) / 2 > e) i--;
         while((i + 1) * (i + 2) / 2 <= e) i++;
         const int j = e - i * (i + 1) / 2;
-        const double v = A[(size_t)i * lda + j] * s_g[i] * s_g[j];
+        double a;
+        if(i >= 2 * nk)     a = Ag[(size_t)(i - 2 * nk) * nsh + j];
+        else if((i ^ j) & 1) a = 0.;
+        else                a = __dmul_rn(i & 1 ? fy2 : fx2, A[2 + (i >> 1) * ((i >> 1) + 1) / 2 + (j >> 1)]);
+        const double v = a * s_g[i] * s_g[j];
         q += i == j ? v : 2. * v;
     }
     // frame: 2 g_f' B g_s + g_f' D g_f

@@ -933,7 +933,8 @@ bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& o
     }
     compact_scan_kernel<<<1, 1024, 0, s>>>(N);
     (*nlaunch)++;
-    if(N.det_available && !N.fused && !normal_det_item_offsets(dp, N, s, nlaunch)) return false;
+    // (the fused evaluation placed the board observations' blocks at their fixed slots)
+    if(N.det_available && !normal_det_item_offsets(dp, N, w0, s, nlaunch)) return false;
     if(copy_sizes) MB200_CUDA_CHECK(cudaMemcpyAsync(N.h_stat, N.stat, 4 * sizeof(int), cudaMemcpyDeviceToHost, s));
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;

@@ -11,6 +11,21 @@ namespace mb200 {
 constexpr int kYld = 68;              // row stride of the panels of Ypan (doubles)
 constexpr int kYpanel = 6 * kYld;     // one (group, block) panel
 
+// The compact block of a board observation of the fused evaluation. Its local columns are numbered as in the full layout:
+// knot k is columns 2k (x surface) and 2k+1 (y surface), then the nsh - 2 nk geometry columns (camera r,t | warp). The
+// knot x knot part of the Gram matrix is fx^2 M on the x surface, fy^2 M on the y surface and zero across, M = Dk'Dk (nk x
+// nk), so M is stored once and the two gradient rows of the full layout (equal) once. In doubles:
+//   [0] fx*fx, [1] fy*fy
+//   [2 ..)                   M, packed lower triangle: M[k1][k2], k2 <= k1, at 2 + k1 (k1 + 1) / 2 + k2
+//   [compact_geo0(nk) ..)    rows 2nk .. nsh-1 of the full layout, nsh doubles each (columns 0 .. row valid)
+//   then                     -J'x over the nsh columns: rows nsh and nsh+1 of the full layout
+// The entries of the full layout are (fx*fx) * M[k1][k2] and (fy*fy) * M[k1][k2], rounded as written.
+constexpr int kCompactMaxKnots = 64;  // knots of one observation's patch (the fused kernel gives up beyond)
+constexpr int kCompactMaxGeo = 8;     // geometry columns: camera extrinsics 6, board warp 2
+__host__ __device__ constexpr int compact_geo0(int nk) { return 2 + nk * (nk + 1) / 2; }
+// the fixed slot of one board observation in the pool (the fused kernel writes board w at w * kCompactSlot)
+constexpr long long kCompactSlot = compact_geo0(kCompactMaxKnots) + (kCompactMaxGeo + 1) * (2 * kCompactMaxKnots + kCompactMaxGeo);
+
 struct NormalBuffers
 {
     double* S;        // [ldS][ldS] row-major, lower: reduced normal matrix over the ACTIVE shared unknowns
@@ -56,10 +71,12 @@ struct NormalBuffers
     cudaStream_t s_side[2];               // forked streams of the Gram kernel's size classes (owned by the workspace)
     cudaEvent_t  ev_fork, ev_join[2];
     int     capA;         // most local columns (incl. the two gradient rows) an item may have in the A pool
-    double* wi_A;         // pool of per-item Gram blocks over the shared columns, [lda][lda] row-major, lower triangle
+    double* wi_A;         // pool of per-item Gram blocks over the shared columns, in one of two layouts (wi_lda says which):
+                          //  full    [lda][lda] row-major, lower triangle; rows nsh, nsh+1: -J'x over the item's shared columns
+                          //  compact the board observations of the fused evaluation (fused_eval.cu); see kCompactSlot
     long long* wi_Aoff;   // [Nwi] offset of each item's block in the pool (doubles)
     long long  A_pool;    // pool size (doubles)
-    int*    wi_lda;       // [Nwi] nsh + 2 rounded up to even; rows nsh, nsh+1: -J'x over the item's shared columns
+    int*    wi_lda;       // [Nwi] full layout: nsh + 2 rounded up to even. Compact layout: ~nk (< 0)
     unsigned short* wi_ccol;    // [Nwi][capA] compact index of each local column (increasing); then n_c, n_c+1
     unsigned char*  wi_segoff;  // [Nwi][nblk_max+1] first local column of each 64-column block of S
     int     nblk_max;     // ldS_max / 64
@@ -115,7 +132,8 @@ bool normal_det_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers
                        double lambda, cudaStream_t s, int* nlaunch);
 bool normal_det_item_prepare(const DevProblem& dp, NormalBuffers& N, cudaStream_t s, int* nlaunch);   // after the compaction
 void normal_det_to_clear(const NormalBuffers& N, WordFill* f);   // before item_prepare: what it and det_finish expect zeroed
-bool normal_det_item_offsets(const DevProblem& dp, NormalBuffers& N, cudaStream_t s, int* nlaunch);   // before it
+// before it: the full-layout blocks of items [first, Nwi), behind the `first` fixed compact slots
+bool normal_det_item_offsets(const DevProblem& dp, NormalBuffers& N, int first, cudaStream_t s, int* nlaunch);
 size_t normal_det_part_scratch_doubles(int nblk_max);
 int normal_det_part_arrive_ints(int nblk_max);
 size_t normal_det_packed_doubles(int nblk_max);

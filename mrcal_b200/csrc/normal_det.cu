@@ -17,7 +17,8 @@
 //                                 6x64 panels per 64-column block the group reaches (zeros where it does
 //                                 not), -inv(L_D) gf as the column that forms the right-hand side
 //   schur_tiles_kernel            one CTA per tile. Phase A: the items' Gram blocks, each warp owning the
-//                                 tile rows = its number (mod 8). Phase S: the panels of the groups that
+//                                 tile rows = its number (mod 8); a compact block (a fused board observation,
+//                                 normal.h) brings a knot row's own surface only. Phase S: the panels of the groups that
 //                                 reach both block r and block c, stacked along K, through DMMA 8x8x4;
 //                                 operands staged with cp.async, double buffered.
 //   reg_blocks_kernel             the regularization rows: one thread per knot (or per unknown), the
@@ -45,14 +46,15 @@ constexpr int kChunkGroups = 6; // phase S: groups per K chunk (36 rows); two CT
 
 }  // namespace
 
-// exclusive scan of lda^2 over the items: one CTA
+// exclusive scan of lda^2 over the items [first, Nwi), behind the fixed slots of the first `first` (the board observations
+// of the fused evaluation, which place their compact blocks themselves): one CTA
 __global__ void __launch_bounds__(1024)
-item_offsets_kernel(NormalBuffers N, int Nwi)
+item_offsets_kernel(NormalBuffers N, int first, int Nwi)
 {
     __shared__ long long s_scan[1024];
     const int tid = threadIdx.x;
-    const int per = (Nwi + 1023) / 1024;
-    const int lo = tid * per, hi = min(lo + per, Nwi);
+    const int per = (Nwi - first + 1023) / 1024;
+    const int lo = first + tid * per, hi = min(lo + per, Nwi);
     long long cnt = 0;
     for(int w = lo; w < hi; w++)
     {
@@ -69,13 +71,13 @@ item_offsets_kernel(NormalBuffers N, int Nwi)
         s_scan[tid] += v;
         __syncthreads();
     }
-    long long base = s_scan[tid] - cnt;
+    long long base = (long long)first * kCompactSlot + s_scan[tid] - cnt;
     for(int w = lo; w < hi; w++)
     {
         N.wi_Aoff[w] = base;
         base += (long long)N.wi_lda[w] * N.wi_lda[w];
     }
-    if(tid == 1023 && s_scan[1023] > N.A_pool) N.stat[3] = 1;   // pool too small: the host takes the other path
+    if(tid == 1023 && (long long)first * kCompactSlot + s_scan[1023] > N.A_pool) N.stat[3] = 1;   // pool too small: the host takes the other path
 }
 
 // After the compaction: compact column of each local column, the two gradient rows, the first local column of
@@ -240,8 +242,9 @@ static_assert(sizeof(TileCommon) % 16 == 0, "the tile and the staging buffers be
 struct alignas(16) TileSmemA
 {
     double tile[TB * TLD];
-    int    meta[kChunkItems][4];           // a0 | na<<8,  b0 | nb<<8,  lda, (unused)
+    int    meta[kChunkItems][4];           // a0 | na<<8,  b0 | nb<<8,  lda (< 0: compact layout, ~nk),  nsh
     long long base[kChunkItems];
+    double f2[kChunkItems][2];             // compact layout: fx*fx, fy*fy
     unsigned char rl[kChunkItems][TB + 4]; // tile row of each local row
     unsigned char cl[kChunkItems][TB + 4]; // tile column of each local column
 };
@@ -498,8 +501,12 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
                 if(b0 > b1) b0 = b1;
                 sa.meta[tid][0] = a0 | ((a1 - a0) << 8);
                 sa.meta[tid][1] = b0 | ((b1 - b0) << 8);
-                sa.meta[tid][2] = N.wi_lda[w];
-                sa.base[tid] = N.wi_Aoff[w];
+                const int lda = N.wi_lda[w];
+                const long long base = N.wi_Aoff[w];
+                sa.meta[tid][2] = lda;
+                sa.meta[tid][3] = nsh;
+                sa.base[tid] = base;
+                if(lda < 0) { sa.f2[tid][0] = __ldg(N.wi_A + base); sa.f2[tid][1] = __ldg(N.wi_A + base + 1); }
             }
             __syncthreads();
             for(int e = tid; e < nch * 2 * TB; e += 256)
@@ -521,8 +528,12 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
             }
             __syncthreads();
             // ---- accumulate. Warp `warp` owns the tile rows = warp (mod 8): no two warps ever touch the same entry, and
-            // every entry sees its contributions in item order. A "task" is one owned row of one item (<= 64 values,
-            // two per lane); tasks are taken 8 at a time so that their loads are in flight together
+            // every entry sees its nonzero contributions in item order. A "task" is one owned row of one item (<= 64 values,
+            // two per lane). A knot row of a compact block holds its surface's columns only: lane j takes knot k2 =
+            // ceil((b0 - s) / 2) + j of surface s and adds f_s^2 M[k1][k2] at column 2 k2 + s; the zeros across the
+            // surfaces are not added (those entries of S start at +0 and receive only zeros). Rows of consecutive tile rows
+            // go to different warps, so the few rows an item brings to a tile are spread over the warps. Tasks are taken 4
+            // at a time so that their loads are in flight together
             {
                 int ti = -1;
                 unsigned cur0 = 0, cur1 = 0;
@@ -530,11 +541,12 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
                 while(!exhausted || cur0 || cur1)
                 {
                     // every task is decoded ONCE: where its values are (an element offset into the pool), where they go
-                    // in the tile, which of the lane's two columns exist. The kernel is bound by the instructions it
-                    // issues here, not by the latency of the loads: 4 tasks in flight are enough
+                    // in the tile, which of the lane's two columns exist, the factor of a knot row. The kernel is bound by
+                    // the instructions it issues here, not by the latency of the loads: 4 tasks in flight are enough
                     constexpr int NT = 4;
                     unsigned src[NT];
                     int dst0[NT], dst1[NT];
+                    double scl[NT];
                     unsigned have = 0;   // bit 2u: column `lane` of task u exists, bit 2u+1: column lane+32
                     int cnt = 0;
 #pragma unroll
@@ -552,18 +564,37 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
                         }
                         if(cur0) { item = ti; lrow = __ffs(cur0) - 1; cur0 &= cur0 - 1; cnt++; }
                         else if(cur1) { item = ti; lrow = 32 + __ffs(cur1) - 1; cur1 &= cur1 - 1; cnt++; }
-                        src[u] = 0u; dst0[u] = dst1[u] = 0;
+                        src[u] = 0u; dst0[u] = dst1[u] = 0; scl[u] = 1.;
                         if(item >= 0)
                         {
                             const int a = (sa.meta[item][0] & 255) + lrow;
                             const int b0 = sa.meta[item][1] & 255, nb = sa.meta[item][1] >> 8;
-                            // lower triangle of the item's block: local column <= local row (always true off the diagonal tiles)
-                            const bool p0 = lane < nb && b0 + lane <= a, p1 = lane + 32 < nb && b0 + lane + 32 <= a;
-                            have |= (p0 ? 1u : 0u) << (2 * u) | (p1 ? 2u : 0u) << (2 * u);
-                            src[u] = (unsigned)(sa.base[item] + (long long)a * sa.meta[item][2] + b0 + lane);
+                            const int lda = sa.meta[item][2];
+                            const int nk = lda < 0 ? ~lda : 0;
                             const int trow = (int)sa.rl[item][lrow] * TLD;
-                            dst0[u] = trow + (p0 ? sa.cl[item][lane] : 0);
-                            dst1[u] = trow + (p1 ? sa.cl[item][lane + 32] : 0);
+                            if(lda >= 0 || a >= 2 * nk)
+                            {
+                                // a row as stored: the full layout, or a geometry / gradient row of a compact block (nsh wide;
+                                // the two gradient rows are one stored row)
+                                const int nsh = sa.meta[item][3];
+                                const long long row = lda >= 0 ? (long long)a * lda : compact_geo0(nk) + (long long)(min(a, nsh) - 2 * nk) * nsh;
+                                // lower triangle of the item's block: local column <= local row (always true off the diagonal tiles)
+                                const bool p0 = lane < nb && b0 + lane <= a, p1 = lane + 32 < nb && b0 + lane + 32 <= a;
+                                have |= (p0 ? 1u : 0u) << (2 * u) | (p1 ? 2u : 0u) << (2 * u);
+                                src[u] = (unsigned)(sa.base[item] + row + b0 + lane);
+                                dst0[u] = trow + (p0 ? sa.cl[item][lane] : 0);
+                                dst1[u] = trow + (p1 ? sa.cl[item][lane + 32] : 0);
+                            }
+                            else
+                            {
+                                const int k1 = a >> 1, sfc = a & 1;
+                                const int k2 = ((b0 + 1 - sfc) >> 1) + lane, col = 2 * k2 + sfc - b0;
+                                const bool p = k2 <= k1 && col < nb;
+                                have |= (p ? 1u : 0u) << (2 * u);
+                                src[u] = (unsigned)(sa.base[item] + 2 + k1 * (k1 + 1) / 2 + k2);
+                                dst0[u] = trow + (p ? sa.cl[item][col] : 0);
+                                scl[u] = sa.f2[item][sfc];
+                            }
                         }
                     }
                     if(cnt == 0) break;
@@ -577,7 +608,8 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
 #pragma unroll
                     for(int u = 0; u < NT; u++)
                     {
-                        if((have >> (2 * u)) & 1u) sa.tile[dst0[u]] += v0[u];
+                        // (the product is rounded on its own, as the full layout's entries were: no contraction into the sum)
+                        if((have >> (2 * u)) & 1u) sa.tile[dst0[u]] += __dmul_rn(scl[u], v0[u]);
                         if((have >> (2 * u + 1)) & 1u) sa.tile[dst1[u]] += v1[u];
                         // two items may bring the same tile entry to DIFFERENT lanes of this warp: the additions of one task
                         // are done (and visible to the warp) before those of the next
@@ -901,11 +933,11 @@ backsub_panels_kernel(NormalBuffers N, const double* __restrict__ sol, double* _
     }
 }
 
-bool normal_det_item_offsets(const DevProblem& dp, NormalBuffers& N, cudaStream_t s, int* nlaunch)
+bool normal_det_item_offsets(const DevProblem& dp, NormalBuffers& N, int first, cudaStream_t s, int* nlaunch)
 {
     const int Nwi = dp.Nobs_board + dp.Nobs_point;
-    if(Nwi == 0) return true;
-    item_offsets_kernel<<<1, 1024, 0, s>>>(N, Nwi);
+    if(Nwi - first <= 0) return true;
+    item_offsets_kernel<<<1, 1024, 0, s>>>(N, first, Nwi);
     (*nlaunch)++;
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;

@@ -206,7 +206,9 @@ static bool build_workspace(mrcal_b200_problem* P)
         auto even = [](int v) { return (v + 1) & ~1; };
         const int lda_board = even(std::min(N.capA, (L.splined ? 160 : L.Nintr_state + 8) + 2));
         const int lda_point = even(std::min(N.capA, (L.splined ? 2 * 16 + 4 + 6 : L.Nintr_state + 6) + 2));
-        N.A_pool = (long long)L.d.Nobs_board * lda_board * lda_board + (long long)L.d.Nobs_point * lda_point * lda_point;
+        // (a splined model's boards may also take the fused evaluation's fixed compact slots)
+        const long long board_block = L.splined ? std::max((long long)lda_board * lda_board, kCompactSlot) : (long long)lda_board * lda_board;
+        N.A_pool = (long long)L.d.Nobs_board * board_block + (long long)L.d.Nobs_point * lda_point * lda_point;
         // (schur_tiles_kernel addresses the pool with 32-bit element offsets: 4 G doubles = 34 GB, more than a problem this
         // library's other buffers would leave room for)
         if(N.A_pool >= (1ll << 32)) N.det_available = false;
@@ -231,27 +233,8 @@ static bool build_workspace(mrcal_b200_problem* P)
     N.fused = N.det_available && L.splined && !L.sel.do_optimize_intrinsics_core && L.sel.do_optimize_intrinsics_distortions &&
               L.sel.do_optimize_frames && L.i_frame0 >= 0 && L.d.Nobs_board > 0 && L.d.W * L.d.H <= 128 &&
               getenv("MRCAL_B200_NO_FUSED") == nullptr;
-    if(N.fused)
-    {
-        // fixed places in the pool: the observation's column count is only known inside the kernel that fills its block
-        auto even = [](int v) { return (v + 1) & ~1; };
-        const int lda_board = even(std::min(N.capA, 160 + 2));
-        const int lda_point = even(std::min(N.capA, 2 * 16 + 4 + 6 + 2));
-        std::vector<long long> off(Nwi);
-        std::vector<int> lda(Nwi);
-        for(int w = 0; w < Nwi; w++)
-        {
-            const bool board = w < L.d.Nobs_board;
-            lda[w] = board ? lda_board : lda_point;
-            off[w] = board ? (long long)w * lda_board * lda_board
-                           : (long long)L.d.Nobs_board * lda_board * lda_board + (long long)(w - L.d.Nobs_board) * lda_point * lda_point;
-        }
-        ok = A.alloc(&N.norm_part, L.d.Nobs_board, true) && A.alloc(&N.qf_part, L.d.Nobs_board, true);
-        if(!ok) return false;
-        MB200_CUDA_CHECK(cudaMemcpyAsync(N.wi_Aoff, off.data(), Nwi * sizeof(long long), cudaMemcpyHostToDevice, P->stream));
-        MB200_CUDA_CHECK(cudaMemcpyAsync(N.wi_lda, lda.data(), Nwi * sizeof(int), cudaMemcpyHostToDevice, P->stream));
-        MB200_CUDA_CHECK(cudaStreamSynchronize(P->stream));   // the staging vectors go out of scope
-    }
+    // (the fused kernel places each board observation's block itself: fixed slots of kCompactSlot doubles, normal.h)
+    if(N.fused && !(A.alloc(&N.norm_part, L.d.Nobs_board, true) && A.alloc(&N.qf_part, L.d.Nobs_board, true))) return false;
     MB200_CUDA_CHECK(cudaEventCreateWithFlags(&N.ev_fork, cudaEventDisableTiming));
     for(int k = 0; k < 2; k++)
     {
@@ -465,12 +448,16 @@ static bool solver_selfcheck(mrcal_b200_problem* P, int which, double lambda)
     {
         if(!normal_selfcheck(P->dp, N, P->op[which], P->d_rowptr, lambda, s, nl)) return false;   // det vs atomic, on the stored Jacobian
         if(!normal_finish(P->dp, N, P->op[which], P->d_rowptr, lambda, s, nl, false) || !grab(Sj)) return false;
+        // the lower triangle and the right-hand side row: what the assembly writes (the rest of S holds whatever the
+        // buffer held before)
         double scale = 0., worst = 0.;
-        for(size_t k = 0; k < Sj.size(); k++)
-        {
-            if(fabs(Sj[k]) > scale) scale = fabs(Sj[k]);
-            if(!(fabs(Sj[k] - Sf[k]) <= worst)) worst = fabs(Sj[k] - Sf[k]);
-        }
+        for(int i = 0; i <= n; i++)
+            for(int j = 0; j < (i < n ? i + 1 : n); j++)
+            {
+                const size_t k = (size_t)i * n + j;
+                if(fabs(Sj[k]) > scale) scale = fabs(Sj[k]);
+                if(!(fabs(Sj[k] - Sf[k]) <= worst)) worst = fabs(Sj[k] - Sf[k]);
+            }
         agree = worst <= 1e-9 * scale;
         if(!agree)
             fprintf(stderr, "mrcal_b200: WARNING: the fused evaluation disagrees with the stored-Jacobian path (|diff| %g of %g): "
@@ -479,24 +466,8 @@ static bool solver_selfcheck(mrcal_b200_problem* P, int which, double lambda)
     N.selfchecked = true;
     if(agree)
     {
-        // back to the fused path: restore the fixed placement of the blocks and redo the evaluation's blocks
+        // back to the fused path: redo the evaluation's blocks (the fused kernel puts them back in their fixed slots)
         N.fused = true;
-        const Layout& L = P->L;
-        auto even = [](int v) { return (v + 1) & ~1; };
-        const int lda_board = even(std::min(N.capA, 160 + 2)), lda_point = even(std::min(N.capA, 2 * 16 + 4 + 6 + 2));
-        const int Nwi = L.d.Nobs_board + L.d.Nobs_point;
-        std::vector<long long> off(Nwi);
-        std::vector<int> lda(Nwi);
-        for(int w = 0; w < Nwi; w++)
-        {
-            const bool board = w < L.d.Nobs_board;
-            lda[w] = board ? lda_board : lda_point;
-            off[w] = board ? (long long)w * lda_board * lda_board
-                           : (long long)L.d.Nobs_board * lda_board * lda_board + (long long)(w - L.d.Nobs_board) * lda_point * lda_point;
-        }
-        MB200_CUDA_CHECK(cudaMemcpyAsync(N.wi_Aoff, off.data(), Nwi * sizeof(long long), cudaMemcpyHostToDevice, s));
-        MB200_CUDA_CHECK(cudaMemcpyAsync(N.wi_lda, lda.data(), Nwi * sizeof(int), cudaMemcpyHostToDevice, s));
-        MB200_CUDA_CHECK(cudaStreamSynchronize(s));
         const EvalBuffers& o = P->op[which];
         MB200_CUDA_CHECK(cudaMemsetAsync(o.norm2, 0, sizeof(double), s));
         if(!normal_clear_marks(N, s) || !launch_unpack_state(P->dp, o.p, s, nl) ||
@@ -885,15 +856,10 @@ extern "C" void mrcal_b200_default_solver_parameters(mrcal_b200_solver_parameter
     p->trustregion_threshold = 0.;
 }
 
-extern "C" bool mrcal_b200_problem_reduced_system(mrcal_b200_problem_t* P, double lambda, int* n_reduced,
-                                                  double* S_out, double* g_reduced, double* g_full)
+// S, g', g_full of the assembly that just ran, to the host
+static bool download_reduced_system(mrcal_b200_problem_t* P, double* S_out, double* g_reduced, double* g_full)
 {
-    if(!build_workspace(P)) return false;
     NormalBuffers& N = P->ws->N;
-    if(n_reduced) *n_reduced = N.n_r;
-    if(S_out == nullptr && g_reduced == nullptr && g_full == nullptr) return true;
-    if(!problem_evaluate(P, P->cur, true, true)) return false;
-    if(!normal_assemble(P->dp, N, P->op[P->cur], P->d_rowptr, lambda, P->stream, &P->launches)) return false;
     // the device holds the system over the active unknowns only; expand to reduced numbering here
     // (inactive rows/columns come out as zero: they are not part of the coupled system)
     std::vector<double> Sc((size_t)N.n_c * N.n_c), gc(N.n_c);
@@ -916,6 +882,46 @@ extern "C" bool mrcal_b200_problem_reduced_system(mrcal_b200_problem_t* P, doubl
         if(S_out) for(int b = 0; b <= a; b++) S_out[(size_t)cinv[a] * N.n_r + cinv[b]] = Sc[(size_t)a * N.n_c + b];
     }
     return true;
+}
+
+extern "C" bool mrcal_b200_problem_reduced_system(mrcal_b200_problem_t* P, double lambda, int* n_reduced,
+                                                  double* S_out, double* g_reduced, double* g_full)
+{
+    if(!build_workspace(P)) return false;
+    NormalBuffers& N = P->ws->N;
+    if(n_reduced) *n_reduced = N.n_r;
+    if(S_out == nullptr && g_reduced == nullptr && g_full == nullptr) return true;
+    if(!problem_evaluate(P, P->cur, true, true)) return false;
+    if(!normal_assemble(P->dp, N, P->op[P->cur], P->d_rowptr, lambda, P->stream, &P->launches)) return false;
+    return download_reduced_system(P, S_out, g_reduced, g_full);
+}
+
+extern "C" bool mrcal_b200_problem_reduced_system_fused(mrcal_b200_problem_t* P, double lambda, int* n_reduced,
+                                                        double* S_out, double* g_reduced, double* g_full)
+{
+    if(!build_workspace(P)) return false;
+    NormalBuffers& N = P->ws->N;
+    if(n_reduced) *n_reduced = N.n_r;
+    if(!N.fused) { set_error("reduced_system_fused: this problem does not take the fused evaluation"); return false; }
+    if(S_out == nullptr && g_reduced == nullptr && g_full == nullptr) return true;
+    // what an optimize() step does: the boards' blocks from the fused evaluation, the other rows from their Jacobian
+    cudaStream_t s = P->stream;
+    int* nl = &P->launches;
+    const EvalBuffers& o = P->op[P->cur];
+    WordFill clear;
+    clear.add(o.norm2, sizeof(double));
+    normal_marks_to_clear(N, &clear);
+    if(!fill_words(clear, s) || !launch_unpack_state(P->dp, o.p, s, nl) || !launch_fused_boards(P->dp, N, o, N.norm_part, s, nl) ||
+       !launch_evaluate(P->dp, o, true, nullptr, s, nl, false) || !normal_prepare(P->dp, N, o, s, nl, true)) return false;
+    MB200_CUDA_CHECK(cudaStreamSynchronize(s));
+    if(!normal_adopt_sizes(N)) return false;
+    if(N.h_stat[3] != 0 || !N.det)
+    {
+        set_error("reduced_system_fused: the fused evaluation's blocks do not fit this problem");
+        return false;
+    }
+    if(!normal_finish(P->dp, N, o, P->d_rowptr, lambda, s, nl, true)) return false;
+    return download_reduced_system(P, S_out, g_reduced, g_full);
 }
 
 extern "C" bool mrcal_b200_problem_optimize(mrcal_b200_problem_t* P, const mrcal_b200_solver_parameters_t* parameters,
