@@ -140,6 +140,20 @@ typedef struct
     int    stype, itype, xtype, dtype, sorted, packed;
 } mrcal_b200_sparse_t;
 
+// replaces image.h:68-80 (the two image types stereo.h uses): w x h pixels, rows stride BYTES apart
+typedef struct
+{
+    union { struct { int w, h; }; struct { int width, height; }; struct { int cols, rows; }; };
+    int stride;
+    uint16_t* data;
+} mrcal_image_uint16_t;
+typedef struct
+{
+    union { struct { int w, h; }; struct { int width, height; }; struct { int cols, rows; }; };
+    int stride;
+    double* data;
+} mrcal_image_double_t;
+
 ////////////////////////////////////////////////////////////////////////////////
 // Part 1b. Lens-model description (host only)
 ////////////////////////////////////////////////////////////////////////////////
@@ -309,6 +323,58 @@ bool mrcal_project(mrcal_point2_t* q, mrcal_point3_t* dq_dp, double* dq_dintrins
 // into the rays of mrcal_observation_point_triangulated_t (mrcal-pywrap.c:1383-1401)
 bool mrcal_unproject(mrcal_point3_t* out, const mrcal_point2_t* q, int N,
                      const mrcal_lensmodel_t* lensmodel, const double* intrinsics);
+
+// Stereo (replaces stereo.h:15-173, stereo.c:19-972, 1242-1417). Host buffers in and out, as in the reference.
+// The geometry is host code; the maps and the ranges are computed on the device, one thread per element.
+//
+// replaces stereo.h:15-31: the resolution of a rectified view (rectification model LATLON, LONLAT or PINHOLE).
+// pixels_per_deg_* < 0 asks for that multiple of camera 0's resolution at (az0, el0), which takes one device
+// projection; LATLON and LONLAT then fit a whole number of pixels into the field of view
+bool mrcal_rectified_resolution(double* pixels_per_deg_az, double* pixels_per_deg_el,
+                                const mrcal_lensmodel_t* lensmodel, const double* intrinsics,
+                                const mrcal_point2_t* azel_fov_deg, const mrcal_point2_t* azel0_deg,
+                                const double* R_cam0_rect0, const mrcal_lensmodel_type_t rectification_model_type);
+// replaces stereo.h:33-80: the rectified system of a stereo pair: imager (Naz, Nel), fxycxy, rt_rect0_ref and the
+// baseline. Rectification model LATLON or PINHOLE; central models only (CAHVORE with E = 0). Of the autodetections
+// only az0's is supported
+bool mrcal_rectified_system2(unsigned int* imagersize_rectified, double* fxycxy_rectified, double* rt_rect0_ref,
+                             double* baseline, double* pixels_per_deg_az, double* pixels_per_deg_el,
+                             mrcal_point2_t* azel_fov_deg, mrcal_point2_t* azel0_deg,
+                             const double az_edge_margin_deg,
+                             const mrcal_lensmodel_t* lensmodel0, const double* intrinsics0,
+                             const double* rt_cam0_ref, const double* rt_cam1_ref,
+                             const mrcal_lensmodel_type_t rectification_model_type,
+                             bool az0_deg_autodetect, bool el0_deg_autodetect,
+                             bool az_fov_deg_autodetect, bool el_fov_deg_autodetect);
+// replaces stereo.h:82-117: the legacy form, az_edge_margin_deg = 10
+bool mrcal_rectified_system(unsigned int* imagersize_rectified, double* fxycxy_rectified, double* rt_rect0_ref,
+                            double* baseline, double* pixels_per_deg_az, double* pixels_per_deg_el,
+                            mrcal_point2_t* azel_fov_deg, mrcal_point2_t* azel0_deg,
+                            const mrcal_lensmodel_t* lensmodel0, const double* intrinsics0,
+                            const double* rt_cam0_ref, const double* rt_cam1_ref,
+                            const mrcal_lensmodel_type_t rectification_model_type,
+                            bool az0_deg_autodetect, bool el0_deg_autodetect,
+                            bool az_fov_deg_autodetect, bool el_fov_deg_autodetect);
+// replaces stereo.h:119-135: rectification_maps (2, Nel, Naz, 2) float32: for each camera and rectified pixel, the
+// pixel of that camera that sees the same ray
+bool mrcal_rectification_maps(float* rectification_maps,
+                              const mrcal_lensmodel_t* lensmodel0, const double* intrinsics0, const double* r_cam0_ref,
+                              const mrcal_lensmodel_t* lensmodel1, const double* intrinsics1, const double* r_cam1_ref,
+                              const mrcal_lensmodel_type_t rectification_model_type,
+                              const double* fxycxy_rectified, const unsigned int* imagersize_rectified,
+                              const double* r_rect0_ref);
+// replaces stereo.h:137-152: range[N] of disparities at rectified pixels qrect0; 0 where d <= 0, d is outside
+// [disparity_min, disparity_max] or the range is not finite
+bool mrcal_stereo_range_sparse(double* range, const double* disparity, const mrcal_point2_t* qrect0, const int N,
+                               const double disparity_min, const double disparity_max,
+                               const mrcal_lensmodel_type_t rectification_model_type,
+                               const double* fxycxy_rectified, const double baseline);
+// replaces stereo.h:154-170: the same for a whole disparity image of scaled uint16 values
+bool mrcal_stereo_range_dense(mrcal_image_double_t* range, const mrcal_image_uint16_t* disparity_scaled,
+                              const uint16_t disparity_scale,
+                              const uint16_t disparity_scaled_min, const uint16_t disparity_scaled_max,
+                              const mrcal_lensmodel_type_t rectification_model_type,
+                              const double* fxycxy_rectified, const double baseline);
 
 // One evaluation of the cost function at the given (unpacked) seed:
 //   b_packed <- packed state, x <- residuals, Jt <- CSR Jacobian dx/db_packed
@@ -573,6 +639,22 @@ bool mrcal_b200_projection_diff(double* Rt10, double* difflen, double* diff,
                                 const mrcal_lensmodel_t* lensmodels, const double* intrinsics,
                                 const double* uncertainties, const double* focus_center, double focus_radius,
                                 bool fit_Rt10);
+
+// The point cloud of disparities in rectified camera-0 coordinates, as mrcal.stereo_unproject() computes it
+// (mrcal/stereo.py:1453-1607) in one pass on the device: p[k] = range[k] * normalize(unproject_rect(qrect0[k])),
+// (0,0,0) where the range is 0. Exactly one source of ranges is given:
+// - disparity_scaled: a whole image, as mrcal_stereo_range_dense() reads it; qrect0 is its pixel grid, p is (h, w)
+// - disparity [N]: as mrcal_stereo_range_sparse() reads it, with disparity_min, disparity_max
+// - ranges [N]: given
+// With the last two, qrect0 [N], or NULL for the pixel grid of width W (N a multiple of W). range [N] receives the
+// ranges (may be NULL). False + mrcal_b200_last_error() on refusal or failure
+bool mrcal_b200_stereo_unproject(mrcal_point3_t* p, double* range,
+                                 const mrcal_image_uint16_t* disparity_scaled, uint16_t disparity_scale,
+                                 uint16_t disparity_scaled_min, uint16_t disparity_scaled_max,
+                                 const double* disparity, const double* ranges, const mrcal_point2_t* qrect0,
+                                 int N, int W, double disparity_min, double disparity_max,
+                                 mrcal_lensmodel_type_t rectification_model_type,
+                                 const double* fxycxy_rectified, double baseline);
 
 // Timing hook for benchmarks: run N cost-function evaluations (residuals +
 // Jacobian) at the current state back to back, return the mean device time per

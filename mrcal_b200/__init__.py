@@ -21,6 +21,9 @@ from .api import (  # noqa: F401
 from .seeding import (  # noqa: F401
     seed_stereographic, estimate_monocular_calobject_poses_Rt_tocam, estimate_joint_frame_poses,
 )
+from .stereo import (  # noqa: F401
+    rectified_resolution, rectified_system, rectification_maps, stereo_range, stereo_unproject,
+)
 from .cameramodel import cameramodel, CameramodelParseException  # noqa: F401
 from ._capi import lib as _lib
 

@@ -47,6 +47,16 @@ class Sparse(C.Structure):
                 ("dtype", C.c_int), ("sorted", C.c_int), ("packed", C.c_int)]
 
 
+class ImageUint16(C.Structure):
+    """mrcal_image_uint16_t (image.h:68-80): w, h in pixels, stride in bytes"""
+    _fields_ = [("w", C.c_int), ("h", C.c_int), ("stride", C.c_int), ("data", C.c_void_p)]
+
+
+class ImageDouble(C.Structure):
+    """mrcal_image_double_t (image.h:68-80)"""
+    _fields_ = [("w", C.c_int), ("h", C.c_int), ("stride", C.c_int), ("data", C.c_void_p)]
+
+
 class SolverParameters(C.Structure):
     _fields_ = [("max_iterations", C.c_int),
                 ("trustregion0", C.c_double),
@@ -112,6 +122,8 @@ EXPORTED_SYMBOLS = (
     "mrcal_b200_problem_drt_cross_reprojection__dbpacked",
     "mrcal_b200_problem_projection_uncertainty",
     "mrcal_b200_implied_Rt10__from_unprojections", "mrcal_b200_projection_diff",
+    "mrcal_rectified_resolution", "mrcal_rectified_system2", "mrcal_rectified_system", "mrcal_rectification_maps",
+    "mrcal_stereo_range_sparse", "mrcal_stereo_range_dense", "mrcal_b200_stereo_unproject",
     "mrcal_b200_nccl_get_unique_id", "mrcal_b200_nccl_comm_init", "mrcal_b200_nccl_comm_destroy",
     "mrcal_b200_problem_set_sharding",
     "mrcal_b200_factorization_create", "mrcal_b200_factorization_destroy",
@@ -163,6 +175,17 @@ lib.mrcal_b200_projection_diff.restype = C.c_bool
 lib.mrcal_b200_projection_diff.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
                                            C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_double, C.c_bool]
+for _n in ["mrcal_rectified_resolution", "mrcal_rectified_system2", "mrcal_rectified_system", "mrcal_rectification_maps",
+           "mrcal_stereo_range_sparse", "mrcal_stereo_range_dense", "mrcal_b200_stereo_unproject"]:
+    getattr(lib, _n).restype = C.c_bool
+lib.mrcal_rectified_system2.argtypes = [C.c_void_p] * 8 + [C.c_double] + [C.c_void_p] * 4 + [C.c_int] + [C.c_bool] * 4
+lib.mrcal_stereo_range_sparse.argtypes = [C.c_void_p] * 3 + [C.c_int, C.c_double, C.c_double, C.c_int, C.c_void_p,
+                                                               C.c_double]
+lib.mrcal_stereo_range_dense.argtypes = [C.c_void_p, C.c_void_p, C.c_uint16, C.c_uint16, C.c_uint16, C.c_int,
+                                         C.c_void_p, C.c_double]
+lib.mrcal_b200_stereo_unproject.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint16, C.c_uint16, C.c_uint16,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_double,
+                                            C.c_double, C.c_int, C.c_void_p, C.c_double]
 lib.mrcal_b200_factorization_create_from_last_callback.restype = C.c_void_p
 lib.mrcal_b200_csr_create.restype = C.c_void_p
 lib.mrcal_b200_csr_destroy.restype = None
