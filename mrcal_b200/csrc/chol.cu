@@ -1,24 +1,25 @@
-// Kernel family 2b: dense Cholesky factorization and triangular solves of the
-// reduced (camera) normal equations, fp64, on the DMMA (fp64 tensor) pipe.
+// Kernel family 2b: what the dense Cholesky needs besides its two persistent kernels (chol_dataflow.cu: the
+// factorization up to n = 8192, and the backward substitution of one right-hand side):
+//   - the factorization above n = 8192, where a chain of short kernels per 64 columns is faster than the persistent
+//     kernel (DESIGN section 9). A two-level blocked right-looking algorithm:
 //
-// Stands in for what the reference gets from CHOLMOD through libdogleg
-// (cholmod_factorize / cholmod_solve; call sites mrcal.c:6435 and
-// mrcal-pywrap.c:196-212, 557). The reference factors the full sparse JtJ with
-// a simplicial LDL'; here the frame/point blocks have already been eliminated
-// (normal.cu), what is left is small and dense, and it is factored as L L'
-// with a two-level blocked right-looking algorithm:
+//       for each 256-column outer panel:
+//           for each 64-column inner block of it:
+//               potrf_diag   one CTA: factor the 64x64 diagonal block in shared
+//                            memory, and invert the factor (potrf_block.cuh)
+//               trsm         rows below: X <- A inv(L_kk)'   (small GEMM)
+//               syrk (K=64)  update of the REST OF THE PANEL only
+//           syrk (K=256)     one DMMA update of the whole trailing matrix
 //
-//   for each 256-column outer panel:
-//       for each 64-column inner block of it:
-//           potrf_diag   one CTA: factor the 64x64 diagonal block in shared
-//                        memory, and invert the factor (potrf_block.cuh)
-//           trsm         rows below: X <- A inv(L_kk)'   (small GEMM)
-//           syrk (K=64)  update of the REST OF THE PANEL only
-//       syrk (K=256)     one DMMA update of the whole trailing matrix
+//   - triangular solves with the factor for nrhs right-hand sides, two short kernels per 64-column block and
+//     direction (the factorization objects' solves)
+//   - min/max of diag(L), for rcond
+//   - fill_words: a few ranges of flags and counters cleared in one launch
+//   - timing and debugging aids
 //
-// Storage: row-major n x n, lower triangle, n padded to a multiple of 64 (the
-// caller puts 1 on the padding diagonal). Rows are K-contiguous, which is what
-// mma.sync.m8n8k4.row.col.f64 wants for both operands of  C -= P P'.
+// Stands in for cholmod_factorize / cholmod_solve as the reference calls them (mrcal.c:6435, mrcal-pywrap.c:196-212,
+// 557). Storage: row-major npad x npad, lower triangle, npad a multiple of 64 (the caller puts 1 on the padding
+// diagonal). Rows are K-contiguous, which is what mma.sync.m8n8k4.row.col.f64 wants for both operands of  C -= P P'.
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <vector>
@@ -293,13 +294,13 @@ static bool syrk_update(double* A, int ld, int n, int c0, int c1, int k0, int k1
     return true;
 }
 
-static bool chol_factor_enqueue(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch, int kinds = 7);
 static bool chol_solve_enqueue(const double* L, int npad, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s, int* nlaunch, int parts = 3);
 
-// The factorization is ~3 short kernels per 64-column block, all with launch-time-constant
-// arguments: replaying a captured CUDA graph takes the host out of the loop (the host would
+// The multi-kernel factorization is ~3 short kernels per 64-column block, a solve 2 per block and direction, all with
+// launch-time-constant arguments: replaying a captured CUDA graph takes the host out of the loop (the host would
 // otherwise bound the rate at which the chain of tiny kernels is issued).
-struct GraphKey { const void* a; const void* b; int npad, nreal, kind; };
+// m: nreal (factorization) or ldb (solve); kind: 0 the factorization, else the solve's parts
+struct GraphKey { const void* a; const void* b; int npad, m, kind; };
 struct GraphEntry { GraphKey key; cudaGraphExec_t exec; int launches; unsigned long stamp; };
 static std::vector<GraphEntry> g_graphs;
 static unsigned long g_stamp = 0;
@@ -308,7 +309,7 @@ template <typename F>
 static bool run_graphed(const GraphKey& key, cudaStream_t s, int* nlaunch, F enqueue)
 {
     for(auto& e : g_graphs)
-        if(e.key.a == key.a && e.key.b == key.b && e.key.npad == key.npad && e.key.nreal == key.nreal && e.key.kind == key.kind)
+        if(e.key.a == key.a && e.key.b == key.b && e.key.npad == key.npad && e.key.m == key.m && e.key.kind == key.kind)
         {
             e.stamp = ++g_stamp;
             MB200_CUDA_CHECK(cudaGraphLaunch(e.exec, s));
@@ -349,65 +350,41 @@ void chol_forget_graphs(const void* A)
         else i++;
 }
 
-bool chol_factor(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch,
-                 CholScratch* scratch, const int* d_run_if)
+bool chol_factor_blocked(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch)
 {
     if(!configure_kernels()) return false;
-    if(chol_dataflow_usable(npad)) return chol_factor_dataflow(A, npad, nreal, invL, d_info, s, nlaunch, scratch, d_run_if);
-    // (the multi-kernel fallback always runs: a factorization nobody asked for costs time, not correctness)
-    return run_graphed(GraphKey{A, d_info, npad, nreal, 0}, s, nlaunch,
-                       [&](int* n) { return chol_factor_enqueue(A, npad, nreal, invL, d_info, s, n); });
+    return run_graphed(GraphKey{A, d_info, npad, nreal, 0}, s, nlaunch, [&](int* n)
+    {
+        MB200_CUDA_CHECK(cudaMemsetAsync(d_info, 0, sizeof(int), s));
+        for(int K0 = 0; K0 < npad; K0 += NBO)
+        {
+            const int K1 = K0 + NBO < npad ? K0 + NBO : npad;
+            for(int k0 = K0; k0 < K1; k0 += NB)
+            {
+                potrf_diag_kernel<false><<<1, 256, kPotrfSmem, s>>>(A, npad, k0, invL + (size_t)(k0 / NB) * NB * NB, d_info, nreal, nullptr);
+                (*n)++;
+                const int nrows_below = npad - (k0 + NB);
+                if(nrows_below > 0)
+                {
+                    trsm_kernel<<<nrows_below / NB, 256, kBlockSmem, s>>>(A, npad, k0, invL + (size_t)(k0 / NB) * NB * NB, npad);
+                    (*n)++;
+                    // rest of this outer panel only
+                    if(!syrk_update(A, npad, npad, k0 + NB, K1, k0, k0 + NB, s, n)) return false;
+                }
+            }
+            // the whole trailing matrix, K = width of the panel
+            if(!syrk_update(A, npad, npad, K1, npad, K0, K1, s, n)) return false;
+        }
+        MB200_CUDA_CHECK(cudaGetLastError());
+        return true;
+    });
 }
 
 bool chol_solve(const double* L, int npad, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s, int* nlaunch, int parts)
 {
     if(nrhs != 1) return chol_solve_enqueue(L, npad, invL, B, ldb, nrhs, s, nlaunch, parts);
-    return run_graphed(GraphKey{L, B, npad, ldb, 1 + 16 * parts}, s, nlaunch,
+    return run_graphed(GraphKey{L, B, npad, ldb, parts}, s, nlaunch,
                        [&](int* n) { return chol_solve_enqueue(L, npad, invL, B, ldb, 1, s, n, parts); });
-}
-
-static bool chol_solve_bwd_enqueue(const double* L, int npad, const double* invL, double* B, int ldb, cudaStream_t s, int* nlaunch);
-
-// L' z = y only (the forward half came out of the factorization itself: see normal_assemble's augmented row)
-bool chol_solve_backward(const double* L, int npad, const double* invL, double* B, int ldb, int* d_info, cudaStream_t s, int* nlaunch,
-                         CholScratch* scratch, const int* d_run_if)
-{
-    if(chol_dataflow_usable(npad)) return chol_solve_backward_dataflow(L, npad, invL, B, d_info, s, nlaunch, scratch, d_run_if);
-    return run_graphed(GraphKey{L, B, npad, ldb, 2}, s, nlaunch,
-                       [&](int* n) { return chol_solve_bwd_enqueue(L, npad, invL, B, ldb, s, n); });
-}
-
-static bool chol_factor_enqueue(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch, int kinds)
-{
-    if(!configure_kernels()) return false;
-    MB200_CUDA_CHECK(cudaMemsetAsync(d_info, 0, sizeof(int), s));
-    for(int K0 = 0; K0 < npad; K0 += NBO)
-    {
-        const int K1 = K0 + NBO < npad ? K0 + NBO : npad;
-        for(int k0 = K0; k0 < K1; k0 += NB)
-        {
-            if(kinds & 1)
-            {
-                potrf_diag_kernel<false><<<1, 256, kPotrfSmem, s>>>(A, npad, k0, invL + (size_t)(k0 / NB) * NB * NB, d_info, nreal, nullptr);
-                if(nlaunch) (*nlaunch)++;
-            }
-            const int nrows_below = npad - (k0 + NB);
-            if(nrows_below > 0)
-            {
-                if(kinds & 2)
-                {
-                    trsm_kernel<<<nrows_below / NB, 256, kBlockSmem, s>>>(A, npad, k0, invL + (size_t)(k0 / NB) * NB * NB, npad);
-                    if(nlaunch) (*nlaunch)++;
-                }
-                // rest of this outer panel only
-                if((kinds & 4) && !syrk_update(A, npad, npad, k0 + NB, K1, k0, k0 + NB, s, nlaunch)) return false;
-            }
-        }
-        // the whole trailing matrix, K = width of the panel
-        if((kinds & 8 || kinds == 7) && !syrk_update(A, npad, npad, K1, npad, K0, K1, s, nlaunch)) return false;
-    }
-    MB200_CUDA_CHECK(cudaGetLastError());
-    return true;
 }
 
 ////////////////////////////////////////////////////////////////////////////////
@@ -510,61 +487,57 @@ void chol_debug_fill_spd(double* A, int npad, cudaStream_t s)
     debug_fill_spd_kernel<<<(unsigned)(((size_t)npad * npad + 255) / 256), 256, 0, s>>>(A, npad);
 }
 
-// Timing aid (not on any product path): device time of `reps` factorizations of an n x n matrix,
-// restricted to the kernel kinds in the mask (1 potrf_diag, 2 trsm, 4 panel syrk, 8 trailing syrk;
-// 15 = everything), launched directly (graph=0) or as a captured graph (graph=1)
-double chol_debug_time(int n, int reps, int kinds, int graph)
+// Timing aid (not on any product path): device time of chol_factor for an n x n matrix (what = 0; net of the refill
+// with an SPD matrix that every repetition needs) or of chol_solve_backward (what = 1), per call, averaged over reps
+// calls; -1 on failure
+double chol_debug_time(int n, int reps, int what)
 {
     const int npad = chol_padded(n);
-    double *A, *invL; int* info;
-    if(cudaMalloc(&A, (size_t)npad * npad * sizeof(double)) != cudaSuccess) return -1.;
-    cudaMalloc(&invL, (size_t)npad * NB * sizeof(double));
-    cudaMalloc(&info, sizeof(int));
-    cudaStream_t s; cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking);
-    configure_kernels();
-    debug_fill_spd_kernel<<<(unsigned)(((size_t)npad * npad + 255) / 256), 256, 0, s>>>(A, npad);
-    cudaGraphExec_t exec = nullptr;
-    if(graph)
+    double *A = nullptr, *invL = nullptr, *rhs = nullptr; int* info = nullptr;
+    cudaStream_t s = nullptr;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    CholScratch sc;
+    bool ok = cudaMalloc(&A, (size_t)npad * npad * sizeof(double)) == cudaSuccess &&
+              cudaMalloc(&invL, (size_t)npad * NB * sizeof(double)) == cudaSuccess &&
+              cudaMalloc(&rhs, (size_t)npad * sizeof(double)) == cudaSuccess && cudaMalloc(&info, sizeof(int)) == cudaSuccess &&
+              cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaEventCreate(&e0) == cudaSuccess && cudaEventCreate(&e1) == cudaSuccess && chol_scratch_create(&sc, npad);
+    // ms per call of: 0 the refill, 1 the refill and the factorization, 2 the backward substitution
+    auto timed = [&](int kind) -> double
     {
-        cudaGraph_t g;
-        cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal);
-        chol_factor_enqueue(A, npad, n, invL, info, s, nullptr, kinds == 15 ? 7 : kinds);
-        cudaStreamEndCapture(s, &g);
-        cudaGraphInstantiate(&exec, g, 0);
-        cudaGraphDestroy(g);
-    }
-    cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    double* rhs = nullptr;
-    if(kinds >= 32)
-    {
-        // 32: persistent factorization; 64: persistent backward substitution; 128: multi-kernel backward substitution
-        cudaMalloc(&rhs, (size_t)npad * sizeof(double));
-        cudaMemsetAsync(rhs, 0, (size_t)npad * sizeof(double), s);
-        chol_factor_dataflow(A, npad, n, invL, info, s, nullptr);
-    }
-    for(int r = -1; r < reps; r++)
-    {
-        if(r == 0) cudaEventRecord(e0, s);
-        if(kinds == 32)
+        for(int r = -1; r < reps && ok; r++)
         {
-            if(r >= 0) debug_fill_spd_kernel<<<(unsigned)(((size_t)npad * npad + 255) / 256), 256, 0, s>>>(A, npad);
-            chol_factor_dataflow(A, npad, n, invL, info, s, nullptr);
+            if(r == 0) ok = cudaEventRecord(e0, s) == cudaSuccess;
+            if(kind <= 1) chol_debug_fill_spd(A, npad, s);
+            if(kind == 1) ok = ok && chol_factor(A, npad, n, invL, info, s, nullptr, &sc);
+            if(kind == 2) ok = ok && chol_solve_backward(A, npad, invL, rhs, info, s, nullptr, &sc);
         }
-        else if(kinds == 33) debug_fill_spd_kernel<<<(unsigned)(((size_t)npad * npad + 255) / 256), 256, 0, s>>>(A, npad);
-        else if(kinds == 64) chol_solve_backward_dataflow(A, npad, invL, rhs, info, s, nullptr);
-        else if(kinds == 128) run_graphed(GraphKey{A, rhs, npad, npad, 2}, s, nullptr, [&](int* nn) { return chol_solve_bwd_enqueue(A, npad, invL, rhs, npad, s, nn); });
-        else if(graph) cudaGraphLaunch(exec, s);
-        else      chol_factor_enqueue(A, npad, n, invL, info, s, nullptr, kinds == 15 ? 7 : kinds);
+        float ms = 0.f;
+        ok = ok && cudaEventRecord(e1, s) == cudaSuccess && cudaEventSynchronize(e1) == cudaSuccess &&
+             cudaEventElapsedTime(&ms, e0, e1) == cudaSuccess;
+        return ms / reps;
+    };
+    double ms = -1.;
+    if(ok && what == 0)
+    {
+        const double fill = timed(0), both = timed(1);
+        if(ok) ms = both - fill;
     }
-    cudaEventRecord(e1, s);
-    cudaEventSynchronize(e1);
-    float ms = 0.f; cudaEventElapsedTime(&ms, e0, e1);
-    if(exec) cudaGraphExecDestroy(exec);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    chol_forget_graphs(A);
-    cudaStreamDestroy(s);
-    cudaFree(A); cudaFree(invL); cudaFree(info); cudaFree(rhs);
-    return ms / reps;
+    else if(ok && what == 1)
+    {
+        chol_debug_fill_spd(A, npad, s);
+        ok = cudaMemsetAsync(rhs, 0, (size_t)npad * sizeof(double), s) == cudaSuccess &&
+             chol_factor(A, npad, n, invL, info, s, nullptr, &sc);
+        const double bwd = timed(2);
+        if(ok) ms = bwd;
+    }
+    if(s) cudaStreamSynchronize(s);
+    chol_scratch_destroy(&sc);
+    if(e0) cudaEventDestroy(e0);
+    if(e1) cudaEventDestroy(e1);
+    if(s) cudaStreamDestroy(s);
+    cudaFree(A); cudaFree(invL); cudaFree(rhs); cudaFree(info);
+    return ms;
 }
 
 // Debugging aid: clock64() stamps of the phases of one diagonal-block factorization (64 values)
@@ -586,24 +559,6 @@ bool chol_debug_potrf_stamps(long long* out64)
     MB200_CUDA_CHECK(cudaDeviceSynchronize());
     MB200_CUDA_CHECK(cudaMemcpy(out64, st, 64 * sizeof(long long), cudaMemcpyDeviceToHost));
     cudaFree(A); cudaFree(invL); cudaFree(info); cudaFree(st);
-    return true;
-}
-
-static bool chol_solve_bwd_enqueue(const double* L, int npad, const double* invL, double* B, int ldb, cudaStream_t s, int* nlaunch)
-{
-    const int nblk = npad / NB;
-    for(int k = nblk - 1; k >= 0; k--)
-    {
-        const int k0 = k * NB;
-        solve_diag_kernel<<<1, NB, 0, s>>>(invL + (size_t)k * NB * NB, B, ldb, k0, true);
-        if(nlaunch) (*nlaunch)++;
-        if(k0 > 0)
-        {
-            solve_update_bwd_kernel<<<(k0 + 255) / 256, 256, 0, s>>>(L, npad, B, ldb, 1, k0);
-            if(nlaunch) (*nlaunch)++;
-        }
-    }
-    MB200_CUDA_CHECK(cudaGetLastError());
     return true;
 }
 

@@ -1,4 +1,4 @@
-// Internal: dense Cholesky on the device (chol.cu)
+// Internal: dense Cholesky on the device (chol_dataflow.cu, chol.cu)
 #pragma once
 #include <cuda_runtime.h>
 
@@ -24,40 +24,38 @@ struct WordFill
 };
 bool fill_words(const WordFill& f, cudaStream_t s);
 
-// Scratch of the persistent kernels (tile flags, the solution slots of the backward substitution): one per
-// owner of a factorization, so that two factorizations in flight never share flags
-struct CholScratch { int* flags = nullptr; double* xbuf = nullptr; };
-bool chol_scratch_create(CholScratch* sc);
+// Scratch of the persistent kernels (tile flags, the solution slots of the backward substitution) for systems of up to
+// npad_max unknowns: one per owner of a factorization, so that two factorizations in flight never share flags
+struct CholScratch { int* flags = nullptr; double* xbuf = nullptr; int npad_max = 0; };
+bool chol_scratch_create(CholScratch* sc, int npad_max);
 void chol_scratch_destroy(CholScratch* sc);
 
+// chol_dataflow.cu, one persistent kernel each (the factorization: up to npad = 8192):
+//
 // A: row-major npad x npad, lower triangle holds the matrix; rows/cols >= nreal
 // are padding (1 on the diagonal). On return the lower triangle holds L.
 // invL: [npad/64][64*64] inverses of the diagonal blocks of L.
 // d_info: device int; 0 if positive definite, else 1 + index of the first bad pivot.
-// scratch: the caller's (nullptr: a per-device default). d_run_if: device flag; 0 there = do nothing (nullptr: always run)
+// scratch: the caller's, for at least npad. d_run_if: device flag; 0 there = do nothing (nullptr: always run)
 bool chol_factor(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch,
-                 CholScratch* scratch = nullptr, const int* d_run_if = nullptr);
+                 CholScratch* scratch, const int* d_run_if = nullptr);
 
-// Solve L L' X = B in place for nrhs right-hand sides stored as rows B[r][0..npad).
+// Only the backward half, L' Z = B in place, one right-hand side B[0..npad). d_info (may be the factorization's): set
+// to -9 if the persistent kernel gave up waiting (never expected; the alternative would be to hang the GPU)
+bool chol_solve_backward(const double* L, int npad, const double* invL, double* B, int* d_info, cudaStream_t s, int* nlaunch,
+                         CholScratch* scratch, const int* d_run_if = nullptr);
+
+// chol.cu: the multi-kernel factorization, which chol_factor runs above npad = 8192 (same arguments; no scratch)
+bool chol_factor_blocked(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch);
+
+// chol.cu: solve L L' X = B in place for nrhs right-hand sides stored as rows B[r][0..npad).
 // parts: 1 = only L Y = B, 2 = only L' X = B, 3 = both
 bool chol_solve(const double* L, int npad, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s, int* nlaunch, int parts = 3);
-
-// Only the backward half, L' Z = B in place, one right-hand side. d_info (may be the factorization's): set to -9
-// if the persistent kernel gave up waiting (never expected; the alternative would be to hang the GPU)
-bool chol_solve_backward(const double* L, int npad, const double* invL, double* B, int ldb, int* d_info, cudaStream_t s, int* nlaunch,
-                         CholScratch* scratch = nullptr, const int* d_run_if = nullptr);
-
-// chol_dataflow.cu: the same two operations as one persistent kernel each (n <= 8192)
-bool chol_dataflow_usable(int npad);
-bool chol_factor_dataflow(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch,
-                          CholScratch* scratch = nullptr, const int* d_run_if = nullptr);
-bool chol_solve_backward_dataflow(const double* L, int npad, const double* invL, double* B, int* d_info, cudaStream_t s, int* nlaunch,
-                                  CholScratch* scratch = nullptr, const int* d_run_if = nullptr);
 
 // drop cached CUDA graphs that reference this buffer (call before freeing it)
 void chol_forget_graphs(const void* A);
 
-double chol_debug_time(int n, int reps, int kinds, int graph);
+double chol_debug_time(int n, int reps, int what);
 bool chol_debug_potrf_stamps(long long* out64);
 
 // d_out2[0] = min, d_out2[1] = max of diag(L)[0..nreal)

@@ -1,22 +1,17 @@
 // Kernel family 2c: the dense Cholesky factorization and the backward substitution
-// as ONE persistent kernel each, for the sizes where the multi-kernel version
-// (chol.cu) is bound by the latency of its chain of ~5 kernels per 64 columns.
+// of every dense system, as ONE persistent kernel each.
 //
-// Left-looking tile algorithm, 64x64 tiles, one CTA per SM, tiles dealt round-robin
-// in column-major order. The owner of tile (i,j) computes
+// Left-looking tile algorithm, 64x64 tiles, one CTA per SM. The owner of tile (i,j) computes
 //       C = A_ij - sum_{k<j} L_ik L_jk'          (DMMA, operands staged with cp.async)
 //       i == j:  L_jj = chol(C), and its inverse (potrf_block.cuh)
 //       i >  j:  L_ij = C inv(L_jj)'             (DMMA)
 // and then raises a flag in global memory (st.release). Consumers poll the flags of the
-// tiles they need (ld.acquire) and pull them from L2. All CTAs are co-resident
-// (cooperative launch), and every tile depends only on tiles that come earlier in the
-// column-major order, which each CTA walks in increasing order: the scheme cannot
-// deadlock. Waits are bounded all the same (a wedged GPU box costs more than a wrong
-// answer that the caller can detect): on timeout *info = -9.
-//
-// The diagonal tile and the tile left of it form one task of one CTA, so the critical path
-// per 64 columns is  potrf_block + one flag hop + one triangular tile product + the last
-// rank-64 update (from shared memory), instead of five kernel boundaries.
+// tiles they need (ld.acquire) and pull them from L2. The diagonal tiles and the tiles
+// left of them -- the critical path -- belong to one CTA, the spine (chol_spine_kernel).
+// All CTAs are co-resident (cooperative launch) and every CTA walks its tasks in an order
+// in which each depends only on earlier ones: the scheme cannot deadlock. Waits are
+// bounded all the same (a wedged GPU box costs more than a wrong answer that the caller
+// can detect): on timeout *info = -9.
 //
 // Stands in for cholmod_factorize / cholmod_solve as libdogleg calls them (call site
 // mrcal.c:6435); the reference has no counterpart of this structure.
@@ -174,121 +169,6 @@ __device__ __forceinline__ void tile_trsm(const double* C, const double* W, doub
 
 __device__ __forceinline__ int tile_flag(int i, int j, int nb) { return j * nb - (j * (j - 1)) / 2 + (i - j); }
 
-// Tasks, in the order every CTA walks them (each depends only on earlier ones):
-//   task 0: the diagonal tile (0,0);
-//   then column by column, j = 0 .. nb-2:  the DIAGONAL STEP d = j+1 first -- the tile (d,j) left of the diagonal
-//   AND the diagonal tile (d,d), by the same CTA: the freshly solved L_dj goes straight from shared memory into
-//   the last rank-64 update of the diagonal tile, no store -> flag -> load hop on the spine -- and after it the
-//   tiles (i,j), i >= j+2.
-__global__ void __launch_bounds__(256, 1)
-chol_dataflow_kernel(double* __restrict__ A, int ld, int nb, int nreal, double* __restrict__ invL, int* __restrict__ info,
-                     int* __restrict__ flags, int* __restrict__ abort_flag, const int* __restrict__ run_if)
-{
-    // the trust-region loop decides on the device whether this operating point needs a Gauss-Newton step at all
-    if(run_if != nullptr && *run_if == 0) return;
-    extern __shared__ __align__(16) unsigned char dsm_raw[];
-    DfSmem& sm = *reinterpret_cast<DfSmem*>(dsm_raw);
-    const int tid = threadIdx.x;
-    const int ntasks = 1 + (nb - 1) * nb / 2;
-    double acc[2][4][2];
-
-    for(int tl = blockIdx.x; tl < ntasks; tl += gridDim.x)
-    {
-        int i, j;
-        bool diag_step;
-        if(tl == 0) { i = 0; j = 0; diag_step = true; }
-        else
-        {
-            int rem = tl - 1;
-            j = 0;
-            while(rem >= nb - 1 - j) { rem -= nb - 1 - j; j++; }
-            diag_step = rem == 0;
-            i = j + 1 + rem;
-        }
-        // diag_step: d = i; tiles (d, j = d-1) [none for d = 0] and (d, d). Otherwise the tile (i, j), i >= j+2
-        const int d = i;
-        const bool have_left = diag_step && d > 0;
-        double* Aij = A + (size_t)i * T * ld + (size_t)j * T;          // (i,j): the left tile of a diagonal step
-        double* Add = A + (size_t)d * T * ld + (size_t)d * T;
-        const int kend = diag_step ? (d > 0 ? d - 1 : 0) : j;         // operands L_ik, L_jk for k < kend
-
-        if(!diag_step || have_left) tile_to_smem(sm.C2, Aij, ld);
-        if(diag_step) tile_to_smem(sm.pb.L, Add, ld);
-        cp_commit();
-        for(int k = 0; k < kend; k++)
-        {
-            if(!wait_flags(sm, flags + tile_flag(i, k, nb), flags + tile_flag(j, k, nb), abort_flag, info)) return;
-            tile_to_smem(sm.opA, A + (size_t)i * T * ld + (size_t)k * T, ld);
-            tile_to_smem(sm.opB, A + (size_t)j * T * ld + (size_t)k * T, ld);
-            cp_commit();
-            cp_wait_all();
-            __syncthreads();
-            acc_zero(acc);
-            tile_mma(acc, sm.opA, sm.opB);
-            tile_sub(sm.C2, acc);
-            if(diag_step)
-            {
-                acc_zero(acc);
-                tile_mma(acc, sm.opA, sm.opA);
-                tile_sub(sm.pb.L, acc);
-            }
-            __syncthreads();
-        }
-        cp_wait_all();
-        __syncthreads();
-
-        if(!diag_step || have_left)
-        {
-            // L_ij = C2 inv(L_jj)'
-            if(!wait_flags(sm, flags + tile_flag(j, j, nb), nullptr, abort_flag, info)) return;
-            tile_to_smem(sm.opB, invL + (size_t)j * T * T, T);
-            cp_commit();
-            cp_wait_all();
-            __syncthreads();
-            tile_trsm(sm.C2, sm.opB, Aij, ld, have_left ? sm.opA : nullptr);
-            __threadfence();
-            __syncthreads();
-            if(tid == 0) st_release(flags + tile_flag(i, j, nb), 1);
-        }
-        if(diag_step)
-        {
-            if(have_left)
-            {
-                acc_zero(acc);
-                tile_mma(acc, sm.opA, sm.opA);
-                tile_sub(sm.pb.L, acc);
-            }
-            potrf_block(sm.pb, info, d * T, nreal);
-            double* invLd = invL + (size_t)d * T * T;
-            for(int e = tid; e < T * T; e += 256)
-            {
-                const int r = e / T, c = e % T;
-                if(c <= r) Add[(size_t)r * ld + c] = sm.pb.L[r * PLD + c];
-                invLd[e] = sm.pb.X[r * PLD + c];
-            }
-            __threadfence();
-            __syncthreads();
-            if(tid == 0) st_release(flags + tile_flag(d, d, nb), 1);
-        }
-        __syncthreads();
-    }
-}
-
-// C = D - acc for [64][PLD] tiles in shared memory (each thread its own fragment elements)
-__device__ __forceinline__ void tile_sub_to(double* C, const double* D, const double (&acc)[2][4][2])
-{
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int wm = warp >> 1, wn = warp & 1, g = lane >> 2, t = lane & 3;
-#pragma unroll
-    for(int a = 0; a < 2; a++)
-#pragma unroll
-        for(int b = 0; b < 4; b++)
-        {
-            const int e = (wm * 16 + a * 8 + g) * PLD + wn * 32 + b * 8 + 2 * t;
-            const double2 v = *reinterpret_cast<const double2*>(&D[e]);
-            *reinterpret_cast<double2*>(&C[e]) = make_double2(v.x - acc[a][b][0], v.y - acc[a][b][1]);
-        }
-}
 // C = D - A A' on the 8x8 granules of the LOWER triangle only (36 of 64: what potrf_block reads), dealt to the 8 warps
 // in row-major order: 5 or 4 granules per warp instead of 8
 __device__ __forceinline__ void tile_syrk_lower_sub(double* C, const double* D, const double* A)
@@ -339,7 +219,7 @@ __device__ __forceinline__ void tile_to_global(double* __restrict__ dst, size_t 
     }
 }
 
-// The same factorization with the SPINE -- the diagonal tiles and the tiles left of them, whose chain of
+// The factorization, with the SPINE -- the diagonal tiles and the tiles left of them, whose chain of
 // potrf_block -> triangular product -> last rank-64 update IS the critical path -- on one CTA that does nothing else:
 // the inverse of a diagonal block goes from potrf_block to the next triangular product through shared memory, and the
 // spine CTA never spends time on the earlier updates of its tiles. Those are "pre" tasks of the other CTAs:
@@ -347,6 +227,7 @@ __device__ __forceinline__ void tile_to_global(double* __restrict__ dst, size_t 
 // which the spine picks up when potrf_block of step d-1 is done (they have had that long to finish).
 // Helper tasks in the order every helper CTA walks them, column by column j = 0 .. nb-3:
 //   tile (j+2, j);  pre(j+2);  tiles (i, j), i = j+3 .. nb-1
+// (none for nb <= 2: steps 0 and 1 have no pre task, and the spine CTA runs alone).
 // Every task depends on spine steps and on EARLIER helper tasks only; the spine depends on its own past and on pre
 // tasks: no cycles, all CTAs co-resident, every CTA walks its list in order: no deadlock. Waits are bounded as above.
 // (registers capped -- no spills at 160 -- so that the small kernels of the Cauchy side fit next to a CTA of this one)
@@ -582,127 +463,111 @@ chol_backward_dataflow_kernel(const double* __restrict__ L, int ld, int nb, cons
     }
 }
 
-constexpr int kMaxBlocks = 128;
-constexpr int kMaxTiles = kMaxBlocks * (kMaxBlocks + 1) / 2;
+// SMs of the current device, once the kernels are set up for it (cached per device)
+int g_num_sms[kMaxDevices];
 
-// per device: kernel attributes, SM count
-struct DeviceCfg { bool configured = false, unavailable = false; int num_sms = 0; };
-DeviceCfg g_cfg[kMaxDevices];
-// scratch of callers that bring none (the timing aids): one per device
-CholScratch g_default_scratch[kMaxDevices];
-
-DeviceCfg* configure()
+// the SM count; 0 (and set_error) if the persistent kernels cannot run on the current device
+int configure()
 {
     int dev = 0;
-    if(cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) { cudaGetLastError(); return nullptr; }
-    DeviceCfg& c = g_cfg[dev];
-    if(c.configured) return &c;
-    if(c.unavailable) return nullptr;
-    int coop = 0;
-    if(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev) != cudaSuccess || !coop ||
-       cudaDeviceGetAttribute(&c.num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-       cudaFuncSetAttribute(chol_dataflow_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DfSmem)) != cudaSuccess ||
-       cudaFuncSetAttribute(chol_spine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DfSmem)) != cudaSuccess)
+    if(cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices)
+    {
+        set_error("the persistent Cholesky kernels: no usable current device: %s", cudaGetErrorString(cudaGetLastError()));
+        return 0;
+    }
+    if(g_num_sms[dev] > 0) return g_num_sms[dev];
+    int coop = 0, sms = 0;
+    cudaError_t e = cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
+    if(e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if(e == cudaSuccess) e = cudaFuncSetAttribute(chol_spine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DfSmem));
+    // (the spine needs a second CTA for its pre tasks from nb = 3 on)
+    if(e != cudaSuccess || !coop || sms < 2)
     {
         cudaGetLastError();
-        c.unavailable = true;
-        return nullptr;
+        set_error("the persistent Cholesky kernels cannot run on device %d (cooperative launch: %d, SMs: %d): %s", dev, coop, sms,
+                  cudaGetErrorString(e));
+        return 0;
     }
-    c.configured = true;
-    return &c;
+    return g_num_sms[dev] = sms;
+}
+
+bool scratch_fits(const CholScratch* sc, int npad)
+{
+    if(sc != nullptr && npad <= sc->npad_max) return true;
+    set_error("Cholesky of a %d x %d system with a scratch for at most %d x %d", npad, npad, sc ? sc->npad_max : 0, sc ? sc->npad_max : 0);
+    return false;
 }
 
 long long* g_debug_stamps = nullptr;   // set by chol_debug_spine_stamps() only
 
-CholScratch* scratch_or_default(CholScratch* sc)
-{
-    if(sc != nullptr && sc->flags != nullptr) return sc;
-    int dev = 0;
-    if(cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return nullptr;
-    CholScratch& d = g_default_scratch[dev];
-    if(d.flags == nullptr && !chol_scratch_create(&d)) return nullptr;
-    return &d;
-}
-
 }  // namespace
 
-bool chol_scratch_create(CholScratch* sc)
+// flags: the abort flag, then for a system of nb blocks one flag per tile of the lower triangle and the spine's nb
+// pre counters; xbuf: the solution slots of the backward substitution
+bool chol_scratch_create(CholScratch* sc, int npad_max)
 {
-    sc->flags = nullptr; sc->xbuf = nullptr;
-    if(cudaMalloc(&sc->flags, (kMaxTiles + 1 + kMaxBlocks) * sizeof(int)) != cudaSuccess ||
-       cudaMalloc(&sc->xbuf, (size_t)kMaxBlocks * T * sizeof(double)) != cudaSuccess)
+    const size_t nb = (size_t)(npad_max / T);
+    sc->flags = nullptr; sc->xbuf = nullptr; sc->npad_max = 0;
+    if(cudaMalloc(&sc->flags, (1 + nb * (nb + 1) / 2 + nb) * sizeof(int)) != cudaSuccess ||
+       cudaMalloc(&sc->xbuf, nb * T * sizeof(double)) != cudaSuccess)
     {
         set_error("cudaMalloc of the factorization scratch failed: %s", cudaGetErrorString(cudaGetLastError()));
         chol_scratch_destroy(sc);
         return false;
     }
+    sc->npad_max = npad_max;
     return true;
 }
 void chol_scratch_destroy(CholScratch* sc)
 {
     if(sc->flags) cudaFree(sc->flags);
     if(sc->xbuf) cudaFree(sc->xbuf);
-    sc->flags = nullptr; sc->xbuf = nullptr;
+    sc->flags = nullptr; sc->xbuf = nullptr; sc->npad_max = 0;
 }
 
-bool chol_dataflow_usable(int npad)
+bool chol_factor(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch,
+                 CholScratch* scratch, const int* d_run_if)
 {
-    static const bool disabled = getenv("MRCAL_B200_CHOL_CLASSIC") != nullptr;
-    return !disabled && npad / T <= kMaxBlocks && configure() != nullptr;
-}
-
-bool chol_factor_dataflow(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch,
-                          CholScratch* scratch, const int* d_run_if)
-{
-    DeviceCfg* cfg = configure();
-    CholScratch* sc = scratch_or_default(scratch);
-    if(!cfg || !sc) { set_error("the persistent Cholesky kernel is not available on this device"); return false; }
-    int nb = npad / T;
-    const int ntiles = 1 + (nb - 1) * nb / 2;   // tasks: see the kernel
-    int ld = npad;
-    int* flags = sc->flags;
-    int* abort_flag = sc->flags + kMaxTiles;
-    static const bool no_spine = getenv("MRCAL_B200_CHOL_NO_SPINE") != nullptr;
-    const bool spine = !no_spine && nb >= 3 && cfg->num_sms >= 2;
-    // d_info, one flag per tile of the lower triangle, the abort flag and (spine) the spine's nb counters behind it
+    if(!scratch_fits(scratch, npad)) return false;
+    // Above 8192 unknowns the multi-kernel factorization (chol.cu) is faster: 39 against 43 ms at n = 12000, 159
+    // against 187 ms at n = 19376 (DESIGN section 9). It ignores d_run_if: a factorization nobody asked for costs
+    // time, not correctness
+    if(npad > 8192) return chol_factor_blocked(A, npad, nreal, invL, d_info, s, nlaunch);
+    const int num_sms = configure();
+    if(num_sms == 0) return false;
+    int nb = npad / T, ld = npad;
+    const int ntiles = nb * (nb + 1) / 2;
+    int* abort_flag = scratch->flags;
+    int* flags = abort_flag + 1;
+    int* pre = flags + ntiles;
     WordFill clear;
     clear.add(d_info, sizeof(int));
-    clear.add(sc->flags, (size_t)(nb * (nb + 1) / 2) * sizeof(int));
-    clear.add(abort_flag, (size_t)(1 + (spine ? nb : 0)) * sizeof(int));
+    clear.add(abort_flag, (size_t)(1 + ntiles + nb) * sizeof(int));
     if(!fill_words(clear, s)) return false;
-    if(spine)
-    {
-        int* pre = sc->flags + kMaxTiles + 1;
-        long long* stamps = g_debug_stamps;
-        void* args[] = {&A, &ld, &nb, &nreal, &invL, &d_info, &flags, &pre, &abort_flag, &d_run_if, &stamps};
-        const int nhelper_tasks = (nb - 1) * nb / 2 - 1;
-        const int grid = 1 + (nhelper_tasks < cfg->num_sms - 1 ? nhelper_tasks : cfg->num_sms - 1);
-        MB200_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)chol_spine_kernel, dim3(grid), dim3(256), args, sizeof(DfSmem), s));
-        if(nlaunch) (*nlaunch)++;
-        return true;
-    }
-    void* args[] = {&A, &ld, &nb, &nreal, &invL, &d_info, &flags, &abort_flag, &d_run_if};
-    const int grid = ntiles < cfg->num_sms ? ntiles : cfg->num_sms;
-    MB200_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)chol_dataflow_kernel, dim3(grid), dim3(256), args, sizeof(DfSmem), s));
+    long long* stamps = g_debug_stamps;
+    void* args[] = {&A, &ld, &nb, &nreal, &invL, &d_info, &flags, &pre, &abort_flag, &d_run_if, &stamps};
+    // the spine CTA and up to one helper CTA per helper task (see the kernel; none for nb <= 2) on the other SMs
+    const int nhelper_tasks = nb >= 3 ? (nb - 1) * nb / 2 - 1 : 0;
+    const int grid = 1 + (nhelper_tasks < num_sms - 1 ? nhelper_tasks : num_sms - 1);
+    MB200_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)chol_spine_kernel, dim3(grid), dim3(256), args, sizeof(DfSmem), s));
     if(nlaunch) (*nlaunch)++;
     return true;
 }
 
-bool chol_solve_backward_dataflow(const double* L, int npad, const double* invL, double* B, int* d_info, cudaStream_t s, int* nlaunch,
-                                  CholScratch* scratch, const int* d_run_if)
+bool chol_solve_backward(const double* L, int npad, const double* invL, double* B, int* d_info, cudaStream_t s, int* nlaunch,
+                         CholScratch* scratch, const int* d_run_if)
 {
-    DeviceCfg* cfg = configure();
-    CholScratch* sc = scratch_or_default(scratch);
-    if(!cfg || !sc) { set_error("the persistent Cholesky kernel is not available on this device"); return false; }
+    const int num_sms = configure();
+    if(num_sms == 0 || !scratch_fits(scratch, npad)) return false;
     int nb = npad / T, ld = npad;
-    int* abort_flag = sc->flags + kMaxTiles;
+    int* abort_flag = scratch->flags;
     WordFill clear;   // the solution slots to all-ones bytes (not yet written), the abort flag to 0
-    clear.add(sc->xbuf, (size_t)nb * T * sizeof(double), 0xffffffffu);
+    clear.add(scratch->xbuf, (size_t)nb * T * sizeof(double), 0xffffffffu);
     clear.add(abort_flag, sizeof(int));
     if(!fill_words(clear, s)) return false;
-    double* xbuf = sc->xbuf;
+    double* xbuf = scratch->xbuf;
     void* args[] = {&L, &ld, &nb, &invL, &B, &xbuf, &abort_flag, &d_info, &d_run_if};
-    const int grid = nb < cfg->num_sms ? nb : cfg->num_sms;
+    const int grid = nb < num_sms ? nb : num_sms;
     MB200_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)chol_backward_dataflow_kernel, dim3(grid), dim3(256), args, 0, s));
     if(nlaunch) (*nlaunch)++;
     return true;
@@ -724,16 +589,18 @@ bool chol_debug_spine_stamps(int n, long long* out, int nmax)
     MB200_CUDA_CHECK(cudaMalloc(&info, sizeof(int)));
     MB200_CUDA_CHECK(cudaMalloc(&st, (size_t)8 * nb * sizeof(long long)));
     MB200_CUDA_CHECK(cudaMemsetAsync(st, 0, (size_t)8 * nb * sizeof(long long), s));
-    bool ok = true;
+    CholScratch sc;
+    bool ok = chol_scratch_create(&sc, npad);
     for(int rep = 0; rep < 3 && ok; rep++)
     {
         chol_debug_fill_spd(A, npad, s);
         g_debug_stamps = rep == 2 ? st : nullptr;
-        ok = chol_factor_dataflow(A, npad, n, invL, info, s, nullptr, nullptr, nullptr);
+        ok = chol_factor(A, npad, n, invL, info, s, nullptr, &sc);
         g_debug_stamps = nullptr;
     }
     ok = ok && cudaMemcpyAsync(out, st, (size_t)8 * nb * sizeof(long long), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
          cudaStreamSynchronize(s) == cudaSuccess;
+    chol_scratch_destroy(&sc);
     cudaFree(A); cudaFree(invL); cudaFree(info); cudaFree(st);
     cudaStreamDestroy(s);
     return ok;

@@ -67,7 +67,7 @@ mrcal_b200_factorization_create(const int32_t* Jrowptr, const int32_t* Jcolidx, 
     if(Nrows > 0) jtj_rows_kernel<<<((size_t)Nrows * 32 + 255) / 256, 256, 0, s>>>(d_p, d_i, d_x, Nrows, F->H, F->npad);
     if(F->npad > F->n) pad_diagonal_kernel<<<(F->npad - F->n + 255) / 256, 256, 0, s>>>(F->H, F->npad, F->n, F->npad);
     int info = -1;
-    bool ok = chol_scratch_create(&F->chol) && chol_factor(F->H, F->npad, F->n, F->invL, F->info, s, nullptr, &F->chol) &&
+    bool ok = chol_scratch_create(&F->chol, F->npad) && chol_factor(F->H, F->npad, F->n, F->invL, F->info, s, nullptr, &F->chol) &&
               cudaMemcpyAsync(&info, F->info, sizeof(int), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
               cudaStreamSynchronize(s) == cudaSuccess;
     if(!ok)
@@ -154,10 +154,11 @@ extern "C" double mrcal_b200_factorization_rcond(mrcal_b200_factorization_t* F)
     return r * r;
 }
 
-// Timing aid for kernel development (scripts/time_cholesky.py); not declared in the public header
-extern "C" double mrcal_b200_debug_time_cholesky(int n, int reps, int kinds, int graph)
+// Timing aid for kernel development (scripts/time_cholesky.py); not declared in the public header.
+// what: 0 the factorization, 1 the backward substitution
+extern "C" double mrcal_b200_debug_time_cholesky(int n, int reps, int what)
 {
-    return chol_debug_time(n, reps, kinds, graph);
+    return chol_debug_time(n, reps, what);
 }
 namespace mb200 { bool chol_debug_spine_stamps(int n, long long* out, int nmax); }
 extern "C" bool mrcal_b200_debug_spine_stamps(int n, long long* out, int nmax) { return mb200::chol_debug_spine_stamps(n, out, nmax); }

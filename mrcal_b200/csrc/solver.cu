@@ -248,7 +248,7 @@ static bool build_workspace(mrcal_b200_problem* P)
     ws->h_ictl = ws->h_info + 8;
     MB200_CUDA_CHECK(cudaHostGetDevicePointer((void**)&ws->h_scal_dev, ws->h_scal, 0));
     MB200_CUDA_CHECK(cudaHostGetDevicePointer((void**)&ws->h_info_dev, ws->h_info, 0));
-    if(!chol_scratch_create(&ws->chol)) return false;
+    if(!chol_scratch_create(&ws->chol, N.ldS_max)) return false;
     MB200_CUDA_CHECK(cudaMemcpyAsync(N.grp_ptr, ptr.data(), ptr.size() * sizeof(int), cudaMemcpyHostToDevice, P->stream));
     if(!items.empty())
         MB200_CUDA_CHECK(cudaMemcpyAsync(N.grp_items, items.data(), items.size() * sizeof(int), cudaMemcpyHostToDevice, P->stream));
@@ -668,7 +668,7 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
                 T->spans[2].push_back({a, T->mark()});
                 const int b = T->mark();
                 if(!normal_extract_y(N, ws->rhs, s, nl)) return false;
-                if(N.n_c > 0 && !chol_solve_backward(N.S, N.ldS, ws->invL, ws->rhs, N.ldS, N.info + 1, s, nl, &ws->chol, run_if)) return false;
+                if(N.n_c > 0 && !chol_solve_backward(N.S, N.ldS, ws->invL, ws->rhs, N.info + 1, s, nl, &ws->chol, run_if)) return false;
                 if(!normal_expand_step(P->dp, N, P->op[P->cur], *lambda, ws->rhs, ws->ds_r, ws->step_gn, s, nl)) return false;
                 dots_kernel<<<3, 1024, 0, s>>>(ws->step_gn, N.g_full, e0, e1, Nstate, ws->scal + 11);
                 (*nl)++;

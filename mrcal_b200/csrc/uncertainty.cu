@@ -571,7 +571,8 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
     // 1-2. the Jacobian at the current state, and the factor: the structured one where the solver's atomics-free
     // assembly builds its panels; otherwise the dense Cholesky factor of J'J, with every unknown "shared"
     DeviceArena mem;
-    struct ForgetGraphs { const void* A = nullptr; ~ForgetGraphs() { if(A) chol_forget_graphs(A); } } forget;   // before mem frees it
+    // the dense route's factorization: its scratch, and the CUDA graphs that reference H (before mem frees it)
+    struct DenseChol { CholScratch sc; const void* A = nullptr; ~DenseChol() { if(A) chol_forget_graphs(A); chol_scratch_destroy(&sc); } } chol;
     mrcal_b200_factorization F;   // its buffers only: it does not own P here
     F.P = P;
     bool other_path = false, dense = false;
@@ -593,13 +594,13 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
         int *info = nullptr, *cid = nullptr, *tp = nullptr, *tsrc = nullptr, *trow = nullptr;
         if(!mem.alloc(&H, (size_t)npad * npad) || !mem.alloc(&invLd, (size_t)npad * TB) || !mem.alloc(&info, 1) ||
            !mem.alloc(&cid, (size_t)Nstate)) return false;
-        forget.A = H;
+        chol.A = H;
         MB200_CUDA_CHECK(cudaMemsetAsync(H, 0, (size_t)npad * npad * sizeof(double), s));
         if(!csr_stable_transpose(P->d_rowptr, op.Jcol, L.Nmeas, P->nnz, Nstate, mem, &tp, &tsrc, &trow, s)) return false;
         dense_jtj_kernel<<<(npad + 127) / 128, 128, 0, s>>>(P->d_rowptr, op.Jcol, op.Jval, tp, tsrc, trow, Nstate, H, npad);
         iota_kernel<<<(Nstate + 255) / 256, 256, 0, s>>>(cid, Nstate);
         int h_info = 0;
-        if(!chol_factor(H, npad, Nstate, invLd, info, s, nullptr)) return false;
+        if(!chol_scratch_create(&chol.sc, npad) || !chol_factor(H, npad, Nstate, invLd, info, s, nullptr, &chol.sc)) return false;
         MB200_CUDA_CHECK(cudaMemcpyAsync(&h_info, info, sizeof(int), cudaMemcpyDeviceToHost, s));
         MB200_CUDA_CHECK(cudaStreamSynchronize(s));
         if(h_info != 0) { set_error("JtJ is not positive definite"); return false; }

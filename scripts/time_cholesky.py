@@ -1,20 +1,35 @@
 #!/usr/bin/env python3
-"""Warm device timings of the dense Cholesky and of its kernel kinds. usage: time_cholesky.py n [n...]"""
+"""Warm device timings of the dense Cholesky: the factorization (net of the refill with an SPD matrix that every call
+needs; the persistent kernel up to n = 8192, the multi-kernel chain above) and the persistent backward substitution of
+one right-hand side. One line per size, then one JSON line
+with the card's name and power limit, read in the same run. usage: time_cholesky.py n [n...]"""
 import ctypes as C
+import json
+import subprocess
 import sys
 sys.path.insert(0, ".")
 from mrcal_b200 import _capi
 f = _capi.lib.mrcal_b200_debug_time_cholesky
+f.argtypes = [C.c_int, C.c_int, C.c_int]
 f.restype = C.c_double
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, limit = [s.strip() for s in out.split(",")]
+        return name, limit
+    except Exception:
+        return "unknown", "unknown"
+
+
+res = {}
 for n in [int(a) for a in sys.argv[1:]] or [1268, 4820]:
-    full_g = f(n, 10, 15, 1)
-    full_d = f(n, 10, 15, 0)
-    parts = {name: f(n, 10, k, 1) for name, k in (("potrf_diag", 1), ("trsm", 2), ("syrk_panel", 4), ("syrk_trailing", 8))}
+    factor, backward = f(n, 10, 0), f(n, 20, 1)
+    assert factor > 0 and backward > 0, f"n={n}: the timing aid failed"
     gf = n ** 3 / 3 / 1e9
-    print(f"n={n}: multi-kernel graph {full_g:.3f} ms ({gf / full_g:.1f} TFLOP/s, GFLOP={gf:.2f}), direct launches {full_d:.3f} ms; "
-          + ", ".join(f"{k} {v:.3f}" for k, v in parts.items()))
-    if n <= 8192:
-        fill = f(n, 10, 33, 0)
-        df = f(n, 10, 32, 0) - fill
-        print(f"n={n}: persistent factorization {df:.3f} ms ({gf / df:.1f} TFLOP/s); backward substitution: persistent {f(n, 20, 64, 0):.4f} ms, "
-              f"multi-kernel graph {f(n, 20, 128, 0):.4f} ms")
+    print(f"n={n}: factorization {factor:.3f} ms ({gf / factor:.1f} TFLOP/s, GFLOP={gf:.2f}); backward substitution {backward:.4f} ms")
+    res[n] = {"factor_ms": round(factor, 4), "backward_ms": round(backward, 5)}
+name, limit = card()
+print(json.dumps({"cholesky": res, "card": name, "power_limit": limit}))

@@ -1,7 +1,7 @@
 """The factorization object (stand-in for mrcal.CHOLMOD_factorization). The
 known-answer case is the reference's test/test-CHOLMOD-factorization.py; the
-larger cases exercise the blocked DMMA Cholesky (several 64-blocks and
-256-panels) against numpy."""
+larger cases exercise the DMMA Cholesky against numpy, from one 64-block to
+130 of them (the persistent kernel up to 128 blocks, the multi-kernel one above)."""
 import numpy as np
 import scipy.linalg
 import pytest
@@ -37,14 +37,14 @@ def test_reference_known_answer():
     assert np.allclose(F.solve_xt_JtJ_bt(bt, sys="L"), np.linalg.solve(L, bt.T).T, rtol=1e-12)
 
 
-@pytest.mark.parametrize("n,m,density", [(50, 200, 0.2), (64, 300, 0.1), (200, 1500, 0.05), (700, 6000, 0.02),
-                                         (1100, 9000, 0.01)])
+# n = 100: two 64-blocks; n = 8300: 130 of them
+@pytest.mark.parametrize("n,m,density", [(50, 200, 0.2), (64, 300, 0.1), (100, 400, 0.1), (200, 1500, 0.05), (700, 6000, 0.02),
+                                         (1100, 9000, 0.01), (8300, 9000, 0.0005)])
 def test_random_sparse(n, m, density):
     rng = np.random.default_rng(n)
     J = scipy.sparse.random(m, n, density=density, random_state=np.random.RandomState(n), format="csr")
     J = (J + scipy.sparse.vstack([scipy.sparse.eye(n) * 0.5, scipy.sparse.csr_matrix((m - n, n))])).tocsr()
-    Jd = J.toarray()
-    H = Jd.T @ Jd
+    H = (J.T @ J).toarray()
     bt = rng.normal(size=(3, n))
     F = mrcal_b200.CHOLMOD_factorization(J)
     xt = F.solve_xt_JtJ_bt(bt)
