@@ -656,6 +656,42 @@ bool mrcal_b200_stereo_unproject(mrcal_point3_t* p, double* range,
                                  mrcal_lensmodel_type_t rectification_model_type,
                                  const double* fxycxy_rectified, double baseline);
 
+/* The reprojection map between two camera models, as mrcal.image_transformation_map() computes it
+   (mrcal/image_transforms.py:276-511): mapxy [H_to][W_to][2] (float32) is, for each pixel of model_to's imager, the
+   pixel of model_from that sees the same point. Each pixel is unprojected through model_to, then
+   - Rt_to_from [4][3] (R, then t) NULL: the cameras share their frame (intrinsics_only)
+   - plane_n [3] given: A_from_to v, with A_to_from = plane_d R_to_from + t_to_from plane_n'
+   - distance given: invert_Rt(Rt_to_from) applied to normalize(v) * (*distance)
+   - otherwise (at infinity): R_to_from' v
+   and projected through model_from in fp64. region [Nregion] (a closed polygon in model_from's pixels) or NULL: map
+   points outside it, by the even-odd rule, and NaN points become (-1, -1). Two passes on the device, one thread per
+   pixel. Refuses a CAHVORE model_to with E != 0. False + mrcal_b200_last_error() on refusal or failure */
+bool mrcal_b200_image_transformation_map(float* mapxy, int W_to, int H_to,
+                                         const mrcal_lensmodel_t* lensmodel_from, const double* intrinsics_from,
+                                         const mrcal_lensmodel_t* lensmodel_to, const double* intrinsics_to,
+                                         const double* Rt_to_from, const double* distance,
+                                         const double* plane_n, double plane_d,
+                                         const mrcal_point2_t* region, int Nregion);
+
+/* An image remapped through a map, as mrcal.transform_image() (cv2.remap()) computes it, pixel for pixel: out
+   [H_out][W_out][channels] (packed) from image [H][W][channels] (rows image_stride bytes apart) and mapxy
+   [H_out][W_out][2] (float32, packed). type: an MRCAL_B200_IMAGE_* element type; channels: 1 or 3; interpolation:
+   MRCAL_B200_INTER_*; border_mode: MRCAL_B200_BORDER_* (OpenCV's values). border_value [channels]: the value of
+   pixels outside the image under BORDER_CONSTANT. Under BORDER_TRANSPARENT those output pixels keep what out held.
+   One thread per output pixel. False + mrcal_b200_last_error() on refusal or failure */
+enum { MRCAL_B200_IMAGE_UINT8 = 0, MRCAL_B200_IMAGE_UINT16 = 1, MRCAL_B200_IMAGE_FLOAT = 2 };
+enum { MRCAL_B200_INTER_NEAREST = 0, MRCAL_B200_INTER_LINEAR = 1 };
+enum { MRCAL_B200_BORDER_CONSTANT = 0, MRCAL_B200_BORDER_TRANSPARENT = 5 };
+bool mrcal_b200_transform_image(void* out, const void* image, int W, int H, int image_stride, int type, int channels,
+                                const float* mapxy, int W_out, int H_out, int interpolation, int border_mode,
+                                const double* border_value);
+/* The same with every buffer on the device: the kernel is enqueued on stream (a cudaStream_t; NULL: the default
+   stream) and the call returns without waiting for it. image, out and image_stride must be aligned to the element
+   size, mapxy to 4 bytes (a float); a buffer that is not is refused */
+bool mrcal_b200_transform_image_device(void* out, const void* image, int W, int H, int image_stride, int type,
+                                       int channels, const float* mapxy, int W_out, int H_out, int interpolation,
+                                       int border_mode, const double* border_value, void* stream);
+
 // Timing hook for benchmarks: run N cost-function evaluations (residuals +
 // Jacobian) at the current state back to back, return the mean device time per
 // evaluation in milliseconds (CUDA events on the library's stream); <0 on error

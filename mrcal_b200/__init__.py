@@ -24,6 +24,10 @@ from .seeding import (  # noqa: F401
 from .stereo import (  # noqa: F401
     rectified_resolution, rectified_system, rectification_maps, stereo_range, stereo_unproject,
 )
+from .image_transforms import (  # noqa: F401
+    scale_focal__best_pinhole_fit, pinhole_model_for_reprojection, image_transformation_map, transform_image,
+    INTER_NEAREST, INTER_LINEAR, BORDER_CONSTANT, BORDER_TRANSPARENT,
+)
 from .cameramodel import cameramodel, CameramodelParseException  # noqa: F401
 from ._capi import lib as _lib
 
