@@ -587,22 +587,24 @@ def optimizer_callback(no_jacobian=False, no_factorization=False, **kwargs):
         P, Ii, X = keep
         J = scipy.sparse.csr_matrix((X, Ii, P), shape=(Nmeas, Nstate))
         if not no_factorization:
-            # the problem's own structure first (frames/points eliminated, dense factor of the reduced system only);
-            # the dense Nstate x Nstate object only where that does not apply
-            if not os.environ.get("MRCAL_B200_DENSE_FACTORIZATION"):
+            # the problem's own structure (frames/points eliminated, dense factor of the reduced system only); the dense
+            # Nstate x Nstate object on request.
+            # "JtJ is not positive definite" is not an error here: mrcal-pywrap.c:1981-1988 returns None. Anything else
+            # (out of memory, a CUDA failure) is one
+            if os.environ.get("MRCAL_B200_DENSE_FACTORIZATION"):
+                try:
+                    factorization = CHOLMOD_factorization(J)
+                except RuntimeError as e:
+                    if "not positive definite" not in str(e):
+                        raise
+                    factorization = None
+            else:
                 h = lib.mrcal_b200_factorization_create_from_last_callback()   # NULL comes back as None
                 if h:
-                    return b, x, J, CHOLMOD_factorization._from_handle(h, J.shape)
-                if "not positive definite" in _capi.last_error():
-                    return b, x, J, None   # not an error: mrcal-pywrap.c:1981-1988
-            try:
-                factorization = CHOLMOD_factorization(J)
-            except RuntimeError as e:
-                # "JtJ is not positive definite" is not an error here: mrcal-pywrap.c:1981-1988 returns None.
-                # Anything else (out of memory, a CUDA failure) is one
-                if "not positive definite" not in str(e):
-                    raise
-                factorization = None
+                    factorization = CHOLMOD_factorization._from_handle(h, J.shape)
+                elif "not positive definite" not in _capi.last_error():
+                    raise RuntimeError("mrcal_optimizer_callback(): factorization failed: " + _capi.last_error() +
+                                       " (MRCAL_B200_DENSE_FACTORIZATION=1 gives the dense factorization of J'J instead)")
     return b, x, J, factorization
 
 

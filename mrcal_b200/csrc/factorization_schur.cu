@@ -357,9 +357,8 @@ __global__ void rank_inactive_kernel(NormalBuffers N, int* __restrict__ ia_rank)
 // Builds the structured factor of P at its current state into F (F->P is set by the caller; F does not own P here).
 // False, with the reason in the error string, if P is sharded or JtJ is not positive definite. The device problem's
 // solver workspace holds L_S and the panels afterwards (they are what the next solver iteration overwrites)
-bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F, bool* other_path)
+bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F)
 {
-    if(other_path) *other_path = false;
     if(comm_active() || P->sharded) { set_error("structured factorization: not available for sharded problems"); return false; }
     if(!solver_build_workspace(P)) return false;
     SolverWorkspace* ws = P->ws.get();
@@ -368,12 +367,6 @@ bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F, bool
     int nl = 0;
     if(!problem_evaluate(P, P->cur, true, true) ||
        !normal_assemble(P->dp, N, P->op[P->cur], P->d_rowptr, 0., s, &nl)) return false;
-    if(!N.det)
-    {
-        if(other_path) *other_path = true;
-        set_error("structured factorization: this problem takes the other assembly path");
-        return false;
-    }
     int h_info[2] = {0, 0}, h_bad = 0;
     if(N.n_c > 0 && !chol_factor(N.S, N.ldS, N.n_c, ws->invL, N.info + 1, s, &nl, &ws->chol)) return false;
     clear_aug_rows_kernel<<<(N.ldS + 255) / 256, 256, 0, s>>>(N, N.n_c, ws->invL);

@@ -16,8 +16,6 @@
 // only the reduced result goes to global memory. For splined models the touched
 // knot columns are data-dependent (mrcal.c:2171-2185), so each CTA discovers
 // its own local column set every time.
-#include <vector>
-
 #include "normal_items.cuh"
 #include "chol.h"
 
@@ -136,10 +134,13 @@ compact_scan_kernel(NormalBuffers N)
     if(tid == 1023) N.stat[0] = s_scan[1023];
 }
 
-// Pass 2, one CTA per work item: the Gram matrix of the item's rows over its local columns
-__global__ void __launch_bounds__(256)
+// Pass 2, one CTA per work item: the Gram matrix of the item's rows over its local columns. The tensor-pipe kernel below
+// takes the items up to kDmmaMaxCols local columns; this one the wider ones (splined observations that touch many knots).
+// Like that kernel, it leaves the shared x shared block and -J'x in the item's own block of the pool and B, D, gf in the
+// item's slots; normal_det.cu sums the blocks into S in a fixed order
+__global__ void __launch_bounds__(256, 1)
 assemble_items_kernel(DevProblem P, NormalBuffers N, int gram_cap, const double* __restrict__ x,
-                      const double* __restrict__ Jval, const int* __restrict__ Jcol)
+                      const double* __restrict__ Jval, const int* __restrict__ Jcol, int w0)
 {
     extern __shared__ __align__(16) double dsm[];
     __shared__ short s_lidx[2][RCH][kMaxRowNnz];
@@ -147,18 +148,19 @@ assemble_items_kernel(DevProblem P, NormalBuffers N, int gram_cap, const double*
     __shared__ double s_xr[2][RCH];
     __shared__ unsigned char s_pa[kMaxRowNnz * (kMaxRowNnz + 1) / 2], s_pb[kMaxRowNnz * (kMaxRowNnz + 1) / 2];
 
-    const int w = blockIdx.x, tid = threadIdx.x;
+    const int w = blockIdx.x + w0, tid = threadIdx.x;
     const ItemDesc d = describe_item(P, w, N.Nframe_groups);
     const int ncam = d.cam0 >= 0 ? 6 : 0, nwarp = d.warp0 >= 0 ? 2 : 0;
     const int nsh = N.wi_nsh[w], nloc = nsh - ncam - nwarp, ntot = nsh + d.nelim;
-    const bool big = ntot > gram_cap;   // Gram matrix does not fit: shared x shared goes straight to global
+    // Gram matrix does not fit: shared x shared is summed in the item's block of the pool, which only this CTA touches
+    const bool big = ntot > gram_cap;
+    double* Aw = N.wi_A + N.wi_Aoff[w];
+    const int lda = N.wi_lda[w];
 
-    // shared-memory carve-up: lmap [clen] shorts | ccol [nsh] ints | gram | gvec [ntot]
+    // shared-memory carve-up: lmap [clen] shorts | gram | gvec [ntot]
     short* lmap = reinterpret_cast<short*>(dsm);
     const int lmap_doubles = (d.clen * (int)sizeof(short) + 7) / 8;
-    int* ccol = reinterpret_cast<int*>(dsm + lmap_doubles);               // compact index of each local column
-    const int ccol_doubles = (N.cap * (int)sizeof(int) + 7) / 8;
-    double* gram = dsm + lmap_doubles + ccol_doubles;
+    double* gram = dsm + lmap_doubles;
     const int ngram = big ? d.nelim * ntot : ntot * (ntot + 1) / 2;
     double* gvec = gram + ngram;   // [ntot] J'x of this item
 
@@ -174,13 +176,10 @@ assemble_items_kernel(DevProblem P, NormalBuffers N, int gram_cap, const double*
         s_pb[e] = (unsigned char)(e - a * (a + 1) / 2);
     }
     for(int i = tid; i < ngram + ntot; i += 256) gram[i] = 0.;
+    if(big) for(int i = tid; i < nsh * lda; i += 256) Aw[i] = 0.;
     __syncthreads();
-    for(int l = tid; l < nsh; l += 256)
-    {
-        const int r = cols[l];
-        ccol[l] = N.cidx[r];
-        if(l < nloc) lmap[r - d.cbase] = (short)l;   // intrinsics columns sit before the eliminated range: reduced == state index
-    }
+    // intrinsics columns sit before the eliminated range: reduced == state index
+    for(int l = tid; l < nloc; l += 256) lmap[cols[l] - d.cbase] = (short)l;
     __syncthreads();
 
     // Rows are consumed in chunks of RCH: while one chunk is being accumulated, the (column, value)
@@ -247,7 +246,7 @@ assemble_items_kernel(DevProblem P, NormalBuffers N, int gram_cap, const double*
                 if(la < lb) { const int t = la; la = lb; lb = t; }
                 if(!big) gram[tri(la, lb)] += v;
                 else if(la >= nsh) gram[(la - nsh) * ntot + lb] += v;            // eliminated x anything
-                else atomicAdd(&N.S[(size_t)ccol[la] * N.ldS + ccol[lb]], v);      // shared x shared
+                else Aw[(size_t)la * lda + lb] += v;                              // shared x shared
             }
             if(tid >= 224 && tid < 224 + d.nnz_row) gvec[lidx[tid - 224]] += val[tid - 224] * s_xr[buf][rr];
             // two different rows can hit the same Gram entry from different threads: one barrier per row.
@@ -257,24 +256,21 @@ assemble_items_kernel(DevProblem P, NormalBuffers N, int gram_cap, const double*
     }
 
     // ---- write out
-    // shared x shared -> S (lower triangle, compact numbering; local order == global order)
+    // shared x shared -> the item's block (every entry of the lower triangle, zeros included)
     if(!big)
         for(int e = tid; e < nsh * (nsh + 1) / 2; e += 256)
         {
             int a = (int)((sqrt(8. * e + 1.) - 1.) * 0.5);
             while(a * (a + 1) / 2 > e) a--;
             while((a + 1) * (a + 2) / 2 <= e) a++;
-            const int b = e - a * (a + 1) / 2;
-            const double v = gram[e];
-            if(v != 0.) atomicAdd(&N.S[(size_t)ccol[a] * N.ldS + ccol[b]], v);
+            Aw[(size_t)a * lda + (e - a * (a + 1) / 2)] = gram[e];
         }
-    // gradient of the shared unknowns: into g' (completed by the Schur kernel) and into the full J'x
+    // rows nsh and nsh+1 of the block: -J'x over the shared columns, as the tensor-pipe kernel leaves them
     for(int l = tid; l < nsh; l += 256)
-        if(gvec[l] != 0.)
-        {
-            atomicAdd(&N.gs[ccol[l]], gvec[l]);
-            atomicAdd(&N.g_full[N.state_index(cols[l])], gvec[l]);
-        }
+    {
+        Aw[(size_t)nsh * lda + l] = -gvec[l];
+        Aw[(size_t)(nsh + 1) * lda + l] = -gvec[l];
+    }
     // eliminated block of this item: B (nelim x nsh), D (nelim x nelim), gf (nelim)
     if(d.nelim > 0)
     {
@@ -305,8 +301,7 @@ assemble_items_kernel(DevProblem P, NormalBuffers N, int gram_cap, const double*
 // 30 nonzeros of each row), every warp owns a fixed set of 8x8 tiles of the lower triangle of G
 // and keeps them in registers for the whole item; the x column makes J'x the last row of G.
 // 3 barriers per 32 rows instead of one per row, ~10x fewer shared-memory transactions than
-// the scalar kernel above (which remains the fallback for items with more than kDmmaMaxCols
-// local columns).
+// the scalar kernel above (which takes the items with more than kDmmaMaxCols local columns).
 constexpr int kDmmaMaxCols = 160;                       // ntot + 1, padded to 8
 constexpr int DCH = 32;                                 // rows per chunk
 // Three instantiations by item width, so that the common narrow items do not pay the register
@@ -315,7 +310,7 @@ constexpr int kDmmaClassT[3]     = {10, 16, 20};
 constexpr int kDmmaClassTiles[3] = {7, 17, 27};
 
 
-template <int kDmmaMaxTiles, int TMIN, int TMAX, bool DET>
+template <int kDmmaMaxTiles, int TMIN, int TMAX>
 __global__ void __launch_bounds__(256)
 assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double* __restrict__ x,
                            const double* __restrict__ Jval, const int* __restrict__ Jcol, int w0)
@@ -336,12 +331,10 @@ assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double*
     const int ncols = ntot + 1;                         // + the x column
     const int T = (ncols + 7) >> 3, ntiles = T * (T + 1) / 2;
 
-    // shared-memory carve-up: lmap [clen] shorts | ccol [cap] ints | D [DCH][ldD]
+    // shared-memory carve-up: lmap [clen] shorts | D [DCH][ldD]
     short* lmap = reinterpret_cast<short*>(dsm);
     const int lmap_doubles = (d.clen * (int)sizeof(short) + 7) / 8;
-    int* ccol = reinterpret_cast<int*>(dsm + lmap_doubles);
-    const int ccol_doubles = (N.cap * (int)sizeof(int) + 7) / 8;
-    double* D = dsm + lmap_doubles + ccol_doubles;
+    double* D = dsm + lmap_doubles;
 
     const int* cols = N.wi_cols + (size_t)w * N.cap;
     for(int i = tid; i < d.clen; i += 256) lmap[i] = -1;
@@ -356,12 +349,7 @@ assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double*
         s_tj[q] = (unsigned char)(q - ti * (ti + 1) / 2);
     }
     __syncthreads();
-    for(int l = tid; l < nsh; l += 256)
-    {
-        const int r = cols[l];
-        ccol[l] = N.cidx[r];
-        if(l < nloc) lmap[r - d.cbase] = (short)l;
-    }
+    for(int l = tid; l < nloc; l += 256) lmap[cols[l] - d.cbase] = (short)l;
     __syncthreads();
 
     double acc[kDmmaMaxTiles][2];
@@ -459,10 +447,10 @@ assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double*
 
     // ---- write out from the accumulators. Lane holds G[8 ti + g][8 tj + 2t + {0,1}]
     double* B = N.wi_B + (size_t)w * 6 * N.cap;
-    // DET: the shared x shared block and the gradient go to this item's own block of the pool (every entry of
-    // the lower triangle exactly once, zeros included); normal_det.cu sums the blocks into S in a fixed order
-    double* Aw = DET ? N.wi_A + N.wi_Aoff[w] : nullptr;
-    const int lda = DET ? N.wi_lda[w] : 0;
+    // the shared x shared block and the gradient go to this item's own block of the pool (every entry of the lower
+    // triangle exactly once, zeros included); normal_det.cu sums the blocks into S in a fixed order
+    double* Aw = N.wi_A + N.wi_Aoff[w];
+    const int lda = N.wi_lda[w];
 #pragma unroll
     for(int i = 0; i < kDmmaMaxTiles; i++)
     {
@@ -476,11 +464,7 @@ assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double*
             const double v = acc[i][h];
             // lower triangle (incl. diagonal) of the (ntot+1)^2 Gram matrix; the (x,x) corner is |x|^2: unused
             if(row > ntot || col > row || col >= ntot) continue;
-            if(row < nsh)
-            {
-                if constexpr(DET) Aw[(size_t)row * lda + col] = v;
-                else if(v != 0.) atomicAdd(&N.S[(size_t)ccol[row] * N.ldS + ccol[col]], v);   // shared x shared
-            }
+            if(row < nsh) Aw[(size_t)row * lda + col] = v;                                      // shared x shared
             else if(row < ntot)
             {
                 const int p = row - nsh;
@@ -496,18 +480,10 @@ assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double*
             {
                 if(col < nsh)
                 {
-                    if constexpr(DET)
-                    {
-                        // rows nsh and nsh+1 of the block: -J'x (the right-hand side rides through the factorization
-                        // as row n_c of S; row n_c+1 collects the plain gradient)
-                        Aw[(size_t)nsh * lda + col] = -v;
-                        Aw[(size_t)(nsh + 1) * lda + col] = -v;
-                    }
-                    else if(v != 0.)
-                    {
-                        atomicAdd(&N.gs[ccol[col]], v);
-                        atomicAdd(&N.g_full[N.state_index(cols[col])], v);
-                    }
+                    // rows nsh and nsh+1 of the block: -J'x (the right-hand side rides through the factorization as
+                    // row n_c of S; row n_c+1 collects the plain gradient)
+                    Aw[(size_t)nsh * lda + col] = -v;
+                    Aw[(size_t)(nsh + 1) * lda + col] = -v;
                 }
                 else N.wi_gf[(size_t)w * 6 + (col - nsh)] = v;
             }
@@ -518,45 +494,6 @@ assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double*
     {
         if(tid < 36) { const int p = tid / 6, qq = tid % 6; if(p >= d.nelim || qq >= d.nelim) N.wi_D[(size_t)w * 36 + tid] = 0.; }
         if(tid >= 64 && tid < 70 && tid - 64 >= d.nelim) N.wi_gf[(size_t)w * 6 + tid - 64] = 0.;
-    }
-}
-
-// Regularization rows touch shared unknowns only: one thread per row. A row whose unknowns are
-// inactive (touched by no observation) stays out of S: inactive_step_kernel deals with it
-// (Also used for the triangulated-point rows [m_begin, m_end) = [m_tri0, m_reg0): extrinsics only.)
-// det_nc >= 0 (the atomics-free path, triangulated rows only): the gradients go to rows det_nc, det_nc+1 of S, which is
-// where that path keeps g' and the plain gradient
-__global__ void assemble_reg_kernel(DevProblem P, NormalBuffers N, const double* __restrict__ x,
-                                    const double* __restrict__ Jval, const int* __restrict__ Jcol,
-                                    const int* __restrict__ rowptr, int m_begin, int m_end, int det_nc)
-{
-    const int m = m_begin + blockIdx.x * blockDim.x + threadIdx.x;
-    if(m >= m_end || !P.reg_owner) return;
-    const int j0 = rowptr[m], j1 = rowptr[m + 1];
-    const double xm = x[m];
-    bool all_active = true;
-    for(int a = j0; a < j1; a++)
-    {
-        if(det_nc < 0) atomicAdd(&N.g_full[Jcol[a]], Jval[a] * xm);
-        if(N.cidx[N.reduced_index(Jcol[a])] < 0) all_active = false;
-    }
-    if(!all_active) return;
-    for(int a = j0; a < j1; a++)
-    {
-        const int ca = N.cidx[N.reduced_index(Jcol[a])];
-        const double va = Jval[a];
-        if(det_nc < 0) atomicAdd(&N.gs[ca], va * xm);
-        else
-        {
-            atomicAdd(&N.S[(size_t)det_nc * N.ldS + ca], -va * xm);
-            atomicAdd(&N.S[(size_t)(det_nc + 1) * N.ldS + ca], -va * xm);
-        }
-        for(int b = j0; b <= a; b++)
-        {
-            const int cb = N.cidx[N.reduced_index(Jcol[b])];
-            const int hi = ca > cb ? ca : cb, lo = ca > cb ? cb : ca;
-            atomicAdd(&N.S[(size_t)hi * N.ldS + lo], va * Jval[b] * ((ca == cb && a != b) ? 2. : 1.));
-        }
     }
 }
 
@@ -612,205 +549,6 @@ __global__ void inactive_step_kernel(DevProblem P, NormalBuffers N, double lambd
     step_full[c] = step;
 }
 
-// 6x6 (or 3x3) SPD inverse by Cholesky, in registers of one thread. Returns false if not PD
-__device__ bool spd_inverse(double* Dinv, const double* D, int n)
-{
-    double L[6][6] = {};
-    for(int j = 0; j < n; j++)
-    {
-        double s = D[j * 6 + j];
-        for(int k = 0; k < j; k++) s -= L[j][k] * L[j][k];
-        if(!(s > 0.)) return false;
-        L[j][j] = sqrt(s);
-        for(int i = j + 1; i < n; i++)
-        {
-            double t = D[i * 6 + j];
-            for(int k = 0; k < j; k++) t -= L[i][k] * L[j][k];
-            L[i][j] = t / L[j][j];
-        }
-    }
-    double X[6][6] = {};   // inv(L)
-    for(int c = 0; c < n; c++)
-    {
-        X[c][c] = 1. / L[c][c];
-        for(int i = c + 1; i < n; i++)
-        {
-            double t = 0.;
-            for(int k = c; k < i; k++) t += L[i][k] * X[k][c];
-            X[i][c] = -t / L[i][i];
-        }
-    }
-    for(int i = 0; i < 6; i++)
-        for(int j = 0; j < 6; j++)
-        {
-            double t = 0.;
-            if(i < n && j < n)
-                for(int k = (i > j ? i : j); k < n; k++) t += X[k][i] * X[k][j];
-            Dinv[i * 6 + j] = t;
-        }
-    return true;
-}
-
-// One CTA per elimination group (a frame, or a point): S -= B' D^-1 B over all
-// pairs of the group's items, g' = gs - B' D^-1 gf
-__global__ void __launch_bounds__(256, 4)
-schur_groups_kernel(NormalBuffers N, double lambda, int ldc)
-{
-    extern __shared__ __align__(16) double dsm[];   // C1[6][cap]
-    __shared__ double s_Dinv[36], s_h[6], s_D[36], s_gf[6];
-    __shared__ int s_ok;
-    const int grp = blockIdx.x, tid = threadIdx.x;
-    const int i0 = N.grp_ptr[grp], i1 = N.grp_ptr[grp + 1];
-    const int nelim = grp < N.Nframe_groups ? 6 : 3;
-    if(tid < 36)
-    {
-        double v = 0.;
-        for(int i = i0; i < i1; i++) v += N.wi_D[(size_t)N.grp_items[i] * 36 + tid];
-        const int p = tid / 6, q = tid % 6;
-        if(p == q && p < nelim) v += lambda;
-        s_D[tid] = v;
-    }
-    if(tid >= 64 && tid < 70)
-    {
-        double v = 0.;
-        for(int i = i0; i < i1; i++) v += N.wi_gf[(size_t)N.grp_items[i] * 6 + (tid - 64)];
-        s_gf[tid - 64] = v;
-    }
-    __syncthreads();
-    if(tid == 0)
-    {
-        double Dinv[36];
-        // a group nobody observes (or all of whose observations are outliers) has D = 0: the
-        // reference would hand CHOLMOD a singular matrix here (mrcal.c:4826-4833); report it
-        s_ok = spd_inverse(Dinv, s_D, nelim) ? 1 : 0;
-        if(!s_ok) { atomicCAS(N.info, 0, 1000000000 + grp); for(int i = 0; i < 36; i++) Dinv[i] = 0.; }
-        for(int i = 0; i < 36; i++) s_Dinv[i] = Dinv[i];
-        // the eliminated part of the full gradient
-        for(int p = 0; p < nelim && blockIdx.y == 0; p++) N.g_full[N.e0 + (grp < N.Nframe_groups ? 6 * grp : 6 * N.Nframe_groups + 3 * (grp - N.Nframe_groups)) + p] = s_gf[p];
-        for(int p = 0; p < 6; p++)
-        {
-            double t = 0.;
-            for(int q = 0; q < 6; q++) t += Dinv[p * 6 + q] * s_gf[q];
-            s_h[p] = t;
-        }
-    }
-    __syncthreads();
-    if(blockIdx.y == 0)
-    {
-        if(tid < 36) N.grp_Dinv[(size_t)grp * 36 + tid] = s_Dinv[tid];
-        if(tid < 6)  N.grp_gf[(size_t)grp * 6 + tid] = s_gf[tid];
-    }
-
-    // shared memory is sized by the widest item actually present (ldc), not by the capacity N.cap: more CTAs per SM,
-    // and this kernel lives on having many atomics in flight
-    double* C1 = dsm;                                      // [6][ldc]: Dinv B1
-    int* r1 = reinterpret_cast<int*>(dsm + 6 * ldc);       // [ldc] compact index of item 1's columns
-    int* r2 = r1 + ldc;                                    // [ldc] ... of item 2's
-    // blockIdx.y picks the pairs (a1, a2 <= a1) with a1 = i0 + blockIdx.y, + gridDim.y, ...: more CTAs than groups
-    for(int a1 = i0 + blockIdx.y; a1 < i1; a1 += gridDim.y)
-    {
-        const int w1 = N.grp_items[a1];
-        const int n1 = N.wi_nsh[w1];
-        const double* B1 = N.wi_B + (size_t)w1 * 6 * N.cap;
-        const int* c1 = N.wi_cols + (size_t)w1 * N.cap;
-        __syncthreads();
-        for(int e = tid; e < nelim * n1; e += 256)
-        {
-            const int p = e / n1, l = e - p * n1;
-            double t = 0.;
-            for(int q = 0; q < nelim; q++) t += s_Dinv[p * 6 + q] * B1[(size_t)q * N.cap + l];
-            C1[p * ldc + l] = t;
-        }
-        for(int l = tid; l < n1; l += 256) r1[l] = N.cidx[c1[l]];
-        __syncthreads();
-        // reduced gradient
-        for(int l = tid; l < n1; l += 256)
-        {
-            double t = 0.;
-            for(int p = 0; p < nelim; p++) t += B1[(size_t)p * N.cap + l] * s_h[p];
-            if(t != 0.) atomicAdd(&N.gs[r1[l]], -t);
-        }
-        for(int a2 = i0; a2 <= a1; a2++)
-        {
-            const int w2 = N.grp_items[a2];
-            const int n2 = N.wi_nsh[w2];
-            const double* __restrict__ B2 = N.wi_B + (size_t)w2 * 6 * N.cap;
-            const int* c2 = N.wi_cols + (size_t)w2 * N.cap;
-            const bool same = a1 == a2;
-            __syncthreads();
-            for(int l = tid; l < n2; l += 256) r2[l] = N.cidx[c2[l]];
-            __syncthreads();
-            for(int e = tid; e < n1 * n2; e += 256)
-            {
-                const int a = e / n2, b = e - a * n2;
-                if(same && b > a) continue;
-                double v = 0.;
-                for(int p = 0; p < nelim; p++) v += C1[p * ldc + a] * B2[(size_t)p * N.cap + b];
-                if(v == 0.) continue;
-                const int r = r1[a], c = r2[b];
-                if(r > c)       atomicAdd(&N.S[(size_t)r * N.ldS + c], -v);
-                else if(r < c)  atomicAdd(&N.S[(size_t)c * N.ldS + r], -v);
-                else            atomicAdd(&N.S[(size_t)r * N.ldS + r], same ? -v : -2. * v);
-            }
-        }
-    }
-}
-
-// df_j = -D_j^-1 (gf_j + B_j ds): one warp per group. ds is the reduced solution (npad, reduced numbering)
-__global__ void __launch_bounds__(256)
-backsub_groups_kernel(NormalBuffers N, const double* __restrict__ ds, double* __restrict__ step_full, int e0)
-{
-    const int grp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if(grp >= N.Ngroups) return;
-    const int nelim = grp < N.Nframe_groups ? 6 : 3;
-    double t[6] = {0., 0., 0., 0., 0., 0.};
-    for(int i = N.grp_ptr[grp]; i < N.grp_ptr[grp + 1]; i++)
-    {
-        const int w = N.grp_items[i];
-        const int n = N.wi_nsh[w];
-        const double* B = N.wi_B + (size_t)w * 6 * N.cap;
-        const int* c = N.wi_cols + (size_t)w * N.cap;
-        for(int l = lane; l < n; l += 32)
-        {
-            const double d = ds[c[l]];
-            for(int p = 0; p < nelim; p++) t[p] += B[(size_t)p * N.cap + l] * d;
-        }
-    }
-    for(int p = 0; p < 6; p++)
-        for(int o = 16; o > 0; o >>= 1) t[p] += __shfl_xor_sync(0xffffffffu, t[p], o);
-    if(lane < nelim)
-    {
-        double v = 0.;
-        for(int q = 0; q < nelim; q++) v += N.grp_Dinv[(size_t)grp * 36 + lane * 6 + q] * (N.grp_gf[(size_t)grp * 6 + q] + t[q]);
-        const int col = grp < N.Nframe_groups ? e0 + 6 * grp : e0 + 6 * N.Nframe_groups + 3 * (grp - N.Nframe_groups);
-        step_full[col + lane] = -v;
-    }
-}
-
-__global__ void set_diagonal_kernel(double* S, int ld, int i0, int i1, double v, bool add)
-{
-    const int i = i0 + blockIdx.x * blockDim.x + threadIdx.x;
-    if(i < i1) { if(add) S[(size_t)i * ld + i] += v; else S[(size_t)i * ld + i] = v; }
-}
-
-// shared part of J'x <-> a contiguous buffer in reduced numbering (for the cross-rank reduction)
-__global__ void gather_shared_kernel(NormalBuffers N, double* __restrict__ buf)
-{
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if(r < N.n_r) buf[r] = N.g_full[N.state_index(r)];
-}
-__global__ void scatter_shared_kernel(NormalBuffers N, const double* __restrict__ buf)
-{
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if(r < N.n_r) N.g_full[N.state_index(r)] = buf[r];
-}
-
-__global__ void augment_rhs_kernel(NormalBuffers N)
-{
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if(c < N.n_c) N.S[(size_t)N.n_c * N.ldS + c] = -N.gs[c];
-}
-
 // One-time, per-device kernel attributes
 static bool configure_kernels()
 {
@@ -820,21 +558,15 @@ static bool configure_kernels()
     if(dev < 0 || dev >= kMaxDevices) { set_error("device index %d out of range", dev); return false; }
     if(configured[dev]) return true;
     MB200_CUDA_CHECK(cudaFuncSetAttribute(assemble_items_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(schur_groups_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-#define MB200_CFG(DET)                                                                                                        \
-    MB200_CUDA_CHECK(cudaFuncSetAttribute((assemble_items_dmma_kernel<kDmmaClassTiles[0], 0, kDmmaClassT[0], DET>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); \
-    MB200_CUDA_CHECK(cudaFuncSetAttribute((assemble_items_dmma_kernel<kDmmaClassTiles[1], kDmmaClassT[0], kDmmaClassT[1], DET>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024)); \
-    MB200_CUDA_CHECK(cudaFuncSetAttribute((assemble_items_dmma_kernel<kDmmaClassTiles[2], kDmmaClassT[1], kDmmaClassT[2], DET>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    MB200_CFG(false)
-    MB200_CFG(true)
-#undef MB200_CFG
+    MB200_CUDA_CHECK(cudaFuncSetAttribute((assemble_items_dmma_kernel<kDmmaClassTiles[0], 0, kDmmaClassT[0]>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    MB200_CUDA_CHECK(cudaFuncSetAttribute((assemble_items_dmma_kernel<kDmmaClassTiles[1], kDmmaClassT[0], kDmmaClassT[1]>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    MB200_CUDA_CHECK(cudaFuncSetAttribute((assemble_items_dmma_kernel<kDmmaClassTiles[2], kDmmaClassT[1], kDmmaClassT[2]>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     configured[dev] = true;
     return true;
 }
 
-template <bool DET>
 static bool launch_gram_dmma(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, int Nwi, int max_ntot,
-                             size_t lmap_bytes, size_t ccol_bytes, cudaStream_t s, int* nlaunch, int w0 = 0)
+                             size_t lmap_bytes, cudaStream_t s, int* nlaunch, int w0)
 {
     Nwi -= w0;
     if(Nwi <= 0) return true;
@@ -842,7 +574,7 @@ static bool launch_gram_dmma(const DevProblem& dp, NormalBuffers& N, const EvalB
     const int ncols_pad = ((max_ntot + 1 + 7) / 8) * 8;
     const int Tmax = ncols_pad / 8;
     auto ld_for = [](int T) { int ld = 8 * T; while(ld % 16 != 4) ld++; return ld; };
-    auto smem_for = [&](int T) { return lmap_bytes + ccol_bytes + (size_t)DCH * ld_for(T) * sizeof(double); };
+    auto smem_for = [&](int T) { return lmap_bytes + (size_t)DCH * ld_for(T) * sizeof(double); };
     // The size classes touch disjoint items: they run side by side on forked streams (owned by the workspace),
     // so that the CTAs of one fill the tails of the other
     const bool c1 = Tmax > kDmmaClassT[0], c2 = Tmax > kDmmaClassT[1];
@@ -854,20 +586,20 @@ static bool launch_gram_dmma(const DevProblem& dp, NormalBuffers& N, const EvalB
     }
     {
         const int T0 = Tmax < kDmmaClassT[0] ? Tmax : kDmmaClassT[0];
-        assemble_items_dmma_kernel<kDmmaClassTiles[0], 0, kDmmaClassT[0], DET><<<Nwi, 256, smem_for(T0), s>>>(dp, N, ld_for(T0), op.x, op.Jval, op.Jcol, w0);
+        assemble_items_dmma_kernel<kDmmaClassTiles[0], 0, kDmmaClassT[0]><<<Nwi, 256, smem_for(T0), s>>>(dp, N, ld_for(T0), op.x, op.Jval, op.Jcol, w0);
         (*nlaunch)++;
     }
     if(c1)
     {
         const int T1 = Tmax < kDmmaClassT[1] ? Tmax : kDmmaClassT[1];
-        assemble_items_dmma_kernel<kDmmaClassTiles[1], kDmmaClassT[0], kDmmaClassT[1], DET><<<Nwi, 256, smem_for(T1), N.s_side[0]>>>(dp, N, ld_for(T1), op.x, op.Jval, op.Jcol, w0);
+        assemble_items_dmma_kernel<kDmmaClassTiles[1], kDmmaClassT[0], kDmmaClassT[1]><<<Nwi, 256, smem_for(T1), N.s_side[0]>>>(dp, N, ld_for(T1), op.x, op.Jval, op.Jcol, w0);
         MB200_CUDA_CHECK(cudaEventRecord(N.ev_join[0], N.s_side[0]));
         MB200_CUDA_CHECK(cudaStreamWaitEvent(s, N.ev_join[0], 0));
         (*nlaunch)++;
     }
     if(c2)
     {
-        assemble_items_dmma_kernel<kDmmaClassTiles[2], kDmmaClassT[1], kDmmaClassT[2], DET><<<Nwi, 256, smem_for(Tmax), N.s_side[1]>>>(dp, N, ld_for(Tmax), op.x, op.Jval, op.Jcol, w0);
+        assemble_items_dmma_kernel<kDmmaClassTiles[2], kDmmaClassT[1], kDmmaClassT[2]><<<Nwi, 256, smem_for(Tmax), N.s_side[1]>>>(dp, N, ld_for(Tmax), op.x, op.Jval, op.Jcol, w0);
         MB200_CUDA_CHECK(cudaEventRecord(N.ev_join[1], N.s_side[1]));
         MB200_CUDA_CHECK(cudaStreamWaitEvent(s, N.ev_join[1], 0));
         (*nlaunch)++;
@@ -902,9 +634,8 @@ bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& o
     if(rider_summed) *rider_summed = false;
     if(!configure_kernels()) return false;
     const size_t lmap_bytes = ((size_t)dp.Nintr_state * sizeof(short) + 7) / 8 * 8;
-    const size_t ccol_bytes = ((size_t)N.cap * sizeof(int) + 7) / 8 * 8;
-    if(lmap_bytes + ccol_bytes + (size_t)7 * (N.cap + 6) * sizeof(double) > 200 * 1024 ||
-       (size_t)(N.cap + 8) * (6 * sizeof(double) + 2 * sizeof(int)) > 100 * 1024)
+    // (the scalar Gram kernel's shared memory for the widest item the model allows: its eliminated rows and J'x)
+    if(lmap_bytes + (size_t)(7 * (N.cap + 6) + 2) * sizeof(double) > 200 * 1024)
     {
         set_error("lens model with %d intrinsics per camera is too large for the assembly kernels", dp.Nintr_state);
         return false;
@@ -934,7 +665,7 @@ bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& o
     compact_scan_kernel<<<1, 1024, 0, s>>>(N);
     (*nlaunch)++;
     // (the fused evaluation placed the board observations' blocks at their fixed slots)
-    if(N.det_available && !normal_det_item_offsets(dp, N, w0, s, nlaunch)) return false;
+    if(!normal_det_item_offsets(dp, N, w0, s, nlaunch)) return false;
     if(copy_sizes) MB200_CUDA_CHECK(cudaMemcpyAsync(N.h_stat, N.stat, 4 * sizeof(int), cudaMemcpyDeviceToHost, s));
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;
@@ -953,66 +684,39 @@ bool normal_clear_marks(NormalBuffers& N, cudaStream_t s)
     return fill_words(f, s);
 }
 
-// After the stream was synchronised: take over what normal_prepare() found
-bool normal_adopt_sizes(NormalBuffers& N)
+// After the stream was synchronised: take over what normal_prepare() found. If the items' blocks outgrew the pool (wide
+// splined observations on the stored-Jacobian path), it grows here and the items are placed again before the assembly
+bool normal_adopt_sizes(NormalBuffers& N, cudaStream_t s)
 {
     N.n_c = N.h_stat[0];
     N.max_ntot = N.h_stat[1];
-    const int ncols_pad = ((N.max_ntot + 1 + 7) / 8) * 8;
-    // The atomics-free path needs every item within the tensor-pipe Gram kernel's width and within its block of the pool
-    // (h_stat[3]: the items' blocks would not fit the pool -- then this assembly takes the other path)
-    N.det = N.det_available && ncols_pad <= kDmmaMaxCols && N.max_ntot + 2 <= N.capA && N.h_stat[3] == 0;
-    // padding rows: one carries the right-hand side through the factorization; the atomics-free path keeps the plain
-    // gradient in a second one
-    N.ldS = chol_padded(N.n_c + (N.det ? 2 : 1));
-    if(N.ldS > N.ldS_max) N.ldS = N.ldS_max;
-    return true;
-}
-
-// One-time cross-check of the two assembly paths against each other on the caller's own problem (first assembly of a
-// workspace): the atomics-free path must reproduce the atomic one to rounding. If it does not, it is switched off for
-// this workspace, loudly. (Costs one extra assembly; MRCAL_B200_NO_SELFCHECK=1 skips it.)
-bool normal_selfcheck(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
-                      double lambda, cudaStream_t s, int* nlaunch)
-{
-    if(N.selfchecked || !N.det_available || comm_active() || getenv("MRCAL_B200_NO_SELFCHECK") != nullptr) { N.selfchecked = true; return true; }
-    N.selfchecked = true;
-    if(!N.det || N.n_c <= 0) return true;
-    const int n = N.n_c;
-    std::vector<double> Sd((size_t)(n + 1) * n), Sa((size_t)(n + 1) * n);
-    if(!normal_finish(dp, N, op, d_rowptr, lambda, s, nlaunch, false)) return false;
-    MB200_CUDA_CHECK(cudaMemcpy2DAsync(Sd.data(), (size_t)n * sizeof(double), N.S, (size_t)N.ldS * sizeof(double),
-                                       (size_t)n * sizeof(double), n + 1, cudaMemcpyDeviceToHost, s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-    const bool det_saved = N.det;
-    const int ld_saved = N.ldS;
-    N.det = false;
-    const bool ok = normal_finish(dp, N, op, d_rowptr, lambda, s, nlaunch, false);
-    if(ok)
+    // wi_ccol holds compact indices up to n_c + 1 in 16 bits
+    if(N.n_c > 65533) { set_error("the reduced system has %d coupled unknowns: at most 65533 are supported", N.n_c); return false; }
+    if(N.h_stat[2] != 0)
     {
-        MB200_CUDA_CHECK(cudaMemcpy2DAsync(Sa.data(), (size_t)n * sizeof(double), N.S, (size_t)N.ldS * sizeof(double),
-                                           (size_t)n * sizeof(double), n + 1, cudaMemcpyDeviceToHost, s));
+        long long need = 0;
+        MB200_CUDA_CHECK(cudaMemcpyAsync(&need, N.pool_need, sizeof(long long), cudaMemcpyDeviceToHost, s));
         MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-    }
-    N.det = det_saved;
-    N.ldS = ld_saved;
-    if(!ok) return false;
-    double scale = 0., worst = 0.;
-    for(int i = 0; i <= n; i++)
-        for(int j = 0; j < (i < n ? i + 1 : n); j++)
+        // (schur_tiles_kernel addresses the pool with 32-bit element offsets)
+        if(need >= (1ll << 32)) { set_error("the observations' normal-equation blocks need %lld doubles: at most 2^32 are supported", need); return false; }
+        double* pool = nullptr;
+        MB200_CUDA_CHECK(cudaMalloc(&pool, (size_t)need * sizeof(double)));
+        // the fused evaluation's fixed slots at the front of the pool stay where they are
+        if(N.fused && (cudaMemcpyAsync(pool, N.wi_A, (size_t)N.A_pool * sizeof(double), cudaMemcpyDeviceToDevice, s) != cudaSuccess ||
+                       cudaStreamSynchronize(s) != cudaSuccess))
         {
-            const double a = Sa[(size_t)i * n + j], d = Sd[(size_t)i * n + j];
-            if(fabs(a) > scale) scale = fabs(a);
-            if(!(fabs(a - d) <= worst)) worst = fabs(a - d);
+            cudaFree(pool);
+            set_error("growing the pool of the observations' blocks: %s", cudaGetErrorString(cudaGetLastError()));
+            return false;
         }
-    if(!(worst <= 1e-9 * scale))
-    {
-        fprintf(stderr, "mrcal_b200: WARNING: the atomics-free assembly disagrees with the atomic one (|diff| %g of %g): "
-                        "using the atomic path for this problem\n", worst, scale);
-        N.det_available = false;
-        N.det = false;
-        N.ldS = chol_padded(N.n_c + 1) > N.ldS_max ? N.ldS_max : chol_padded(N.n_c + 1);
+        MB200_CUDA_CHECK(cudaFree(N.wi_A));
+        N.wi_A = pool;
+        N.A_pool = need;
+        N.replace_items = true;
     }
+    // padding rows: one carries the right-hand side through the factorization, the second the plain gradient
+    N.ldS = chol_padded(N.n_c + 2);
+    if(N.ldS > N.ldS_max) N.ldS = N.ldS_max;
     return true;
 }
 
@@ -1021,7 +725,7 @@ bool normal_assemble(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& 
 {
     if(!normal_prepare(dp, N, op, s, nlaunch, false)) return false;
     MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-    return normal_adopt_sizes(N) && normal_finish(dp, N, op, d_rowptr, lambda, s, nlaunch, false);
+    return normal_adopt_sizes(N, s) && normal_finish(dp, N, op, d_rowptr, lambda, s, nlaunch, false);
 }
 
 // Pass 2: Gram matrices, Schur elimination, regularization, right-hand side: S, g', J'x
@@ -1029,105 +733,38 @@ bool normal_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op
                    double lambda, cudaStream_t s, int* nlaunch, bool boards_done, double* also_clear, int also_clear_n)
 {
     const size_t lmap_bytes = ((size_t)dp.Nintr_state * sizeof(short) + 7) / 8 * 8;
-    const size_t ccol_bytes = ((size_t)N.cap * sizeof(int) + 7) / 8 * 8;
     const int Nwi = dp.Nobs_board + dp.Nobs_point;
+    // (boards_done: the fused evaluation left the board observations' blocks; only the point observations remain)
+    const int w0 = boards_done ? dp.Nobs_board : 0;
     const int max_ntot = N.max_ntot;
-    const int ncols_pad = ((max_ntot + 1 + 7) / 8) * 8;
-    if(Nwi == 0) N.det = false;
-    if(!N.det) N.ldS = chol_padded(N.n_c + 1) > N.ldS_max ? N.ldS_max : chol_padded(N.n_c + 1);
+    if(N.replace_items)
+    {
+        if(!normal_det_item_offsets(dp, N, w0, s, nlaunch)) return false;
+        N.replace_items = false;
+    }
     // every accumulator and counter of the assembly (and the caller's scalars) zeroed in one launch
     WordFill clear;
     clear.add(N.g_full, (size_t)dp.Nstate * sizeof(double));
     clear.add(N.info, sizeof(int));
     if(also_clear) clear.add(also_clear, (size_t)also_clear_n * sizeof(double));
-    if(N.det) normal_det_to_clear(N, &clear);
+    normal_det_to_clear(N, &clear);
     if(!fill_words(clear, s)) return false;
 
-    if(N.det)
+    if(!normal_det_item_prepare(dp, N, s, nlaunch)) return false;
+    if(((max_ntot + 1 + 7) / 8) * 8 <= kDmmaMaxCols)
     {
-        if(!normal_det_item_prepare(dp, N, s, nlaunch)) return false;
-        // (boards_done: the fused evaluation left the board observations' blocks; only the point observations remain)
-        if(!launch_gram_dmma<true>(dp, N, op, Nwi, max_ntot, lmap_bytes, ccol_bytes, s, nlaunch, boards_done ? dp.Nobs_board : 0)) return false;
-        if(!normal_det_finish(dp, N, op, d_rowptr, lambda, s, nlaunch)) return false;
-        if(dp.Ntri > 0)
-        {
-            assemble_reg_kernel<<<(dp.Ntri + 127) / 128, 128, 0, s>>>(dp, N, op.x, op.Jval, op.Jcol, d_rowptr, dp.m_tri0, dp.m_reg0, N.n_c);
-            (*nlaunch)++;
-        }
-        if(!normal_det_rhs(N, s, nlaunch)) return false;
-        MB200_CUDA_CHECK(cudaGetLastError());
-        return true;
+        if(!launch_gram_dmma(dp, N, op, Nwi, max_ntot, lmap_bytes, s, nlaunch, w0)) return false;
     }
-
-    const int ldc_schur = ((max_ntot > 0 ? max_ntot : 1) + 7) & ~7;   // widest item present (nsh + nelim >= nsh)
-    const size_t smem_schur = (size_t)ldc_schur * (6 * sizeof(double) + 2 * sizeof(int));
-
-    // ---- pass 2: Gram matrices -> S, g', B, D
-    const int gram_cap = max_ntot < kGramMax ? (max_ntot > 8 ? max_ntot : 8) : kGramMax;
-    size_t gram_doubles = (size_t)gram_cap * (gram_cap + 1) / 2 + gram_cap;
-    if(max_ntot > kGramMax && (size_t)7 * max_ntot > gram_doubles) gram_doubles = (size_t)7 * max_ntot;
-    const size_t smem_items = lmap_bytes + ccol_bytes + (gram_doubles + 2) * sizeof(double);
-
-    MB200_CUDA_CHECK(cudaMemsetAsync(N.S, 0, (size_t)N.ldS * N.ldS * sizeof(double), s));
-    MB200_CUDA_CHECK(cudaMemsetAsync(N.gs, 0, (size_t)N.ldS_max * sizeof(double), s));
-    if(Nwi > 0)
+    else if(Nwi > w0)
     {
-        if(ncols_pad <= kDmmaMaxCols)
-        {
-            if(!launch_gram_dmma<false>(dp, N, op, Nwi, max_ntot, lmap_bytes, ccol_bytes, s, nlaunch)) return false;
-        }
-        else
-        {
-            assemble_items_kernel<<<Nwi, 256, smem_items, s>>>(dp, N, gram_cap, op.x, op.Jval, op.Jcol);
-            (*nlaunch)++;
-        }
-    }
-    const int Nreg = dp.Nmeas - dp.m_reg0;
-    if(Nreg > 0)
-    {
-        assemble_reg_kernel<<<(Nreg + 127) / 128, 128, 0, s>>>(dp, N, op.x, op.Jval, op.Jcol, d_rowptr, dp.m_reg0, dp.Nmeas, -1);
+        const int gram_cap = max_ntot < kGramMax ? max_ntot : kGramMax;
+        size_t gram_doubles = (size_t)gram_cap * (gram_cap + 1) / 2 + gram_cap;
+        if(max_ntot > kGramMax && (size_t)7 * max_ntot > gram_doubles) gram_doubles = (size_t)7 * max_ntot;
+        assemble_items_kernel<<<Nwi - w0, 256, lmap_bytes + (gram_doubles + 2) * sizeof(double), s>>>(dp, N, gram_cap, op.x, op.Jval, op.Jcol, w0);
         (*nlaunch)++;
     }
-    if(dp.Ntri > 0)
-    {
-        assemble_reg_kernel<<<(dp.Ntri + 127) / 128, 128, 0, s>>>(dp, N, op.x, op.Jval, op.Jcol, d_rowptr, dp.m_tri0, dp.m_reg0, -1);
-        (*nlaunch)++;
-    }
-    if(N.Ngroups > 0)
-    {
-        schur_groups_kernel<<<dim3(N.Ngroups, N.schur_split), 256, smem_schur, s>>>(N, lambda, ldc_schur);
-        (*nlaunch)++;
-    }
-    if(comm_active())
-    {
-        // THE collective of the algorithm: the reduced normal equations, summed over the frame shards.
-        // g' and the shared part of J'x ride along (gather -> reduce -> scatter)
-        gather_shared_kernel<<<(N.n_r + 255) / 256, 256, 0, s>>>(N, N.gsh);
-        (*nlaunch)++;
-        if(!comm_allreduce_sum(N.S, (size_t)N.ldS * N.ldS, s)) return false;
-        if(!comm_allreduce_sum(N.gs, (size_t)2 * N.ldS_max, s)) return false;   // gs and gsh are contiguous
-        scatter_shared_kernel<<<(N.n_r + 255) / 256, 256, 0, s>>>(N, N.gsh);
-        (*nlaunch)++;
-    }
-    // padding rows of the factorization; diagonal loading of the coupled block
-    if(N.ldS > N.n_c)
-    {
-        set_diagonal_kernel<<<(N.ldS - N.n_c + 255) / 256, 256, 0, s>>>(N.S, N.ldS, N.n_c, N.ldS, 1., false);
-        (*nlaunch)++;
-    }
-    if(lambda > 0. && N.n_c > 0)
-    {
-        set_diagonal_kernel<<<(N.n_c + 255) / 256, 256, 0, s>>>(N.S, N.ldS, 0, N.n_c, lambda, true);
-        (*nlaunch)++;
-    }
-    // The forward substitution for free: -g' goes in as row n_c (a padding row) of S. After the
-    // factorization that row of L is y' with L y = -g', because the panel TRSM treats it like any
-    // other row. Only the backward substitution is left to do explicitly.
-    if(N.n_c > 0)
-    {
-        augment_rhs_kernel<<<(N.n_c + 255) / 256, 256, 0, s>>>(N);
-        (*nlaunch)++;
-    }
+    if(!normal_det_finish(dp, N, op, d_rowptr, lambda, s, nlaunch)) return false;
+    if(!normal_det_rhs(N, s, nlaunch)) return false;
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;
 }
@@ -1146,50 +783,26 @@ bool normal_extract_y(const NormalBuffers& N, double* rhs, cudaStream_t s, int* 
     return true;
 }
 
-// rhs[c] = -g'[c] for the compact system; padding 0
-__global__ void compact_rhs_kernel(NormalBuffers N, double* __restrict__ rhs)
-{
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if(c < N.ldS) rhs[c] = c < N.n_c ? -N.gs[c] : 0.;
-}
-// compact solution -> reduced-length vector (for the back-substitution) and the full-length step
-__global__ void scatter_compact_kernel(NormalBuffers N, const double* __restrict__ sol, double* __restrict__ ds_r,
-                                       double* __restrict__ step_full)
+// compact solution -> the shared part of the full-length step
+__global__ void scatter_compact_kernel(NormalBuffers N, const double* __restrict__ sol, double* __restrict__ step_full)
 {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if(c >= N.n_c) return;
     const int r = N.cinv[c];
-    ds_r[r] = sol[c];
     step_full[N.state_index(r)] = sol[c];
-}
-
-bool normal_rhs(const NormalBuffers& N, double* rhs, cudaStream_t s, int* nlaunch)
-{
-    compact_rhs_kernel<<<(N.ldS + 255) / 256, 256, 0, s>>>(N, rhs);
-    (*nlaunch)++;
-    MB200_CUDA_CHECK(cudaGetLastError());
-    return true;
 }
 
 // the full-length Gauss-Newton step from the compact solution `sol`
 bool normal_expand_step(const DevProblem& dp, const NormalBuffers& N, const EvalBuffers& op, double lambda,
-                        const double* sol, double* ds_r, double* step_full, cudaStream_t s, int* nlaunch)
+                        const double* sol, double* step_full, cudaStream_t s, int* nlaunch)
 {
-    if(N.n_c > 0) { scatter_compact_kernel<<<(N.n_c + 255) / 256, 256, 0, s>>>(N, sol, ds_r, step_full); (*nlaunch)++; }
+    if(N.n_c > 0) { scatter_compact_kernel<<<(N.n_c + 255) / 256, 256, 0, s>>>(N, sol, step_full); (*nlaunch)++; }
     if(N.n_r > N.n_c)
     {
         inactive_step_kernel<<<(N.n_r + 255) / 256, 256, 0, s>>>(dp, N, lambda, op.x, op.Jval, step_full);
         (*nlaunch)++;
     }
-    if(N.Ngroups > 0)
-    {
-        if(N.det) { if(!normal_det_backsub(N, sol, step_full, s, nlaunch)) return false; }
-        else
-        {
-            backsub_groups_kernel<<<(N.Ngroups * 32 + 255) / 256, 256, 0, s>>>(N, ds_r, step_full, N.e0);
-            (*nlaunch)++;
-        }
-    }
+    if(!normal_det_backsub(N, sol, step_full, s, nlaunch)) return false;
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;
 }

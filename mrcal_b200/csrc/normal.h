@@ -36,11 +36,11 @@ struct NormalBuffers
     int     n_c;      // ... of which touched by some observation: the coupled ("active") ones
     int     max_ntot; // widest work item (local columns) at the operating point of the last normal_prepare()
     double* gs;       // [ldS_max] reduced gradient g' (compact numbering)
-    double* gsh;      // [ldS_max] staging for the shared part of J'x (reduced numbering); follows gs in memory
     int*    active;   // [n_r] flag
     int*    cidx;     // [n_r] reduced -> compact index, -1 if inactive
     int*    cinv;     // [ldS_max] compact -> reduced index
-    int*    stat;     // device: [0] n_c, [1] widest item (local columns)
+    int*    stat;     // device: [0] n_c, [1] widest item (local columns), [2] the items' blocks outgrow the pool,
+                      // [3] the fused evaluation gave up on an observation
     int*    h_stat;   // pinned host mirror of stat
     bool    splined;
     double* g_full;   // [Nstate] J'x, state numbering
@@ -55,16 +55,10 @@ struct NormalBuffers
     double* wi_gf;    // [Nwi][6]
 
     int     Ngroups, Nframe_groups;
-    int     schur_split;   // CTAs per group in the Schur kernel (<= most items in any group)
     int*    grp_ptr;    // [Ngroups+1]
     int*    grp_items;  // work item ids
-    double* grp_Dinv;   // [Ngroups][36]
-    double* grp_gf;     // [Ngroups][6]
 
-    // ---- the atomics-free assembly (normal_det.cu): every entry of S is summed by ONE thread in a fixed order
-    bool    det_available;   // the buffers below exist (MRCAL_B200_ATOMIC_ASSEMBLY=1 turns the path off)
-    bool    det;          // in use for this assembly
-    bool    selfchecked;  // the one-time cross-check against the atomic path has run
+    // ---- the assembly without atomics (normal_det.cu): every entry of S is summed by ONE thread in a fixed order
     bool    fused;        // the board rows are evaluated by fused_eval.cu: blocks straight from the projection, no J
     double* norm_part;    // [Nobs_board] per-observation |x|^2
     double* qf_part;      // [Nobs_board] per-observation g'(J'J)g
@@ -75,10 +69,12 @@ struct NormalBuffers
                           //  full    [lda][lda] row-major, lower triangle; rows nsh, nsh+1: -J'x over the item's shared columns
                           //  compact the board observations of the fused evaluation (fused_eval.cu); see kCompactSlot
     long long* wi_Aoff;   // [Nwi] offset of each item's block in the pool (doubles)
-    long long  A_pool;    // pool size (doubles)
+    long long  A_pool;    // pool size (doubles); grows when the items' blocks do not fit (normal_adopt_sizes)
+    long long* pool_need; // device: what the last placement of the items needed (doubles)
+    bool    replace_items;   // the pool grew since the items were placed: place them again before the next assembly
     int*    wi_lda;       // [Nwi] full layout: nsh + 2 rounded up to even. Compact layout: ~nk (< 0)
     unsigned short* wi_ccol;    // [Nwi][capA] compact index of each local column (increasing); then n_c, n_c+1
-    unsigned char*  wi_segoff;  // [Nwi][nblk_max+1] first local column of each 64-column block of S
+    unsigned short* wi_segoff;  // [Nwi][nblk_max+1] first local column of each 64-column block of S
     int     nblk_max;     // ldS_max / 64
     double* Ypan;         // [Ngroups][nblk_max][6][kYld] inv(L_D) B of each group, dense per 64-column block (present blocks
                           // only). Rows padded to kYld: a panel goes to shared memory as ONE bulk copy and lands with a
@@ -104,28 +100,23 @@ bool normal_clear_marks(NormalBuffers& N, cudaStream_t s);
 void normal_marks_to_clear(const NormalBuffers& N, WordFill* f);   // the same buffers, into the caller's fill
 bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, cudaStream_t s, int* nlaunch, bool boards_done,
                     double* rider = nullptr, bool* rider_summed = nullptr, bool copy_sizes = true);
-bool normal_adopt_sizes(NormalBuffers& N);
+bool normal_adopt_sizes(NormalBuffers& N, cudaStream_t s);   // (s: the stream the pool is used on, when it grows)
 // also_clear: n doubles of the caller's that are zeroed with the assembly's own accumulators (one launch)
 bool normal_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
                    double lambda, cudaStream_t s, int* nlaunch, bool boards_done, double* also_clear = nullptr, int also_clear_n = 0);
 // fused_eval.cu
 bool launch_fused_boards(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& out, double* norm_part, cudaStream_t s, int* nlaunch);
 bool launch_quadform_boards(const DevProblem& dp, const NormalBuffers& N, const double* g_full, double* part, double* out, cudaStream_t s, int* nlaunch);
-bool normal_selfcheck(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
-                      double lambda, cudaStream_t s, int* nlaunch);
 // S, g', g_full at the operating point `op` (needs its x and Jacobian). lambda: diagonal loading.
 // Updates N.n_c / N.ldS (one small device->host read)
 bool normal_assemble(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
                      double lambda, cudaStream_t s, int* nlaunch);
 // rhs <- y, L y = -g': read from the augmented row of the factor (valid after chol_factor)
 bool normal_extract_y(const NormalBuffers& N, double* rhs, cudaStream_t s, int* nlaunch);
-// rhs <- -g' (compact numbering, ldS entries)
-bool normal_rhs(const NormalBuffers& N, double* rhs, cudaStream_t s, int* nlaunch);
 // full-length Gauss-Newton step from the compact solution: active shared unknowns, inactive shared
 // unknowns (from their regularization blocks), eliminated unknowns (back-substitution).
-// ds_r: scratch, n_r doubles
 bool normal_expand_step(const DevProblem& dp, const NormalBuffers& N, const EvalBuffers& op, double lambda,
-                        const double* sol, double* ds_r, double* step_full, cudaStream_t s, int* nlaunch);
+                        const double* sol, double* step_full, cudaStream_t s, int* nlaunch);
 
 // normal_det.cu: the stages after the per-item Gram matrices, without atomics
 bool normal_det_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,

@@ -23,6 +23,8 @@
 //                                 operands staged with cp.async, double buffered.
 //   reg_blocks_kernel             the regularization rows: one thread per knot (or per unknown), the
 //                                 single owner of the entries it adds to
+//   tri_rows_kernel               the triangulated-point rows: one CTA per entry of the extrinsics block
+//                                 and of the gradient rows, walking the pairs of the entry's camera
 //
 // The right-hand side travels as row n_c of S (forward substitution for free, as before), the plain
 // gradient J'x of the shared unknowns as row n_c+1.
@@ -30,7 +32,6 @@
 // Replaces what the reference gets from libdogleg's Jt*x and CHOLMOD's A*A' + factorization of the full
 // sparse JtJ (call site mrcal.c:6435).
 #include "normal_items.cuh"
-#include "chol.h"
 #include "chol.h"
 
 namespace mb200 {
@@ -77,7 +78,13 @@ item_offsets_kernel(NormalBuffers N, int first, int Nwi)
         N.wi_Aoff[w] = base;
         base += (long long)N.wi_lda[w] * N.wi_lda[w];
     }
-    if(tid == 1023 && (long long)first * kCompactSlot + s_scan[1023] > N.A_pool) N.stat[3] = 1;   // pool too small: the host takes the other path
+    if(tid == 1023)
+    {
+        // pool too small: normal_adopt_sizes() grows it and the items are placed again
+        const long long need = (long long)first * kCompactSlot + s_scan[1023];
+        *N.pool_need = need;
+        if(need > N.A_pool) N.stat[2] = 1;
+    }
 }
 
 // After the compaction: compact column of each local column, the two gradient rows, the first local column of
@@ -90,7 +97,7 @@ item_prepare_kernel(NormalBuffers N, int Nwi, int n_c, int nblk)
     const int nsh = N.wi_nsh[w];
     const int* cols = N.wi_cols + (size_t)w * N.cap;
     unsigned short* cc = N.wi_ccol + (size_t)w * N.capA;
-    unsigned char* seg = N.wi_segoff + (size_t)w * (N.nblk_max + 1);
+    unsigned short* seg = N.wi_segoff + (size_t)w * (N.nblk_max + 1);
     const int n = nsh + 2;
     for(int l = lane; l < n; l += 32)
     {
@@ -99,9 +106,9 @@ item_prepare_kernel(NormalBuffers N, int Nwi, int n_c, int nblk)
         const int blk = c >> 6;
         const int prev = l == 0 ? -1 : ((l - 1 < nsh ? N.cidx[cols[l - 1]] : n_c + (l - 1 - nsh)) >> 6);
         // blocks (prev, blk] start at local column l
-        for(int b = prev + 1; b <= blk; b++) seg[b] = (unsigned char)l;
+        for(int b = prev + 1; b <= blk; b++) seg[b] = (unsigned short)l;
         if(blk != prev) atomicOr(&N.wi_present[(size_t)blk * N.wwords + (w >> 5)], 1u << (w & 31));
-        if(l == n - 1) for(int b = blk + 1; b <= nblk; b++) seg[b] = (unsigned char)n;
+        if(l == n - 1) for(int b = blk + 1; b <= nblk; b++) seg[b] = (unsigned short)n;
     }
 }
 
@@ -141,7 +148,7 @@ __global__ void __launch_bounds__(256)
 groups_panels_kernel(NormalBuffers N, double lambda, int n_c, int nblk)
 {
     __shared__ double s_D[36], s_gf[6], s_Linv[36], s_h[6];
-    __shared__ unsigned s_blk[8];   // up to 256 blocks
+    extern __shared__ unsigned s_blk[];   // [bwords] the blocks the group reaches
     const int grp = blockIdx.x, tid = threadIdx.x;
     const int i0 = N.grp_ptr[grp], i1 = N.grp_ptr[grp + 1];
     const int nelim = grp < N.Nframe_groups ? 6 : 3;
@@ -159,7 +166,7 @@ groups_panels_kernel(NormalBuffers N, double lambda, int n_c, int nblk)
         for(int i = i0; i < i1; i++) v += N.wi_gf[(size_t)N.grp_items[i] * 6 + (tid - 64)];
         s_gf[tid - 64] = v;
     }
-    if(tid >= 96 && tid < 104) s_blk[tid - 96] = 0u;
+    for(int i = tid; i < N.bwords; i += 256) s_blk[i] = 0u;
     __syncthreads();
     if(tid == 0)
     {
@@ -199,7 +206,7 @@ groups_panels_kernel(NormalBuffers N, double lambda, int n_c, int nblk)
         for(int e = tid; e < kYpanel; e += 256) Yg[(size_t)b * kYpanel + e] = 0.;
         if(tid == 0) atomicOr(&N.grp_present[(size_t)b * N.gwords + (grp >> 5)], 1u << (grp & 31));
     }
-    if(tid < N.bwords) N.grp_blkmask[(size_t)grp * N.bwords + tid] = s_blk[tid];
+    for(int i = tid; i < N.bwords; i += 256) N.grp_blkmask[(size_t)grp * N.bwords + i] = s_blk[i];
     __syncthreads();
     // Y = inv(L) B, item after item: items of one group may share columns (the board warp; the intrinsics of a
     // camera seen twice), and the order of the additions is part of the result
@@ -242,7 +249,7 @@ static_assert(sizeof(TileCommon) % 16 == 0, "the tile and the staging buffers be
 struct alignas(16) TileSmemA
 {
     double tile[TB * TLD];
-    int    meta[kChunkItems][4];           // a0 | na<<8,  b0 | nb<<8,  lda (< 0: compact layout, ~nk),  nsh
+    int    meta[kChunkItems][4];           // a0 | na<<16,  b0 | nb<<16,  lda (< 0: compact layout, ~nk),  nsh
     long long base[kChunkItems];
     double f2[kChunkItems][2];             // compact layout: fx*fx, fy*fy
     unsigned char rl[kChunkItems][TB + 4]; // tile row of each local row
@@ -315,7 +322,8 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 constexpr int kPackedExtras = 8;      // doubles behind the packed tiles (sharded solves)
 constexpr int kMaxParts = 64;         // a tile's contributors may be split over this many CTAs
 constexpr int kCtasPerTile = 4;       // the grid: this many CTAs per tile on average (kernel_ctas()); parts are cut to fit
-__host__ __device__ inline int kernel_ctas(int ntiles) { return kCtasPerTile * ntiles; }
+// (at least kMaxParts: the one tile of a small system, which every observation reaches, may be split as far as a tile can be)
+__host__ __device__ inline int kernel_ctas(int ntiles) { return kCtasPerTile * ntiles > kMaxParts ? kCtasPerTile * ntiles : kMaxParts; }
 
 __device__ __forceinline__ void tile_row_col(int itile, int& r, int& c)
 {
@@ -493,14 +501,14 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
             if(tid < nch)
             {
                 const int w = sc.wl[ch + tid];
-                const unsigned char* seg = N.wi_segoff + (size_t)w * (N.nblk_max + 1);
+                const unsigned short* seg = N.wi_segoff + (size_t)w * (N.nblk_max + 1);
                 const int nsh = N.wi_nsh[w];
                 const int a0 = seg[r], a1 = seg[r + 1];
                 int b0 = seg[c], b1 = seg[c + 1];
                 if(b1 > nsh) b1 = nsh;              // the gradient rows are rows only
                 if(b0 > b1) b0 = b1;
-                sa.meta[tid][0] = a0 | ((a1 - a0) << 8);
-                sa.meta[tid][1] = b0 | ((b1 - b0) << 8);
+                sa.meta[tid][0] = a0 | ((a1 - a0) << 16);
+                sa.meta[tid][1] = b0 | ((b1 - b0) << 16);
                 const int lda = N.wi_lda[w];
                 const long long base = N.wi_Aoff[w];
                 sa.meta[tid][2] = lda;
@@ -516,13 +524,13 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
                 const unsigned short* cc = N.wi_ccol + (size_t)w * N.capA;
                 if(k < TB)
                 {
-                    const int a0 = sa.meta[i][0] & 255, na = sa.meta[i][0] >> 8;
+                    const int a0 = sa.meta[i][0] & 0xffff, na = sa.meta[i][0] >> 16;
                     if(k < na) sa.rl[i][k] = (unsigned char)(cc[a0 + k] - TB * r);
                 }
                 else
                 {
                     const int kk = k - TB;
-                    const int b0 = sa.meta[i][1] & 255, nb = sa.meta[i][1] >> 8;
+                    const int b0 = sa.meta[i][1] & 0xffff, nb = sa.meta[i][1] >> 16;
                     if(kk < nb) sa.cl[i][kk] = (unsigned char)(cc[b0 + kk] - TB * c);
                 }
             }
@@ -557,7 +565,7 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
                         {
                             ti++;
                             if(ti >= nch) { exhausted = true; break; }
-                            const int na = sa.meta[ti][0] >> 8, nb = sa.meta[ti][1] >> 8;
+                            const int na = sa.meta[ti][0] >> 16, nb = sa.meta[ti][1] >> 16;
                             if(na == 0 || nb == 0) continue;
                             cur0 = __ballot_sync(0xffffffffu, lane < na && (sa.rl[ti][lane] & 7) == warp);
                             cur1 = __ballot_sync(0xffffffffu, lane + 32 < na && (sa.rl[ti][lane + 32] & 7) == warp);
@@ -567,8 +575,8 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
                         src[u] = 0u; dst0[u] = dst1[u] = 0; scl[u] = 1.;
                         if(item >= 0)
                         {
-                            const int a = (sa.meta[item][0] & 255) + lrow;
-                            const int b0 = sa.meta[item][1] & 255, nb = sa.meta[item][1] >> 8;
+                            const int a = (sa.meta[item][0] & 0xffff) + lrow;
+                            const int b0 = sa.meta[item][1] & 0xffff, nb = sa.meta[item][1] >> 16;
                             const int lda = sa.meta[item][2];
                             const int nk = lda < 0 ? ~lda : 0;
                             const int trow = (int)sa.rl[item][lrow] * TLD;
@@ -883,6 +891,60 @@ __global__ void reg_blocks_kernel(DevProblem P, NormalBuffers N, int n_c, const 
     }
 }
 
+// The triangulated-point rows (mrcal.c:5180-5653) touch the extrinsics of the two cameras of a pair only. One CTA per
+// entry of the extrinsics x extrinsics block of S (t < nx (nx+1) / 2, lower triangle) and of the two gradient rows (the
+// nx CTAs behind): its threads take the pairs that see the entry's first camera (tri_cam_rows, in order) in turn, each
+// adds what a row brings to the entry -- the product of the row's values on the two columns (a pair of observations of
+// the same camera names each column twice: the values are summed) -- and the threads' sums are added in a fixed tree.
+// Every column is in the coupled system: mark_tri_active_kernel made it so
+__global__ void __launch_bounds__(256)
+tri_rows_kernel(DevProblem P, NormalBuffers N, int n_c, const double* __restrict__ x, const double* __restrict__ Jval,
+                const int* __restrict__ Jcol, const int* __restrict__ rowptr)
+{
+    __shared__ double s_part[8];
+    const int nx = 6 * P.Ncam_e;
+    const int t = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
+    const int ntri = nx * (nx + 1) / 2;
+    int ka, kb = -1;   // kb < 0: the gradient entry of column ka
+    if(t < ntri)
+    {
+        ka = (int)((sqrtf(8.f * t + 1.f) - 1.f) * 0.5f);
+        while(ka * (ka + 1) / 2 > t) ka--;
+        while((ka + 1) * (ka + 2) / 2 <= t) ka++;
+        kb = t - ka * (ka + 1) / 2;
+    }
+    else ka = t - ntri;
+    const int ca = P.i_extr0 + ka, cb = P.i_extr0 + (kb >= 0 ? kb : 0);
+    const int ia = N.cidx[N.reduced_index(ca)], ib = N.cidx[N.reduced_index(cb)];
+    if(ia < 0 || (kb >= 0 && ib < 0)) return;   // (CTA-uniform)
+    const int e = ka / 6;
+    double sum = 0.;
+    for(int k = P.tri_cam_ptr[e] + tid; k < P.tri_cam_ptr[e + 1]; k += 256)
+    {
+        const int m = P.m_tri0 + P.tri_cam_rows[k];
+        double va = 0., vb = 0.;
+        for(int j = rowptr[m]; j < rowptr[m + 1]; j++)
+        {
+            const int c = Jcol[j];
+            if(c == ca) va += Jval[j];
+            if(c == cb) vb += Jval[j];
+        }
+        sum += kb >= 0 ? va * vb : va * x[m];
+    }
+#pragma unroll
+    for(int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    if(lane == 0) s_part[tid >> 5] = sum;
+    __syncthreads();
+    if(tid != 0) return;
+    sum = ((s_part[0] + s_part[1]) + (s_part[2] + s_part[3])) + ((s_part[4] + s_part[5]) + (s_part[6] + s_part[7]));
+    if(kb >= 0) N.S[(size_t)ia * N.ldS + ib] += sum;
+    else
+    {
+        N.S[(size_t)n_c * N.ldS + ia] -= sum;
+        N.S[(size_t)(n_c + 1) * N.ldS + ia] -= sum;
+    }
+}
+
 // gs = g' and the shared part of J'x out of rows n_c, n_c+1 of S; row n_c+1 becomes plain padding
 __global__ void finish_rhs_kernel(NormalBuffers N, int n_c)
 {
@@ -990,7 +1052,7 @@ bool normal_det_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers
     const int ntiles = nblk * (nblk + 1) / 2;
     if(N.Ngroups > 0)
     {
-        groups_panels_kernel<<<N.Ngroups, 256, 0, s>>>(N, lambda, N.n_c, nblk);
+        groups_panels_kernel<<<N.Ngroups, 256, (size_t)N.bwords * sizeof(unsigned), s>>>(N, lambda, N.n_c, nblk);
         (*nlaunch)++;
     }
     const bool sharded = comm_active();
@@ -1025,7 +1087,12 @@ bool normal_det_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers
         reg_blocks_kernel<<<(Nreg_blocks + 127) / 128, 128, 0, s>>>(dp, N, N.n_c, op.x, op.Jval, op.Jcol, sharded);
         (*nlaunch)++;
     }
-    (void)d_rowptr;
+    if(dp.Ntri > 0 && dp.opt_extr)
+    {
+        const int nx = 6 * dp.Ncam_e;
+        tri_rows_kernel<<<nx * (nx + 1) / 2 + nx, 256, 0, s>>>(dp, N, N.n_c, op.x, op.Jval, op.Jcol, d_rowptr);
+        (*nlaunch)++;
+    }
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;
 }

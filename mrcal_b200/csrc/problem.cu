@@ -204,6 +204,15 @@ mrcal_b200_problem_create_triangulated(const double* intrinsics, const mrcal_pos
     }
 
     tri_set_obs0.push_back(Nobservations_point_triangulated);
+    // the pairs of each camera, in order: what the assembly's owner of an extrinsics entry walks (normal_det.cu)
+    std::vector<int> tri_cam_ptr(Ncameras_extrinsics + 1, 0), tri_cam_rows;
+    for(int e = 0; e < Ncameras_extrinsics; e++)
+    {
+        tri_cam_ptr[e] = (int)tri_cam_rows.size();
+        for(size_t ip = 0; ip < tri_pairs.size() / 2; ip++)
+            if(tri_cam_e[tri_pairs[2 * ip]] == e || tri_cam_e[tri_pairs[2 * ip + 1]] == e) tri_cam_rows.push_back((int)ip);
+    }
+    tri_cam_ptr[Ncameras_extrinsics] = (int)tri_cam_rows.size();
     std::unique_ptr<mrcal_b200_problem> P(new mrcal_b200_problem());
     Dims d;
     d.Nmeas_tri = (int)(tri_pairs.size() / 2);
@@ -281,11 +290,12 @@ mrcal_b200_problem_create_triangulated(const double* intrinsics, const mrcal_pos
     const size_t nfeat = (size_t)d.Nobs_board * d.W * d.H;
     int *d_obs_board, *d_obs_point, *d_board_j0, *d_point_j0, *d_imagersizes;
     int *d_tri_pairs = nullptr, *d_tri_cam_e = nullptr, *d_tri_outlier = nullptr, *d_tri_j0 = nullptr;
-    int *d_tri_set_obs0 = nullptr, *d_tri_set_m0 = nullptr;
+    int *d_tri_set_obs0 = nullptr, *d_tri_set_m0 = nullptr, *d_tri_cam_ptr = nullptr, *d_tri_cam_rows = nullptr;
     double* d_tri_px = nullptr;
     bool ok = A.alloc(&d_tri_pairs, tri_pairs.size()) && A.alloc(&d_tri_cam_e, tri_cam_e.size()) && A.alloc(&d_tri_outlier, tri_outlier.size()) &&
               A.alloc(&d_tri_j0, tri_j0.size()) && A.alloc(&d_tri_px, tri_px.size()) &&
               A.alloc(&d_tri_set_obs0, tri_set_obs0.size()) && A.alloc(&d_tri_set_m0, tri_set_m0.size()) &&
+              A.alloc(&d_tri_cam_ptr, tri_cam_ptr.size()) && A.alloc(&d_tri_cam_rows, tri_cam_rows.size()) &&
               A.alloc(&P->d_tri_outlier_seed, tri_outlier.size()) &&
               A.alloc(&P->d_seed_intr, (size_t)d.Ncam_i * L.Nintr) && A.alloc(&P->d_seed_rtcam, 6 * (size_t)d.Ncam_e) &&
               A.alloc(&P->d_seed_rtframe, 6 * (size_t)d.Nframes) && A.alloc(&P->d_seed_points, 3 * (size_t)d.Npoints) &&
@@ -317,6 +327,7 @@ mrcal_b200_problem_create_triangulated(const double* intrinsics, const mrcal_pos
          upload(d_tri_outlier, tri_outlier.data(), tri_outlier.size(), s) && upload(d_tri_j0, tri_j0.data(), tri_j0.size(), s) &&
          upload(d_tri_px, tri_px.data(), tri_px.size(), s) &&
          upload(d_tri_set_obs0, tri_set_obs0.data(), tri_set_obs0.size(), s) && upload(d_tri_set_m0, tri_set_m0.data(), tri_set_m0.size(), s) &&
+         upload(d_tri_cam_ptr, tri_cam_ptr.data(), tri_cam_ptr.size(), s) && upload(d_tri_cam_rows, tri_cam_rows.data(), tri_cam_rows.size(), s) &&
          upload(P->d_tri_outlier_seed, tri_outlier.data(), tri_outlier.size(), s);
     if(!ok) return nullptr;
     if(cudaStreamSynchronize(s) != cudaSuccess) { set_error("upload failed"); return nullptr; }   // the staging vectors go out of scope
@@ -347,6 +358,7 @@ mrcal_b200_problem_create_triangulated(const double* intrinsics, const mrcal_pos
     dp.m_tri0 = L.m_tri0; dp.Ntri = d.Nmeas_tri;
     dp.tri_px = d_tri_px; dp.tri_cam_e = d_tri_cam_e; dp.tri_outlier = d_tri_outlier; dp.tri_pairs = d_tri_pairs; dp.tri_j0 = d_tri_j0;
     dp.Ntri_sets = (int)tri_set_m0.size(); dp.tri_set_obs0 = d_tri_set_obs0; dp.tri_set_m0 = d_tri_set_m0;
+    dp.tri_cam_ptr = d_tri_cam_ptr; dp.tri_cam_rows = d_tri_cam_rows;
     P->Nobs_tri = Nobservations_point_triangulated;
     // the extrinsics regularization needs the frames off/extrinsics on case to see u_rtcam: always unpacked
 

@@ -66,6 +66,8 @@ struct DevProblem
     int*          tri_outlier;     // [Nobs_tri] flags; outlier rejection adds to them (outliers.cu)
     const int*    tri_pairs;       // [Ntri][2] observation indices i0 < i1
     const int*    tri_j0;          // [Ntri+1] first Jacobian entry of each pair's row
+    const int*    tri_cam_ptr;     // [Ncam_e+1] the pairs that see camera e: tri_cam_rows[tri_cam_ptr[e] .. tri_cam_ptr[e+1])
+    const int*    tri_cam_rows;    // pair indices, increasing within each camera
     int           Ntri_sets;       // triangulated points (sets of consecutive observations)
     const int*    tri_set_obs0;    // [Ntri_sets+1] first observation of each set
     const int*    tri_set_m0;      // [Ntri_sets] first measurement (pair) of each set, relative to m_tri0

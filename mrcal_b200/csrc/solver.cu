@@ -156,8 +156,6 @@ static bool build_workspace(mrcal_b200_problem* P)
     N.ldS = N.ldS_max;
     N.n_c = N.n_r;
     N.splined = L.splined;
-    N.schur_split = 1;
-    // gs | gsh contiguous (one reduction)
     N.cap = L.Nintr_state + 8;
     N.Nframe_groups = (elim && L.i_frame0 >= 0) ? L.d.Nframes : 0;
     const int Npoint_groups = (elim && L.i_point0 >= 0) ? L.Npoints_variable : 0;
@@ -178,59 +176,52 @@ static bool build_workspace(mrcal_b200_problem* P)
             }
         for(int g = 0; g < N.Ngroups; g++)
         {
-            if((int)buckets[g].size() > N.schur_split) N.schur_split = (int)buckets[g].size();
             ptr[g] = (int)items.size();
             items.insert(items.end(), buckets[g].begin(), buckets[g].end());
         }
         ptr[N.Ngroups] = (int)items.size();
-        if(N.schur_split > 8) N.schur_split = 8;
     }
 
-    bool ok = A.alloc(&N.S, (size_t)N.ldS_max * N.ldS_max) && A.alloc(&N.gs, 2 * (size_t)N.ldS_max, true) && A.alloc(&N.g_full, L.Nstate, true) &&
+    bool ok = A.alloc(&N.S, (size_t)N.ldS_max * N.ldS_max) && A.alloc(&N.gs, (size_t)N.ldS_max, true) && A.alloc(&N.g_full, L.Nstate, true) &&
               A.alloc(&N.info, 4, true) && A.alloc(&N.active, N.n_r, true) && A.alloc(&N.cidx, N.n_r, true) &&
-              A.alloc(&N.cinv, N.ldS_max, true) && A.alloc(&N.stat, 4, true) && A.alloc(&ws->ds_r, N.n_r, true) &&
+              A.alloc(&N.cinv, N.ldS_max, true) && A.alloc(&N.stat, 4, true) &&
               A.alloc(&N.wi_nsh, Nwi, true) && A.alloc(&N.wi_cols, (size_t)Nwi * N.cap) &&
               A.alloc(&N.wi_B, (size_t)Nwi * 6 * N.cap) && A.alloc(&N.wi_D, (size_t)Nwi * 36) && A.alloc(&N.wi_gf, (size_t)Nwi * 6) &&
               A.alloc(&N.grp_ptr, (size_t)N.Ngroups + 1) && A.alloc(&N.grp_items, items.size()) &&
-              A.alloc(&N.grp_Dinv, (size_t)N.Ngroups * 36) && A.alloc(&N.grp_gf, (size_t)N.Ngroups * 6) &&
               A.alloc(&ws->invL, (size_t)N.ldS_max * kCholBlock) && A.alloc(&ws->rhs, N.ldS_max, true) &&
               A.alloc(&ws->step_gn, L.Nstate, true) && A.alloc(&ws->step, L.Nstate, true) && A.alloc(&ws->scal, 64, true) &&
               A.alloc(&ws->ictl, 8, true);
     if(!ok) return false;
-    // the atomics-free assembly (normal_det.cu)
+    // the assembly without atomics (normal_det.cu). Its pool of per-item blocks is sized for the items the problem has in
+    // the common case; wider ones (splined boards that touch more knots) make it grow (normal_adopt_sizes)
     N.nblk_max = N.ldS_max / kCholBlock;
-    N.det_available = getenv("MRCAL_B200_ATOMIC_ASSEMBLY") == nullptr && Nwi > 0 && N.nblk_max <= 256;
-    if(N.det_available)
+    N.capA = N.cap + 2;
     {
-        N.capA = N.cap + 2 < 162 ? N.cap + 2 : 162;
         auto even = [](int v) { return (v + 1) & ~1; };
         const int lda_board = even(std::min(N.capA, (L.splined ? 160 : L.Nintr_state + 8) + 2));
         const int lda_point = even(std::min(N.capA, (L.splined ? 2 * 16 + 4 + 6 : L.Nintr_state + 6) + 2));
         // (a splined model's boards may also take the fused evaluation's fixed compact slots)
         const long long board_block = L.splined ? std::max((long long)lda_board * lda_board, kCompactSlot) : (long long)lda_board * lda_board;
         N.A_pool = (long long)L.d.Nobs_board * board_block + (long long)L.d.Nobs_point * lda_point * lda_point;
-        // (schur_tiles_kernel addresses the pool with 32-bit element offsets: 4 G doubles = 34 GB, more than a problem this
-        // library's other buffers would leave room for)
-        if(N.A_pool >= (1ll << 32)) N.det_available = false;
     }
-    if(N.det_available)
-    {
-        N.gwords = (N.Ngroups + 31) / 32; if(N.gwords < 1) N.gwords = 1;
-        N.wwords = (Nwi + 31) / 32;
-        N.bwords = (N.nblk_max + 31) / 32;
-        ok = A.alloc(&N.wi_A, (size_t)N.A_pool) && A.alloc(&N.wi_Aoff, Nwi, true) && A.alloc(&N.wi_lda, Nwi, true) &&
-             A.alloc(&N.wi_ccol, (size_t)Nwi * N.capA, true) && A.alloc(&N.wi_segoff, (size_t)Nwi * (N.nblk_max + 1), true) &&
-             A.alloc(&N.Ypan, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * N.nblk_max * kYpanel) &&
-             A.alloc(&N.grp_present, (size_t)N.nblk_max * N.gwords, true) && A.alloc(&N.wi_present, (size_t)N.nblk_max * N.wwords, true) &&
-             A.alloc(&N.grp_blkmask, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * N.bwords, true) &&
-             A.alloc(&N.grp_Linv, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * 36, true) && A.alloc(&N.grp_h, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * 6, true);
-        if(!ok) return false;
-        if(!A.alloc(&N.part_scratch, normal_det_part_scratch_doubles(N.nblk_max)) || !A.alloc(&N.part_arrive, normal_det_part_arrive_ints(N.nblk_max), true)) return false;
-        // (always there: the communicator may be created after this workspace)
-        if(!A.alloc(&N.S_packed, normal_det_packed_doubles(N.nblk_max))) return false;
-    }
+    // (schur_tiles_kernel addresses the pool with 32-bit element offsets: 4 G doubles = 34 GB)
+    if(N.A_pool >= (1ll << 32)) { set_error("the observations' normal-equation blocks need %lld doubles: at most 2^32 are supported", N.A_pool); return false; }
+    N.gwords = (N.Ngroups + 31) / 32; if(N.gwords < 1) N.gwords = 1;
+    N.wwords = (Nwi + 31) / 32;
+    N.bwords = (N.nblk_max + 31) / 32;
+    MB200_CUDA_CHECK(cudaMalloc(&N.wi_A, (size_t)(N.A_pool > 0 ? N.A_pool : 1) * sizeof(double)));   // (owned by the workspace: it may grow)
+    ok = A.alloc(&N.pool_need, 1, true) && A.alloc(&N.wi_Aoff, Nwi, true) && A.alloc(&N.wi_lda, Nwi, true) &&
+         A.alloc(&N.wi_ccol, (size_t)Nwi * N.capA, true) && A.alloc(&N.wi_segoff, (size_t)Nwi * (N.nblk_max + 1), true) &&
+         A.alloc(&N.Ypan, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * N.nblk_max * kYpanel) &&
+         A.alloc(&N.grp_present, (size_t)N.nblk_max * N.gwords, true) && A.alloc(&N.wi_present, (size_t)N.nblk_max * N.wwords, true) &&
+         A.alloc(&N.grp_blkmask, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * N.bwords, true) &&
+         A.alloc(&N.grp_Linv, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * 36, true) && A.alloc(&N.grp_h, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * 6, true) &&
+         A.alloc(&N.part_scratch, normal_det_part_scratch_doubles(N.nblk_max)) && A.alloc(&N.part_arrive, normal_det_part_arrive_ints(N.nblk_max), true) &&
+         // (always there: the communicator may be created after this workspace)
+         A.alloc(&N.S_packed, normal_det_packed_doubles(N.nblk_max));
+    if(!ok) return false;
     // the fused evaluation (fused_eval.cu): splined models with the core locked, boards of at most 128 corners
-    N.fused = N.det_available && L.splined && !L.sel.do_optimize_intrinsics_core && L.sel.do_optimize_intrinsics_distortions &&
+    N.fused = L.splined && !L.sel.do_optimize_intrinsics_core && L.sel.do_optimize_intrinsics_distortions &&
               L.sel.do_optimize_frames && L.i_frame0 >= 0 && L.d.Nobs_board > 0 && L.d.W * L.d.H <= 128 &&
               getenv("MRCAL_B200_NO_FUSED") == nullptr;
     // (the fused kernel places each board observation's block itself: fixed slots of kCompactSlot doubles, normal.h)
@@ -241,7 +232,6 @@ static bool build_workspace(mrcal_b200_problem* P)
         MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&N.s_side[k], cudaStreamNonBlocking));
         MB200_CUDA_CHECK(cudaEventCreateWithFlags(&N.ev_join[k], cudaEventDisableTiming));
     }
-    N.gsh = N.gs + N.ldS_max;
     MB200_CUDA_CHECK(cudaMallocHost(&ws->h_scal, 64 * sizeof(double)));
     MB200_CUDA_CHECK(cudaMallocHost(&ws->h_info, 16 * sizeof(int)));
     N.h_stat = ws->h_info + 4;
@@ -413,74 +403,6 @@ __global__ void combine_step_dev_kernel(int n, const double* __restrict__ scal, 
     p_new[i] = p[i] + sv;
 }
 
-// One-time cross-checks on the caller's own problem (first assembly of a workspace): the atomics-free assembly against
-// the atomic one (normal_selfcheck), and the fused evaluation's blocks against the ones made from a stored Jacobian.
-// A path that disagrees is switched off for this workspace, loudly. MRCAL_B200_NO_SELFCHECK=1 skips all of it
-static bool solver_selfcheck(mrcal_b200_problem* P, int which, double lambda)
-{
-    SolverWorkspace* ws = P->ws.get();
-    NormalBuffers& N = ws->N;
-    cudaStream_t s = P->stream;
-    int* nl = &P->launches;
-    if(N.selfchecked || getenv("MRCAL_B200_NO_SELFCHECK") != nullptr || comm_active()) { N.selfchecked = true; return true; }
-    if(!N.fused) return normal_selfcheck(P->dp, N, P->op[which], P->d_rowptr, lambda, s, nl);
-    // fused: its S first, then the same point through the stored Jacobian
-    const int n = N.n_c;
-    std::vector<double> Sf, Sj;
-    auto grab = [&](std::vector<double>& out) -> bool
-    {
-        out.assign((size_t)(n + 1) * (n > 0 ? n : 1), 0.);
-        if(n <= 0) return true;
-        MB200_CUDA_CHECK(cudaMemcpy2DAsync(out.data(), (size_t)n * sizeof(double), N.S, (size_t)N.ldS * sizeof(double),
-                                           (size_t)n * sizeof(double), n + 1, cudaMemcpyDeviceToHost, s));
-        MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-        return true;
-    };
-    if(!N.det) { N.selfchecked = true; return true; }
-    if(!normal_finish(P->dp, N, P->op[which], P->d_rowptr, lambda, s, nl, true) || !grab(Sf)) return false;
-    N.fused = false;
-    // (the per-assembly placement of the blocks is what the stored-Jacobian path uses)
-    if(!problem_evaluate(P, which, true, false) || !normal_prepare(P->dp, N, P->op[which], s, nl, false)) return false;
-    MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-    if(!normal_adopt_sizes(N)) return false;
-    bool agree = N.n_c == n && N.det;
-    if(agree)
-    {
-        if(!normal_selfcheck(P->dp, N, P->op[which], P->d_rowptr, lambda, s, nl)) return false;   // det vs atomic, on the stored Jacobian
-        if(!normal_finish(P->dp, N, P->op[which], P->d_rowptr, lambda, s, nl, false) || !grab(Sj)) return false;
-        // the lower triangle and the right-hand side row: what the assembly writes (the rest of S holds whatever the
-        // buffer held before)
-        double scale = 0., worst = 0.;
-        for(int i = 0; i <= n; i++)
-            for(int j = 0; j < (i < n ? i + 1 : n); j++)
-            {
-                const size_t k = (size_t)i * n + j;
-                if(fabs(Sj[k]) > scale) scale = fabs(Sj[k]);
-                if(!(fabs(Sj[k] - Sf[k]) <= worst)) worst = fabs(Sj[k] - Sf[k]);
-            }
-        agree = worst <= 1e-9 * scale;
-        if(!agree)
-            fprintf(stderr, "mrcal_b200: WARNING: the fused evaluation disagrees with the stored-Jacobian path (|diff| %g of %g): "
-                            "not using it for this problem\n", worst, scale);
-    }
-    N.selfchecked = true;
-    if(agree)
-    {
-        // back to the fused path: redo the evaluation's blocks (the fused kernel puts them back in their fixed slots)
-        N.fused = true;
-        const EvalBuffers& o = P->op[which];
-        MB200_CUDA_CHECK(cudaMemsetAsync(o.norm2, 0, sizeof(double), s));
-        if(!normal_clear_marks(N, s) || !launch_unpack_state(P->dp, o.p, s, nl) ||
-           !launch_fused_boards(P->dp, N, o, N.norm_part, s, nl) ||
-           !launch_evaluate(P->dp, o, true, nullptr, s, nl, false) ||
-           !normal_prepare(P->dp, N, o, s, nl, true)) return false;
-        if(comm_active() && !comm_allreduce_sum(o.norm2, 1, s)) return false;
-        MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-        if(!normal_adopt_sizes(N)) return false;
-    }
-    return true;
-}
-
 static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameters_t& par, double* lambda,
                         mrcal_b200_solve_info_t* info, PhaseTimer* T, double* norm2_final)
 {
@@ -520,7 +442,6 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
     };
     auto assemble = [&](int which) -> bool
     {
-        if(!N.selfchecked && !solver_selfcheck(P, which, *lambda)) return false;
         const int a = T->mark();
         // (the scalars of the Cauchy step that follows are cleared with the assembly's accumulators)
         if(!normal_finish(P->dp, N, P->op[which], P->d_rowptr, *lambda, s, nl, N.fused, ws->scal, 32)) return false;
@@ -546,17 +467,8 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
         }
         MB200_CUDA_CHECK(cudaStreamSynchronize(s));
         info->Nsyncs++;
-        return normal_adopt_sizes(N);   // n_c, widest item: from the prepare() that ran last
+        return normal_adopt_sizes(N, s);   // n_c, widest item: from the prepare() that ran last
     };
-    // an observation whose patch of control points outgrows the fused kernel's tables (a board filling the imager):
-    // this workspace goes back to the stored-Jacobian path, starting with the evaluation that found out
-    auto evaluate_checked = [&](int which) -> bool
-    {
-        if(!evaluate(which)) return false;
-        return true;
-    };
-    (void)evaluate_checked;
-
     // rows whose sums this rank contributes to cross-rank reductions: the regularization rows are
     // replicated on every rank but counted once
     const int Nrows_mine = P->dp.reg_owner ? Nmeas : P->dp.m_reg0;
@@ -669,7 +581,7 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
                 const int b = T->mark();
                 if(!normal_extract_y(N, ws->rhs, s, nl)) return false;
                 if(N.n_c > 0 && !chol_solve_backward(N.S, N.ldS, ws->invL, ws->rhs, N.info + 1, s, nl, &ws->chol, run_if)) return false;
-                if(!normal_expand_step(P->dp, N, P->op[P->cur], *lambda, ws->rhs, ws->ds_r, ws->step_gn, s, nl)) return false;
+                if(!normal_expand_step(P->dp, N, P->op[P->cur], *lambda, ws->rhs, ws->step_gn, s, nl)) return false;
                 dots_kernel<<<3, 1024, 0, s>>>(ws->step_gn, N.g_full, e0, e1, Nstate, ws->scal + 11);
                 (*nl)++;
                 if(overlap) MB200_CUDA_CHECK(cudaStreamWaitEvent(s, N.ev_join[0], 0));
@@ -700,24 +612,14 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
             if(factored_now && need_gn)
             {
                 info->Nfactorizations++;
-                int bad = (ws->h_info[0] != 0 || ws->h_info[1] != 0) ? 1 : 0;
+                const bool bad = ws->h_info[0] != 0 || ws->h_info[1] != 0;
                 if(ws->h_info[1] == -9)
                 {
                     set_error("the persistent factorization kernel gave up waiting for a tile (code -9): not a property of the matrix");
                     return false;
                 }
-                // sharded: a frame block that is singular on ONE rank has been reported to every rank with the reduced system
-                // itself (normal_det.cu:unpack_extras_kernel) and the factorization is replicated. The other assembly path
-                // asks around
-                if(comm_active() && !N.det)
-                {
-                    ws->h_scal[SC_N] = (double)bad;
-                    MB200_CUDA_CHECK(cudaMemcpyAsync(ws->scal + SC_N, ws->h_scal + SC_N, sizeof(double), cudaMemcpyHostToDevice, s));
-                    if(!comm_allreduce_sum(ws->scal + SC_N, 1, s)) return false;
-                    MB200_CUDA_CHECK(cudaMemcpyAsync(ws->h_scal + SC_N, ws->scal + SC_N, sizeof(double), cudaMemcpyDeviceToHost, s));
-                    MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-                    bad = ws->h_scal[SC_N] != 0.;
-                }
+                // (sharded: a frame block that is singular on ONE rank has been reported to every rank with the reduced system
+                // itself, normal_det.cu:unpack_extras_kernel, and the factorization is replicated)
                 if(bad)
                 {
                     // singular JtJ: add lambda I "from now on", as libdogleg does (1e-10, then x10), and do this operating point again
@@ -914,8 +816,8 @@ extern "C" bool mrcal_b200_problem_reduced_system_fused(mrcal_b200_problem_t* P,
     if(!fill_words(clear, s) || !launch_unpack_state(P->dp, o.p, s, nl) || !launch_fused_boards(P->dp, N, o, N.norm_part, s, nl) ||
        !launch_evaluate(P->dp, o, true, nullptr, s, nl, false) || !normal_prepare(P->dp, N, o, s, nl, true)) return false;
     MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-    if(!normal_adopt_sizes(N)) return false;
-    if(N.h_stat[3] != 0 || !N.det)
+    if(!normal_adopt_sizes(N, s)) return false;
+    if(N.h_stat[3] != 0)
     {
         set_error("reduced_system_fused: the fused evaluation's blocks do not fit this problem");
         return false;

@@ -14,7 +14,6 @@ struct SolverWorkspace
     NormalBuffers N{};
     double* invL = nullptr;
     double* rhs = nullptr;        // [ldS] compact solution
-    double* ds_r = nullptr;       // [n_r] the same in reduced numbering
     double* step_gn = nullptr;    // [Nstate]
     double* step = nullptr;       // [Nstate]
     double* scal = nullptr;       // [64] device scalars
@@ -29,6 +28,7 @@ struct SolverWorkspace
     ~SolverWorkspace()
     {
         chol_forget_graphs(N.S);
+        if(N.wi_A) cudaFree(N.wi_A);
         for(int k = 0; k < 2; k++)
         {
             if(N.s_side[k]) cudaStreamDestroy(N.s_side[k]);
@@ -69,8 +69,7 @@ namespace mb200 {
 bool schur_factorization_solve(mrcal_b200_factorization* F, double* out, const double* bt, int Nrhs, int sys);
 double schur_factorization_rcond(mrcal_b200_factorization* F);
 void schur_factorization_release(mrcal_b200_factorization* F);
-// other_path (may be NULL): set when the failure is that this problem's reduced system is assembled without the panels
-bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F, bool* other_path = nullptr);
+bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F);
 // csr_ops.cu
 bool csr_stable_transpose(const int* p, const int* col, int Nrows, int nnz, int Ncols, DeviceArena& arena,
                           int** tp, int** tsrc, int** trow, cudaStream_t s);

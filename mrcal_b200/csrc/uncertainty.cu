@@ -19,11 +19,6 @@
 // are never eliminated, so X is needed only on the shared unknowns and the backward pass stops after L_S' (the panels
 // are not needed in that direction). Without regularization rows Var = sigma^2 Z'Z (:784-843).
 //
-// Where the solver assembles the reduced system with atomics (no panels: parametric models whose observations touch all
-// of their camera's shared columns), the factor is instead the dense Cholesky factor of J'J, built without atomics from
-// a stable transpose of J (dense_jtj_kernel) and factored by the solver's DMMA Cholesky; every unknown is then "shared"
-// and the same tiled L_S kernels run on it.
-//
 // The many-right-hand-side pieces are DMMA (mma.sync.m8n8k4.f64) kernels that take a tile of 32 right-hand sides:
 //   panels  Bs[tile][64-col block] -= Zf[tile][groups of the block] Y[groups][block]   one CTA per (block, tile)
 //   L_S     left-looking blocked solve, 64x64 blocks: every off-diagonal block of L_S is one GEMM against the tile,
@@ -469,34 +464,6 @@ __global__ void __launch_bounds__(256) sigma_kernel(const double* __restrict__ x
     }
 }
 
-// Dense J'J (lower triangle, ld x ld row-major, 1 on the padding diagonal) from the stable transpose of J: thread i owns
-// row i and walks the rows of J that touch column i in order, adding J[r][i] J[r][j] for the row's columns j <= i. One
-// owner per entry, a fixed order: no atomics
-__global__ void dense_jtj_kernel(const int* __restrict__ rowptr, const int* __restrict__ Jcol, const double* __restrict__ Jval,
-                                 const int* __restrict__ tp, const int* __restrict__ tsrc, const int* __restrict__ trow,
-                                 int Nstate, double* __restrict__ H, int ld)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if(i >= ld) return;
-    double* h = H + (size_t)i * ld;
-    if(i >= Nstate) { h[i] = 1.; return; }
-    for(int k = tp[i]; k < tp[i + 1]; k++)
-    {
-        const double v = Jval[tsrc[k]];
-        const int r = trow[k];
-        for(int e = rowptr[r]; e < rowptr[r + 1]; e++)
-        {
-            const int j = Jcol[e];
-            if(j <= i) h[j] += v * Jval[e];
-        }
-    }
-}
-__global__ void iota_kernel(int* __restrict__ a, int n)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if(i < n) a[i] = i;
-}
-
 bool launch_rows(const DevProblem& dp, const NormalBuffers& N, const RowArgs& A, const double* pcam, int Npts,
                  double* Bf, double* Bs, double* Bi, double* G, cudaStream_t s)
 {
@@ -568,54 +535,18 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
     MB200_CUDA_CHECK(cudaFuncSetAttribute(panels_forward_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
     MB200_CUDA_CHECK(cudaFuncSetAttribute(ls_solve_tiled_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
     MB200_CUDA_CHECK(cudaFuncSetAttribute(ls_solve_tiled_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
-    // 1-2. the Jacobian at the current state, and the factor: the structured one where the solver's atomics-free
-    // assembly builds its panels; otherwise the dense Cholesky factor of J'J, with every unknown "shared"
+    // 1-2. the Jacobian at the current state, and the structured factor
     DeviceArena mem;
-    // the dense route's factorization: its scratch, and the CUDA graphs that reference H (before mem frees it)
-    struct DenseChol { CholScratch sc; const void* A = nullptr; ~DenseChol() { if(A) chol_forget_graphs(A); chol_scratch_destroy(&sc); } } chol;
     mrcal_b200_factorization F;   // its buffers only: it does not own P here
     F.P = P;
-    bool other_path = false, dense = false;
-    NormalBuffers N;
-    const double *Lfac = nullptr, *invLfac = nullptr;
     const EvalBuffers& op = P->op[P->cur];
     const int Nstate = L.Nstate;
-    if(schur_factor_build(P, &F, &other_path))
-    {
-        N = P->ws->N;
-        Lfac = N.S;
-        invLfac = P->ws->invL;
-    }
-    else if(other_path)
-    {
-        dense = true;
-        const int npad = chol_padded(Nstate);
-        double *H = nullptr, *invLd = nullptr;
-        int *info = nullptr, *cid = nullptr, *tp = nullptr, *tsrc = nullptr, *trow = nullptr;
-        if(!mem.alloc(&H, (size_t)npad * npad) || !mem.alloc(&invLd, (size_t)npad * TB) || !mem.alloc(&info, 1) ||
-           !mem.alloc(&cid, (size_t)Nstate)) return false;
-        chol.A = H;
-        MB200_CUDA_CHECK(cudaMemsetAsync(H, 0, (size_t)npad * npad * sizeof(double), s));
-        if(!csr_stable_transpose(P->d_rowptr, op.Jcol, L.Nmeas, P->nnz, Nstate, mem, &tp, &tsrc, &trow, s)) return false;
-        dense_jtj_kernel<<<(npad + 127) / 128, 128, 0, s>>>(P->d_rowptr, op.Jcol, op.Jval, tp, tsrc, trow, Nstate, H, npad);
-        iota_kernel<<<(Nstate + 255) / 256, 256, 0, s>>>(cid, Nstate);
-        int h_info = 0;
-        if(!chol_scratch_create(&chol.sc, npad) || !chol_factor(H, npad, Nstate, invLd, info, s, nullptr, &chol.sc)) return false;
-        MB200_CUDA_CHECK(cudaMemcpyAsync(&h_info, info, sizeof(int), cudaMemcpyDeviceToHost, s));
-        MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-        if(h_info != 0) { set_error("JtJ is not positive definite"); return false; }
-        N = NormalBuffers{};
-        N.e0 = N.e1 = 0;
-        N.n_r = N.n_c = Nstate;
-        N.ldS = npad;
-        N.cidx = cid;
-        N.Ngroups = N.Nframe_groups = 0;
-        Lfac = H;
-        invLfac = invLd;
-    }
-    else return false;
-    const int Nelim = dense ? 0 : F.Nelim;
-    const int nBi = dense ? 0 : N.n_r;
+    if(!schur_factor_build(P, &F)) return false;
+    const NormalBuffers N = P->ws->N;
+    const double* Lfac = N.S;
+    const double* invLfac = P->ws->invL;
+    const int Nelim = F.Nelim;
+    const int nBi = N.n_r;
     // 3. K, if the method needs it (the Jacobian was evaluated above)
     double *K = nullptr, *sigma = nullptr;
     int* bad = nullptr;
@@ -676,12 +607,12 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
             panels_forward_tiled_kernel<<<dim3(nblkS, (nr + RT - 1) / RT), 256, kTileSmem, s>>>(N, Bf, Nelim, Bs, nr);
         }
         if(N.n_c > 0) ls_solve_tiled_kernel<false><<<(nr + RT - 1) / RT, 256, kTileSmem, s>>>(Lfac, N.ldS, invLfac, Bs, N.ldS, nr, nblkS, N.n_c);
-        if(!dense) schur_inactive_tri(&F, Bi, nr, true, s);
+        schur_inactive_tri(&F, Bi, nr, true, s);
         ztz_kernel<<<(unsigned)((np * 32 + 255) / 256), 256, 0, s>>>(N, Bf, Nelim, Bs, Bi, nBi, np, V);
         // X on the shared unknowns = inv(L_S') Z_s, inv(L_I') Z_i
         if(reg)
         {
-            if(!dense) schur_inactive_tri(&F, Bi, nr, false, s);
+            schur_inactive_tri(&F, Bi, nr, false, s);
             if(N.n_c > 0) ls_solve_tiled_kernel<true><<<(nr + RT - 1) / RT, 256, kTileSmem, s>>>(Lfac, N.ldS, invLfac, Bs, N.ldS, nr, nblkS, N.n_c);
         }
         finish_kernel<<<(unsigned)((np * 32 + 255) / 256), 256, 0, s>>>(N, Bs, Bi, P->d_rowptr, op.Jcol, op.Jval, L.m_reg0,

@@ -193,3 +193,25 @@ def solve_cases():
     inp["do_apply_outlier_rejection"] = True
     cases.append(("tri_divergent_rejection", inp))
     return cases
+
+
+def reduced_reference(J, x, e0, e1, lam=0.0):
+    """S, g', J'x and the scale of S's accuracy, from J and x with numpy: the unknowns [e0, e1) eliminated"""
+    Jd = J.toarray()
+    H = Jd.T @ Jd + lam * np.eye(Jd.shape[1])
+    g = Jd.T @ x
+    n = H.shape[0]
+    sh = np.r_[0:e0, e1:n]
+    el = np.r_[e0:e1]
+    if len(el) == 0:
+        return H, g, g, np.abs(H).max()
+    # eliminated unknowns nothing constrains (a point seen only by outlier observations, at lambda = 0) have zero rows
+    # in J'J: they couple to nothing, so they drop out of the elimination -- the device leaves them out the same way
+    # instead of inverting their zero block
+    free = ~np.any(H[el] != 0, axis=1)
+    el = el[~free]
+    A, B, D = H[np.ix_(sh, sh)], H[np.ix_(sh, el)], H[np.ix_(el, el)]
+    assert np.linalg.cond(D) < 1e12, "the constrained part of the eliminated block is singular"
+    Dinv = np.linalg.inv(D)
+    # S is a difference of two nearly equal terms: the achievable accuracy is relative to |A|
+    return A - B @ Dinv @ B.T, g[sh] - B @ Dinv @ g[el], g, (np.abs(A).max() if A.size else 1.)

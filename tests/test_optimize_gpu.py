@@ -179,7 +179,9 @@ def test_problem_handle_resolve_and_info():
     s2 = P.optimize()
     b2 = P.download(into_inputs=False)["b_packed"]
     assert abs(s1["Niterations"] - s2["Niterations"]) <= 1 and s1["Niterations"] > 0
-    assert np.abs(b1 - b2).max() < 1e-6        # atomics reorder sums: not bitwise, but close
+    # the reduced system is the same bit for bit (test_assembly_gpu.py); the scalar sums of the step logic (jv_kernel)
+    # and of the cost still add with atomics: not bitwise, but close
+    assert np.abs(b1 - b2).max() < 1e-6
     assert s1["Nkernel_launches"] > 0 and 0 < s1["Nreduced"] <= P.Nstate - 6 * 40
     assert s1["norm2_x_final"] < s1["norm2_x_initial"]
     # a solve started at the optimum stops immediately

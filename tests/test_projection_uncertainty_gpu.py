@@ -111,7 +111,7 @@ def _gate(Var, Var_ref, cond):
 
 def _cases():
     out = []
-    # parametric: camera 1's observations touch all of its shared columns, so the dense device factor is used
+    # parametric: camera 1's observations touch all of its shared columns
     for reg in (True, False):
         for method in METHODS:
             for icam in ((0, 1) if reg else (1,)):
