@@ -11,8 +11,9 @@
 //               syrk (K=64)  update of the REST OF THE PANEL only
 //           syrk (K=256)     one DMMA update of the whole trailing matrix
 //
-//   - triangular solves with the factor for nrhs right-hand sides, two short kernels per 64-column block and
-//     direction (the factorization objects' solves)
+//   - triangular solves with the factor for nrhs right-hand sides (the factorization objects' solves, and through the
+//     structured factor projection_uncertainty()'s), chosen by nrhs and the number of 64-column blocks: two short
+//     kernels per block and direction, or a DMMA kernel that takes a tile of kSolveTile right-hand sides per CTA
 //   - min/max of diag(L), for rcond
 //   - fill_words: a few ranges of flags and counters cleared in one launch
 //   - timing and debugging aids
@@ -25,6 +26,7 @@
 #include <vector>
 
 #include "chol.h"
+#include "dmma.cuh"
 #include "potrf_block.cuh"
 #include "problem.h"
 
@@ -126,12 +128,6 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool va
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
-__device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b)
-{
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                 : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-
 // TILE = 128: 8 warps as 4 x 2, warp tile 32 x 64 (4 x 8 DMMA tiles)   -- large trailing matrices
 // TILE =  64: 8 warps as 4 x 2, warp tile 16 x 32 (2 x 4 DMMA tiles)   -- small ones: 4x the CTAs, so the
 //             update spreads over the whole chip instead of a few dozen SMs
@@ -231,6 +227,145 @@ syrk_dmma_kernel(double* __restrict__ A, int ld, int n, int c0, int c1, int k0, 
     }
 }
 
+////////////////////////////////////////////////////////////////////////////////
+// triangular solves, Nrhs right-hand sides stored as rows: B[rhs][n]
+////////////////////////////////////////////////////////////////////////////////
+// y_k = invL_kk b_k  (transpose=false)  or  invL_kk' b_k (transpose=true); one CTA per rhs
+__global__ void __launch_bounds__(64)
+solve_diag_kernel(const double* __restrict__ invL, double* __restrict__ B, int ldb, int k0, bool transpose)
+{
+    __shared__ double b[NB];
+    double* v = B + (size_t)blockIdx.x * ldb + k0;
+    const int i = threadIdx.x;
+    b[i] = v[i];
+    __syncthreads();
+    double acc = 0.;
+    if(!transpose) { for(int m = 0; m <= i; m++) acc += invL[i * NB + m] * b[m]; }
+    else           { for(int m = i; m < NB; m++) acc += invL[m * NB + i] * b[m]; }
+    v[i] = acc;
+}
+
+// forward:  b_i -= L(i, k0:k0+64) y_k for rows i >= k0+64. One warp per row, all rhs
+__global__ void __launch_bounds__(256)
+solve_update_fwd_kernel(const double* __restrict__ L, int ld, int n, double* __restrict__ B, int ldb, int nrhs, int k0)
+{
+    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    const int i = k0 + NB + warp;
+    if(i >= n) return;
+    const double l0 = L[(size_t)i * ld + k0 + lane], l1 = L[(size_t)i * ld + k0 + 32 + lane];
+    for(int r = 0; r < nrhs; r++)
+    {
+        const double* y = B + (size_t)r * ldb + k0;
+        double acc = l0 * y[lane] + l1 * y[32 + lane];
+#pragma unroll
+        for(int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        if(lane == 0) B[(size_t)r * ldb + i] -= acc;
+    }
+}
+
+// backward: b_j -= sum_r L(k0+r, j) z_k[r] for columns j < k0. One thread per column, all rhs
+__global__ void __launch_bounds__(256)
+solve_update_bwd_kernel(const double* __restrict__ L, int ld, double* __restrict__ B, int ldb, int nrhs, int k0)
+{
+    __shared__ double z[NB];
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    for(int r = 0; r < nrhs; r++)
+    {
+        __syncthreads();
+        if(threadIdx.x < NB) z[threadIdx.x] = B[(size_t)r * ldb + k0 + threadIdx.x];
+        __syncthreads();
+        if(j < k0)
+        {
+            double acc = 0.;
+#pragma unroll 8
+            for(int m = 0; m < NB; m++) acc += L[(size_t)(k0 + m) * ld + j] * z[m];
+            B[(size_t)r * ldb + j] -= acc;
+        }
+    }
+}
+
+// L y = b (BWD = false) or L' x = b (BWD = true) for a tile of kSolveTile right-hand sides B[r][0..ldb), in place,
+// left-looking over 64-blocks: block i takes the GEMM of every already-solved block k with L's block (i,k) (or (k,i)'),
+// then the GEMM with the stored inverse of its diagonal block. Unknowns >= nreal are treated as zero
+template <bool BWD>
+__global__ void __launch_bounds__(256)
+ls_solve_tiled_kernel(const double* __restrict__ L, int ld, const double* __restrict__ invL, double* __restrict__ B, int ldb,
+                      int Nrhs, int nblk, int nreal)
+{
+    extern __shared__ __align__(16) double dsm[];
+    double (*sA)[kSolveTileLd] = reinterpret_cast<double (*)[kSolveTileLd]>(dsm);
+    double (*sM)[kSolveTileLd] = reinterpret_cast<double (*)[kSolveTileLd]>(dsm + kSolveTile * kSolveTileLd);
+    const int r0 = blockIdx.x * kSolveTile;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g8 = lane >> 2, t4 = lane & 3;
+    const int mt = warp >> 1, nt0 = (warp & 1) * 4;
+    auto gemm = [&](double (&acc)[4][2], bool trans)
+    {
+#pragma unroll 4
+        for(int ks = 0; ks < NB / 4; ks++)
+        {
+            const double a = sA[mt * 8 + g8][ks * 4 + t4];
+#pragma unroll
+            for(int j = 0; j < 4; j++)
+            {
+                const int n = (nt0 + j) * 8 + g8, k = ks * 4 + t4;
+                dmma(acc[j][0], acc[j][1], a, trans ? sM[k][n] : sM[n][k]);
+            }
+        }
+    };
+    auto load_rhs = [&](int kb)
+    {
+        for(int e = tid; e < kSolveTile * NB; e += 256)
+        {
+            const int r = e >> 6, m = e & 63, c = kb * NB + m;
+            sA[r][m] = (r0 + r < Nrhs && c < nreal) ? B[(size_t)(r0 + r) * ldb + c] : 0.;
+        }
+    };
+    for(int step = 0; step < nblk; step++)
+    {
+        const int i = BWD ? nblk - 1 - step : step;
+        double acc[4][2] = {};
+        for(int s = 0; s < step; s++)
+        {
+            const int k = BWD ? nblk - 1 - s : s;
+            load_rhs(k);
+            // forward: sM[n][m] = L(i*64+n, k*64+m);  backward: sM[m][n] = L(k*64+m, i*64+n)
+            for(int e = tid; e < NB * NB; e += 256)
+            {
+                const int a = e >> 6, b = e & 63;
+                const int row = BWD ? k * NB + a : i * NB + a, col = BWD ? i * NB + b : k * NB + b;
+                sM[a][b] = (row < nreal && col < nreal) ? L[(size_t)row * ld + col] : 0.;
+            }
+            __syncthreads();
+            gemm(acc, BWD);
+            __syncthreads();
+        }
+        load_rhs(i);
+        for(int e = tid; e < NB * NB; e += 256) sM[e >> 6][e & 63] = invL[(size_t)i * NB * NB + e];
+        __syncthreads();
+#pragma unroll
+        for(int j = 0; j < 4; j++)
+        {
+            sA[mt * 8 + g8][(nt0 + j) * 8 + 2 * t4] -= acc[j][0];
+            sA[mt * 8 + g8][(nt0 + j) * 8 + 2 * t4 + 1] -= acc[j][1];
+            acc[j][0] = acc[j][1] = 0.;
+        }
+        __syncthreads();
+        // forward: y[n] = sum_m invL[n][m] b[m];  backward: x[n] = sum_m invL[m][n] b[m]
+        gemm(acc, BWD);
+        const int r = r0 + mt * 8 + g8;
+        if(r < Nrhs)
+#pragma unroll
+            for(int j = 0; j < 4; j++)
+                for(int h = 0; h < 2; h++)
+                {
+                    const int c = i * NB + (nt0 + j) * 8 + 2 * t4 + h;
+                    if(c < nreal) B[(size_t)r * ldb + c] = acc[j][h];
+                }
+        __syncthreads();
+    }
+}
+
 __global__ void fill_words_kernel(WordFill f)
 {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
@@ -271,6 +406,8 @@ static bool configure_kernels()
     MB200_CUDA_CHECK(cudaFuncSetAttribute(trsm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBlockSmem));
     MB200_CUDA_CHECK(cudaFuncSetAttribute(potrf_diag_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
     MB200_CUDA_CHECK(cudaFuncSetAttribute(potrf_diag_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
+    MB200_CUDA_CHECK(cudaFuncSetAttribute(ls_solve_tiled_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveTileSmem));
+    MB200_CUDA_CHECK(cudaFuncSetAttribute(ls_solve_tiled_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveTileSmem));
     configured = true;
     return true;
 }
@@ -293,8 +430,6 @@ static bool syrk_update(double* A, int ld, int n, int c0, int c1, int k0, int k1
     if(nlaunch) (*nlaunch)++;
     return true;
 }
-
-static bool chol_solve_enqueue(const double* L, int npad, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s, int* nlaunch, int parts = 3);
 
 // The multi-kernel factorization is ~3 short kernels per 64-column block, a solve 2 per block and direction, all with
 // launch-time-constant arguments: replaying a captured CUDA graph takes the host out of the loop (the host would
@@ -380,70 +515,6 @@ bool chol_factor_blocked(double* A, int npad, int nreal, double* invL, int* d_in
     });
 }
 
-bool chol_solve(const double* L, int npad, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s, int* nlaunch, int parts)
-{
-    if(nrhs != 1) return chol_solve_enqueue(L, npad, invL, B, ldb, nrhs, s, nlaunch, parts);
-    return run_graphed(GraphKey{L, B, npad, ldb, parts}, s, nlaunch,
-                       [&](int* n) { return chol_solve_enqueue(L, npad, invL, B, ldb, 1, s, n, parts); });
-}
-
-////////////////////////////////////////////////////////////////////////////////
-// triangular solves, Nrhs right-hand sides stored as rows: B[rhs][n]
-////////////////////////////////////////////////////////////////////////////////
-// y_k = invL_kk b_k  (transpose=false)  or  invL_kk' b_k (transpose=true); one CTA per rhs
-__global__ void __launch_bounds__(64)
-solve_diag_kernel(const double* __restrict__ invL, double* __restrict__ B, int ldb, int k0, bool transpose)
-{
-    __shared__ double b[NB];
-    double* v = B + (size_t)blockIdx.x * ldb + k0;
-    const int i = threadIdx.x;
-    b[i] = v[i];
-    __syncthreads();
-    double acc = 0.;
-    if(!transpose) { for(int m = 0; m <= i; m++) acc += invL[i * NB + m] * b[m]; }
-    else           { for(int m = i; m < NB; m++) acc += invL[m * NB + i] * b[m]; }
-    v[i] = acc;
-}
-
-// forward:  b_i -= L(i, k0:k0+64) y_k for rows i >= k0+64. One warp per row, all rhs
-__global__ void __launch_bounds__(256)
-solve_update_fwd_kernel(const double* __restrict__ L, int ld, int n, double* __restrict__ B, int ldb, int nrhs, int k0)
-{
-    const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    const int i = k0 + NB + warp;
-    if(i >= n) return;
-    const double l0 = L[(size_t)i * ld + k0 + lane], l1 = L[(size_t)i * ld + k0 + 32 + lane];
-    for(int r = 0; r < nrhs; r++)
-    {
-        const double* y = B + (size_t)r * ldb + k0;
-        double acc = l0 * y[lane] + l1 * y[32 + lane];
-#pragma unroll
-        for(int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-        if(lane == 0) B[(size_t)r * ldb + i] -= acc;
-    }
-}
-
-// backward: b_j -= sum_r L(k0+r, j) z_k[r] for columns j < k0. One thread per column, all rhs
-__global__ void __launch_bounds__(256)
-solve_update_bwd_kernel(const double* __restrict__ L, int ld, double* __restrict__ B, int ldb, int nrhs, int k0)
-{
-    __shared__ double z[NB];
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
-    for(int r = 0; r < nrhs; r++)
-    {
-        __syncthreads();
-        if(threadIdx.x < NB) z[threadIdx.x] = B[(size_t)r * ldb + k0 + threadIdx.x];
-        __syncthreads();
-        if(j < k0)
-        {
-            double acc = 0.;
-#pragma unroll 8
-            for(int m = 0; m < NB; m++) acc += L[(size_t)(k0 + m) * ld + j] * z[m];
-            B[(size_t)r * ldb + j] -= acc;
-        }
-    }
-}
-
 static bool chol_solve_enqueue(const double* L, int npad, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s, int* nlaunch, int parts)
 {
     const int nblk = npad / NB;
@@ -472,6 +543,30 @@ static bool chol_solve_enqueue(const double* L, int npad, const double* invL, do
     }
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;
+}
+
+// The per-block kernels parallelise over the rows under each 64-block and loop over the right-hand sides: their time
+// grows as nblk x nrhs. The tiled kernel runs one CTA per kSolveTile right-hand sides through all nblk^2/2 block pairs:
+// its time grows as nblk^2 and hardly with nrhs. So the crossover moves with nblk. Measured on H100 (DESIGN section
+// 9), the tiled kernel wins from 2 to 3 nblk right-hand sides on for L' and 4 to 7 nblk for L; it takes over at 8 nblk
+constexpr int kTiledSolveRhsPerBlock = 8;
+
+bool chol_solve(const double* L, int npad, int nreal, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s,
+                int* nlaunch, int parts)
+{
+    if(nrhs >= kTiledSolveRhsPerBlock * (npad / NB))
+    {
+        if(!configure_kernels()) return false;
+        const unsigned tiles = (unsigned)((nrhs + kSolveTile - 1) / kSolveTile);
+        if(parts & 1) ls_solve_tiled_kernel<false><<<tiles, 256, kSolveTileSmem, s>>>(L, npad, invL, B, ldb, nrhs, npad / NB, nreal);
+        if(parts & 2) ls_solve_tiled_kernel<true><<<tiles, 256, kSolveTileSmem, s>>>(L, npad, invL, B, ldb, nrhs, npad / NB, nreal);
+        if(nlaunch) *nlaunch += (parts & 1) + (parts >> 1);
+        MB200_CUDA_CHECK(cudaGetLastError());
+        return true;
+    }
+    if(nrhs != 1) return chol_solve_enqueue(L, npad, invL, B, ldb, nrhs, s, nlaunch, parts);
+    return run_graphed(GraphKey{L, B, npad, ldb, parts}, s, nlaunch,
+                       [&](int* n) { return chol_solve_enqueue(L, npad, invL, B, ldb, 1, s, n, parts); });
 }
 
 __global__ void debug_fill_spd_kernel(double* A, int n)

@@ -48,9 +48,15 @@ bool chol_solve_backward(const double* L, int npad, const double* invL, double* 
 // chol.cu: the multi-kernel factorization, which chol_factor runs above npad = 8192 (same arguments; no scratch)
 bool chol_factor_blocked(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch);
 
-// chol.cu: solve L L' X = B in place for nrhs right-hand sides stored as rows B[r][0..npad).
-// parts: 1 = only L Y = B, 2 = only L' X = B, 3 = both
-bool chol_solve(const double* L, int npad, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s, int* nlaunch, int parts = 3);
+// Right-hand sides per tile of the many-right-hand-side DMMA kernels (chol.cu's tiled solve, the structured factor's
+// forward panels), the row stride (doubles) of their tiles staged in shared memory, and that shared memory
+constexpr int kSolveTile = 32, kSolveTileLd = 68;
+constexpr size_t kSolveTileSmem = (size_t)(kSolveTile + kCholBlock) * kSolveTileLd * sizeof(double);
+
+// chol.cu: solve L L' X = B in place for nrhs right-hand sides stored as rows B[r][0..npad); unknowns >= nreal are
+// padding. parts: 1 = only L Y = B, 2 = only L' X = B, 3 = both. The kernels are chosen by nrhs
+bool chol_solve(const double* L, int npad, int nreal, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s,
+                int* nlaunch, int parts = 3);
 
 // drop cached CUDA graphs that reference this buffer (call before freeing it)
 void chol_forget_graphs(const void* A);

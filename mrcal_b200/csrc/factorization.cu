@@ -109,19 +109,30 @@ extern "C" bool mrcal_b200_factorization_solve_xt_JtJ_bt(mrcal_b200_factorizatio
 // L the Cholesky factor and D = I. The reference's CHOLMOD has its own P and a genuine D (simplicial LDL'), so
 // the individual pieces differ from CHOLMOD's -- but every identity between them holds, which is what callers
 // use (mrcal/model_analysis.py:837-841: sys='P', then 'L', then 'D')
+namespace mb200 {
+bool sys_steps(int sys, SysSteps* st)
+{
+    switch(sys)
+    {
+    case MRCAL_B200_SYS_A:    *st = {true,  true,  false, false}; return true;
+    case MRCAL_B200_SYS_LDLt: *st = {true,  true,  true,  true};  return true;
+    case MRCAL_B200_SYS_LD: case MRCAL_B200_SYS_L:   *st = {true,  false, true, true}; return true;
+    case MRCAL_B200_SYS_DLt: case MRCAL_B200_SYS_Lt: *st = {false, true,  true, true}; return true;
+    case MRCAL_B200_SYS_D:    *st = {false, false, true,  true};  return true;
+    case MRCAL_B200_SYS_P:    *st = {false, false, false, true};  return true;   // out = P b
+    case MRCAL_B200_SYS_Pt:   *st = {false, false, true,  false}; return true;   // out = P' b
+    default: set_error("Unknown sys %d given", sys); return false;
+    }
+}
+}  // namespace mb200
+
 extern "C" bool mrcal_b200_factorization_solve_sys(mrcal_b200_factorization_t* F, double* out, const double* bt, int Nrhs, int sys)
 {
     if(Nrhs <= 0) return true;
-    if(F->P != nullptr) return schur_factorization_solve(F, out, bt, Nrhs, sys);
-    int parts;
-    switch(sys)
-    {
-    case MRCAL_B200_SYS_A: case MRCAL_B200_SYS_LDLt: parts = 3; break;
-    case MRCAL_B200_SYS_LD: case MRCAL_B200_SYS_L:   parts = 1; break;
-    case MRCAL_B200_SYS_DLt: case MRCAL_B200_SYS_Lt: parts = 2; break;
-    case MRCAL_B200_SYS_D: case MRCAL_B200_SYS_P: case MRCAL_B200_SYS_Pt: parts = 0; break;
-    default: set_error("Unknown sys %d given", sys); return false;
-    }
+    SysSteps st;
+    if(!sys_steps(sys, &st)) return false;
+    if(F->P != nullptr) return schur_factorization_solve(F, out, bt, Nrhs, st);
+    const int parts = (st.fwd ? 1 : 0) | (st.bwd ? 2 : 0);
     if(parts == 0)
     {
         if(out != bt) memcpy(out, bt, (size_t)Nrhs * F->n * sizeof(double));
@@ -133,7 +144,7 @@ extern "C" bool mrcal_b200_factorization_solve_sys(mrcal_b200_factorization_t* F
     cudaStream_t s = F->stream;
     MB200_CUDA_CHECK(cudaMemcpy2DAsync(d_b, (size_t)F->npad * sizeof(double), bt, (size_t)F->n * sizeof(double),
                                        (size_t)F->n * sizeof(double), Nrhs, cudaMemcpyHostToDevice, s));
-    if(!chol_solve(F->H, F->npad, F->invL, d_b, F->npad, Nrhs, s, nullptr, parts)) return false;
+    if(!chol_solve(F->H, F->npad, F->n, F->invL, d_b, F->npad, Nrhs, s, nullptr, parts)) return false;
     MB200_CUDA_CHECK(cudaMemcpy2DAsync(out, (size_t)F->n * sizeof(double), d_b, (size_t)F->npad * sizeof(double),
                                        (size_t)F->n * sizeof(double), Nrhs, cudaMemcpyDeviceToHost, s));
     MB200_CUDA_CHECK(cudaStreamSynchronize(s));

@@ -17,6 +17,7 @@
 //
 // The object OWNS the device problem it was made from (the one the last mrcal_optimizer_callback() call left in the
 // cache): mrcal_b200_factorization_create_from_last_callback().
+#include "dmma.cuh"
 #include "solver_internal.h"
 
 namespace mb200 {
@@ -91,7 +92,7 @@ __device__ __forceinline__ int group_col0(const NormalBuffers& N, int grp)
     return grp < N.Nframe_groups ? 6 * grp : 6 * N.Nframe_groups + 3 * (grp - N.Nframe_groups);
 }
 
-// state-ordered right-hand sides -> the three pieces of the permuted vector. bt: [Nrhs][Nstate]
+// state-ordered right-hand sides <-> the three pieces of the permuted vector. bt, out: [Nrhs][Nstate]
 // Bf: [Nrhs][Nelim]   Bs: [Nrhs][ldS] (compact, zero padded)   Bi: [Nrhs][n_r] (reduced numbering; active slots unused)
 __global__ void split_state_kernel(NormalBuffers N, const double* __restrict__ bt, int Nstate, int Nrhs,
                                    double* __restrict__ Bf, int Nelim, double* __restrict__ Bs, double* __restrict__ Bi)
@@ -99,12 +100,7 @@ __global__ void split_state_kernel(NormalBuffers N, const double* __restrict__ b
     const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if(idx >= (long)Nrhs * Nstate) return;
     const int rhs = (int)(idx / Nstate), c = (int)(idx - (long)rhs * Nstate);
-    const double v = bt[idx];
-    if(c >= N.e0 && c < N.e1) { Bf[(size_t)rhs * Nelim + (c - N.e0)] = v; return; }
-    const int r = N.reduced_index(c);
-    const int cc = N.cidx[r];
-    if(cc >= 0) Bs[(size_t)rhs * N.ldS + cc] = v;
-    else        Bi[(size_t)rhs * N.n_r + r] = v;
+    *N.at(N.slot(c), Bf, Nelim, Bs, Bi, rhs) = bt[idx];
 }
 __global__ void join_state_kernel(NormalBuffers N, double* __restrict__ out, int Nstate, int Nrhs,
                                   const double* __restrict__ Bf, int Nelim, const double* __restrict__ Bs, const double* __restrict__ Bi)
@@ -112,15 +108,7 @@ __global__ void join_state_kernel(NormalBuffers N, double* __restrict__ out, int
     const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if(idx >= (long)Nrhs * Nstate) return;
     const int rhs = (int)(idx / Nstate), c = (int)(idx - (long)rhs * Nstate);
-    double v;
-    if(c >= N.e0 && c < N.e1) v = Bf[(size_t)rhs * Nelim + (c - N.e0)];
-    else
-    {
-        const int r = N.reduced_index(c);
-        const int cc = N.cidx[r];
-        v = cc >= 0 ? Bs[(size_t)rhs * N.ldS + cc] : Bi[(size_t)rhs * N.n_r + r];
-    }
-    out[idx] = v;
+    out[idx] = *N.at(N.slot(c), Bf, Nelim, Bs, Bi, rhs);
 }
 // the same two maps for vectors that are ALREADY in the permuted order [eliminated | compact | uncoupled (reduced order)]
 __global__ void split_permuted_kernel(NormalBuffers N, const double* __restrict__ bt, int Nstate, int Nrhs, bool to_pieces,
@@ -131,19 +119,12 @@ __global__ void split_permuted_kernel(NormalBuffers N, const double* __restrict_
     const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if(idx >= (long)Nrhs * Nstate) return;
     const int rhs = (int)(idx / Nstate), c = (int)(idx - (long)rhs * Nstate);
-    // c is a STATE index; its slot in the permuted vector:
-    int slot;
-    double* piece;
-    if(c >= N.e0 && c < N.e1) { slot = c - N.e0; piece = &Bf[(size_t)rhs * Nelim + (c - N.e0)]; }
-    else
-    {
-        const int r = N.reduced_index(c);
-        const int cc = N.cidx[r];
-        if(cc >= 0) { slot = Nelim + cc; piece = &Bs[(size_t)rhs * N.ldS + cc]; }
-        else        { slot = Nelim + N.n_c + ia_rank[r]; piece = &Bi[(size_t)rhs * N.n_r + r]; }
-    }
-    if(to_pieces) *piece = bt[(size_t)rhs * Nstate + slot];
-    else          out[(size_t)rhs * Nstate + slot] = *piece;
+    // c is a STATE index; its place in the permuted vector:
+    const NormalBuffers::Slot sl = N.slot(c);
+    const int perm = sl.piece == 0 ? sl.i : sl.piece == 1 ? Nelim + sl.i : Nelim + N.n_c + ia_rank[sl.i];
+    double* piece = N.at(sl, Bf, Nelim, Bs, Bi, rhs);
+    if(to_pieces) *piece = bt[(size_t)rhs * Nstate + perm];
+    else          out[(size_t)rhs * Nstate + perm] = *piece;
 }
 
 // L_D z = b (forward) or L_D' x = z (backward) per group and right-hand side, in place in Bf
@@ -167,30 +148,78 @@ __global__ void groups_tri_kernel(NormalBuffers N, double* __restrict__ Bf, int 
     for(int p = 0; p < nelim; p++) b[p] = o[p];
 }
 
-// Bs[rhs][64 blk .. +64) -= sum over the groups that reach block blk of  Y_g[blk]' z_g      (forward, before L_S)
-// One CTA per (block, right-hand side): thread = column of the block; groups in index order: deterministic
-__global__ void __launch_bounds__(64)
-panels_forward_kernel(NormalBuffers N, const double* __restrict__ Bf, int Nelim, double* __restrict__ Bs)
+// Forward panels: Bs[r][64 blk + col] -= sum over the groups g that reach block blk of  Zf[r][g] Y_g[blk][:, col].
+// One CTA per (block, tile of kSolveTile right-hand sides); the groups in index order, 8 per stage, each padded to 8
+// unknowns. (The panels carry the solver's right-hand-side column at compact index n_c: not part of the factor)
+__global__ void __launch_bounds__(256)
+panels_forward_tiled_kernel(NormalBuffers N, const double* __restrict__ Bf, int Nelim, double* __restrict__ Bs, int Nrhs)
 {
-    const int blk = blockIdx.x, rhs = blockIdx.y, col = threadIdx.x;
-    // (the panels carry the solver's right-hand-side column at compact index n_c: not part of the factor)
-    if(TB * blk + col >= N.n_c) return;
+    extern __shared__ __align__(16) double dsm[];
+    double (*sA)[kSolveTileLd] = reinterpret_cast<double (*)[kSolveTileLd]>(dsm);
+    double (*sM)[kSolveTileLd] = reinterpret_cast<double (*)[kSolveTileLd]>(dsm + kSolveTile * kSolveTileLd);
+    const int blk = blockIdx.x, r0 = blockIdx.y * kSolveTile;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g8 = lane >> 2, t4 = lane & 3;
+    const int mt = warp >> 1, nt0 = (warp & 1) * 4;   // warp: rows mt*8.., n-tiles nt0..nt0+3
+    double acc[4][2] = {};
     const unsigned* present = N.grp_present + (size_t)blk * N.gwords;
-    double acc = 0.;
+    int gid[8], nb = 0;
+    auto stage = [&]()
+    {
+        for(int e = tid; e < kSolveTile * 64; e += 256)
+        {
+            const int r = e >> 6, kk = e & 63, q = kk >> 3, pp = kk & 7;
+            double v = 0.;
+            if(q < nb && r0 + r < Nrhs)
+            {
+                const int g = gid[q], ne = g < N.Nframe_groups ? 6 : 3;
+                const int col0 = g < N.Nframe_groups ? 6 * g : 6 * N.Nframe_groups + 3 * (g - N.Nframe_groups);
+                if(pp < ne) v = Bf[(size_t)(r0 + r) * Nelim + col0 + pp];
+            }
+            sA[r][kk] = v;
+        }
+        for(int e = tid; e < 64 * TB; e += 256)
+        {
+            const int kk = e >> 6, col = e & 63, q = kk >> 3, pp = kk & 7;
+            double v = 0.;
+            if(q < nb)
+            {
+                const int g = gid[q], ne = g < N.Nframe_groups ? 6 : 3;
+                if(pp < ne) v = N.Ypan[((size_t)g * N.nblk_max + blk) * kYpanel + pp * kYld + col];
+            }
+            sM[kk][col] = v;
+        }
+        __syncthreads();
+        const int ksteps = 2 * nb;
+        for(int ks = 0; ks < ksteps; ks++)
+        {
+            const double a = sA[mt * 8 + g8][ks * 4 + t4];
+#pragma unroll
+            for(int j = 0; j < 4; j++) dmma(acc[j][0], acc[j][1], a, sM[ks * 4 + t4][(nt0 + j) * 8 + g8]);
+        }
+        __syncthreads();
+        nb = 0;
+    };
     for(int w = 0; w < N.gwords; w++)
     {
         unsigned m = present[w];
         while(m)
         {
-            const int grp = 32 * w + __ffs(m) - 1;
+            gid[nb++] = 32 * w + __ffs(m) - 1;
             m &= m - 1;
-            const double* Y = N.Ypan + ((size_t)grp * N.nblk_max + blk) * kYpanel;
-            const double* z = Bf + (size_t)rhs * Nelim + group_col0(N, grp);
-            const int nelim = grp < N.Nframe_groups ? 6 : 3;
-            for(int p = 0; p < nelim; p++) acc += Y[p * kYld + col] * z[p];
+            if(nb == 8) stage();
         }
     }
-    Bs[(size_t)rhs * N.ldS + TB * blk + col] -= acc;
+    if(nb > 0) stage();
+    const int r = r0 + mt * 8 + g8;
+    if(r >= Nrhs) return;
+#pragma unroll
+    for(int j = 0; j < 4; j++)
+        for(int h = 0; h < 2; h++)
+        {
+            const int col = TB * blk + (nt0 + j) * 8 + 2 * t4 + h;
+            if(col < N.n_c) Bs[(size_t)r * N.ldS + col] -= acc[j][h];
+        }
 }
 // z_g -= Y_g x_s  (backward, after L_S'): one warp per (group, right-hand side)
 __global__ void __launch_bounds__(256)
@@ -264,25 +293,43 @@ __global__ void diag_minmax_rest_kernel(NormalBuffers N, const double* __restric
 
 }  // namespace
 
-bool schur_factorization_solve(mrcal_b200_factorization* F, double* out, const double* bt, int Nrhs, int sys)
+bool schur_solve_pieces(const mrcal_b200_factorization* F, double* Bf, double* Bs, double* Bi, int Nrhs, bool forward,
+                        BackSolve backward, cudaStream_t s)
+{
+    const SolverWorkspace* ws = F->P->ws.get();
+    const NormalBuffers& N = ws->N;
+    const int Nelim = F->Nelim, nblk = N.ldS / TB;
+    const long gr = (long)Nrhs * N.Ngroups, ir = (long)Nrhs * N.n_r;
+    if(forward)
+    {
+        if(N.Ngroups > 0)
+        {
+            groups_tri_kernel<<<(unsigned)((gr + 127) / 128), 128, 0, s>>>(N, Bf, Nelim, Nrhs, true);
+            panels_forward_tiled_kernel<<<dim3(nblk, (Nrhs + kSolveTile - 1) / kSolveTile), 256, kSolveTileSmem, s>>>(N, Bf, Nelim, Bs, Nrhs);
+        }
+        if(N.n_c > 0 && !chol_solve(N.S, N.ldS, N.n_c, ws->invL, Bs, N.ldS, Nrhs, s, nullptr, 1)) return false;
+        if(N.n_r > N.n_c) inactive_tri_kernel<<<(unsigned)((ir + 255) / 256), 256, 0, s>>>(N, F->ia_L, F->ia_first, Bi, Nrhs, true);
+    }
+    if(backward != BackSolve::none)
+    {
+        if(N.n_r > N.n_c) inactive_tri_kernel<<<(unsigned)((ir + 255) / 256), 256, 0, s>>>(N, F->ia_L, F->ia_first, Bi, Nrhs, false);
+        if(N.n_c > 0 && !chol_solve(N.S, N.ldS, N.n_c, ws->invL, Bs, N.ldS, Nrhs, s, nullptr, 2)) return false;
+        if(backward == BackSolve::all && N.Ngroups > 0)
+        {
+            panels_backward_kernel<<<(unsigned)((gr * 32 + 255) / 256), 256, 0, s>>>(N, Bf, Nelim, Bs, Nrhs, nblk);
+            groups_tri_kernel<<<(unsigned)((gr + 127) / 128), 128, 0, s>>>(N, Bf, Nelim, Nrhs, false);
+        }
+    }
+    MB200_CUDA_CHECK(cudaGetLastError());
+    return true;
+}
+
+bool schur_factorization_solve(mrcal_b200_factorization* F, double* out, const double* bt, int Nrhs, const SysSteps& st)
 {
     mrcal_b200_problem* P = F->P;
-    SolverWorkspace* ws = P->ws.get();
-    NormalBuffers& N = ws->N;
+    NormalBuffers& N = P->ws->N;
     cudaStream_t s = P->stream;
-    const int Nstate = P->L.Nstate, Nelim = F->Nelim, nblk = N.ldS / TB;
-    bool fwd, bwd, permuted_in, permuted_out;
-    switch(sys)
-    {
-    case MRCAL_B200_SYS_A:    fwd = true;  bwd = true;  permuted_in = false; permuted_out = false; break;
-    case MRCAL_B200_SYS_LDLt: fwd = true;  bwd = true;  permuted_in = true;  permuted_out = true;  break;
-    case MRCAL_B200_SYS_LD: case MRCAL_B200_SYS_L:   fwd = true;  bwd = false; permuted_in = true; permuted_out = true; break;
-    case MRCAL_B200_SYS_DLt: case MRCAL_B200_SYS_Lt: fwd = false; bwd = true;  permuted_in = true; permuted_out = true; break;
-    case MRCAL_B200_SYS_D:    fwd = false; bwd = false; permuted_in = true;  permuted_out = true;  break;
-    case MRCAL_B200_SYS_P:    fwd = false; bwd = false; permuted_in = false; permuted_out = true;  break;   // out = P b
-    case MRCAL_B200_SYS_Pt:   fwd = false; bwd = false; permuted_in = true;  permuted_out = false; break;   // out = P' b
-    default: set_error("Unknown sys %d given", sys); return false;
-    }
+    const int Nstate = P->L.Nstate, Nelim = F->Nelim;
     DeviceArena tmp;
     double *d_in, *d_out, *Bf, *Bs, *Bi;
     if(!tmp.alloc(&d_in, (size_t)Nrhs * Nstate) || !tmp.alloc(&d_out, (size_t)Nrhs * Nstate) ||
@@ -292,30 +339,10 @@ bool schur_factorization_solve(mrcal_b200_factorization* F, double* out, const d
     MB200_CUDA_CHECK(cudaMemcpyAsync(d_in, bt, (size_t)Nrhs * Nstate * sizeof(double), cudaMemcpyHostToDevice, s));
     const long tot = (long)Nrhs * Nstate;
     const unsigned gtot = (unsigned)((tot + 255) / 256);
-    if(permuted_in) split_permuted_kernel<<<gtot, 256, 0, s>>>(N, d_in, Nstate, Nrhs, true, Bf, Nelim, Bs, Bi, F->ia_first + N.n_r, nullptr);
+    if(st.permuted_in) split_permuted_kernel<<<gtot, 256, 0, s>>>(N, d_in, Nstate, Nrhs, true, Bf, Nelim, Bs, Bi, F->ia_first + N.n_r, nullptr);
     else            split_state_kernel<<<gtot, 256, 0, s>>>(N, d_in, Nstate, Nrhs, Bf, Nelim, Bs, Bi);
-    const long gr = (long)Nrhs * N.Ngroups, ir = (long)Nrhs * N.n_r;
-    if(fwd)
-    {
-        if(N.Ngroups > 0)
-        {
-            groups_tri_kernel<<<(unsigned)((gr + 127) / 128), 128, 0, s>>>(N, Bf, Nelim, Nrhs, true);
-            panels_forward_kernel<<<dim3(nblk, Nrhs), 64, 0, s>>>(N, Bf, Nelim, Bs);
-        }
-        if(N.n_c > 0 && !chol_solve(N.S, N.ldS, ws->invL, Bs, N.ldS, Nrhs, s, nullptr, 1)) return false;
-        if(N.n_r > N.n_c) inactive_tri_kernel<<<(unsigned)((ir + 255) / 256), 256, 0, s>>>(N, F->ia_L, F->ia_first, Bi, Nrhs, true);
-    }
-    if(bwd)
-    {
-        if(N.n_r > N.n_c) inactive_tri_kernel<<<(unsigned)((ir + 255) / 256), 256, 0, s>>>(N, F->ia_L, F->ia_first, Bi, Nrhs, false);
-        if(N.n_c > 0 && !chol_solve(N.S, N.ldS, ws->invL, Bs, N.ldS, Nrhs, s, nullptr, 2)) return false;
-        if(N.Ngroups > 0)
-        {
-            panels_backward_kernel<<<(unsigned)((gr * 32 + 255) / 256), 256, 0, s>>>(N, Bf, Nelim, Bs, Nrhs, nblk);
-            groups_tri_kernel<<<(unsigned)((gr + 127) / 128), 128, 0, s>>>(N, Bf, Nelim, Nrhs, false);
-        }
-    }
-    if(permuted_out) split_permuted_kernel<<<gtot, 256, 0, s>>>(N, nullptr, Nstate, Nrhs, false, Bf, Nelim, Bs, Bi, F->ia_first + N.n_r, d_out);
+    if(!schur_solve_pieces(F, Bf, Bs, Bi, Nrhs, st.fwd, st.bwd ? BackSolve::all : BackSolve::none, s)) return false;
+    if(st.permuted_out) split_permuted_kernel<<<gtot, 256, 0, s>>>(N, nullptr, Nstate, Nrhs, false, Bf, Nelim, Bs, Bi, F->ia_first + N.n_r, d_out);
     else             join_state_kernel<<<gtot, 256, 0, s>>>(N, d_out, Nstate, Nrhs, Bf, Nelim, Bs, Bi);
     MB200_CUDA_CHECK(cudaGetLastError());
     MB200_CUDA_CHECK(cudaMemcpyAsync(out, d_out, (size_t)Nrhs * Nstate * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -361,6 +388,8 @@ bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F)
 {
     if(comm_active() || P->sharded) { set_error("structured factorization: not available for sharded problems"); return false; }
     if(!solver_build_workspace(P)) return false;
+    // every solve with the factor takes the forward panels' tiles (schur_solve_pieces): more than 48 KB of shared memory
+    MB200_CUDA_CHECK(cudaFuncSetAttribute(panels_forward_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveTileSmem));
     SolverWorkspace* ws = P->ws.get();
     NormalBuffers& N = ws->N;
     cudaStream_t s = P->stream;
@@ -387,20 +416,6 @@ bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F)
     F->n = P->L.Nstate;
     F->Nelim = N.e1 - N.e0;
     return true;
-}
-
-// L_D z = b / L_D' x = z and L_I z = b / L_I' x = z on pieces laid out as schur_factorization_solve() lays them out
-void schur_groups_tri(const mrcal_b200_factorization* F, double* Bf, int Nrhs, bool forward, cudaStream_t s)
-{
-    const NormalBuffers& N = F->P->ws->N;
-    const long gr = (long)Nrhs * N.Ngroups;
-    if(gr > 0) groups_tri_kernel<<<(unsigned)((gr + 127) / 128), 128, 0, s>>>(N, Bf, F->Nelim, Nrhs, forward);
-}
-void schur_inactive_tri(const mrcal_b200_factorization* F, double* Bi, int Nrhs, bool forward, cudaStream_t s)
-{
-    const NormalBuffers& N = F->P->ws->N;
-    const long ir = (long)Nrhs * N.n_r;
-    if(N.n_r > N.n_c) inactive_tri_kernel<<<(unsigned)((ir + 255) / 256), 256, 0, s>>>(N, F->ia_L, F->ia_first, Bi, Nrhs, forward);
 }
 
 }  // namespace mb200

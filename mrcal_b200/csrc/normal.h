@@ -91,6 +91,23 @@ struct NormalBuffers
 
     __host__ __device__ int reduced_index(int c) const { return c < e0 ? c : c - (e1 - e0); }
     __host__ __device__ int state_index(int r) const { return r < e0 ? r : r + (e1 - e0); }
+
+    // Where state column c lives in the three pieces of a permuted vector (the structured factor's right-hand sides,
+    // factorization_schur.cu): piece 0 = Bf[.][i] (eliminated), 1 = Bs[.][i] (coupled, compact numbering),
+    // 2 = Bi[.][i] (uncoupled, reduced numbering)
+    struct Slot { int piece, i; };
+    __device__ Slot slot(int c) const
+    {
+        if(c >= e0 && c < e1) return {0, c - e0};
+        const int r = reduced_index(c);
+        return cidx[r] >= 0 ? Slot{1, cidx[r]} : Slot{2, r};
+    }
+    // that slot of right-hand side `rhs`
+    template <typename T>
+    __device__ T* at(Slot s, T* Bf, int Nelim, T* Bs, T* Bi, size_t rhs) const
+    {
+        return s.piece == 0 ? &Bf[rhs * Nelim + s.i] : s.piece == 1 ? &Bs[rhs * ldS + s.i] : &Bi[rhs * n_r + s.i];
+    }
 };
 
 // The same in pieces, for a caller that wants to pick its own moment to wait for the device:

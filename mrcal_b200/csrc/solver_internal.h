@@ -66,15 +66,25 @@ struct mrcal_b200_factorization
 };
 
 namespace mb200 {
-bool schur_factorization_solve(mrcal_b200_factorization* F, double* out, const double* bt, int Nrhs, int sys);
+// What solve_xt_JtJ_bt(sys=...) does with a factor P JtJ P' = L L' (D = I): the solve with L, the one with L', and
+// whether the input and the output are in the permuted order. The dense factor has P = I.
+// sys_steps (factorization.cu): false, with the error set, for an unknown sys
+struct SysSteps { bool fwd, bwd, permuted_in, permuted_out; };
+bool sys_steps(int sys, SysSteps* st);
+
+bool schur_factorization_solve(mrcal_b200_factorization* F, double* out, const double* bt, int Nrhs, const SysSteps& st);
 double schur_factorization_rcond(mrcal_b200_factorization* F);
 void schur_factorization_release(mrcal_b200_factorization* F);
 bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F);
+// The triangular solves with the structured factor, in place on the pieces of the permuted right-hand sides as
+// NormalBuffers::slot() lays them out. forward: L_D, the panels, L_S, L_I. backward: L_I', L_S', then (all) the panels
+// and L_D'; `shared` stops after L_S', with X on the shared unknowns only
+enum class BackSolve { none, shared, all };
+bool schur_solve_pieces(const mrcal_b200_factorization* F, double* Bf, double* Bs, double* Bi, int Nrhs, bool forward,
+                        BackSolve backward, cudaStream_t s);
 // csr_ops.cu
 bool csr_stable_transpose(const int* p, const int* col, int Nrows, int nnz, int Ncols, DeviceArena& arena,
                           int** tp, int** tsrc, int** trow, cudaStream_t s);
-void schur_groups_tri(const mrcal_b200_factorization* F, double* Bf, int Nrhs, bool forward, cudaStream_t s);
-void schur_inactive_tri(const mrcal_b200_factorization* F, double* Bi, int Nrhs, bool forward, cudaStream_t s);
 // cross_reprojection.cu: K = drt/db_packed (6 x Nstate, row-major) into device memory; evaluate: evaluate the
 // Jacobian at the current state first (false: the caller just did)
 bool cross_reprojection_K(mrcal_b200_problem* P, int icam_intrinsics, bool evaluate, double* d_K);

@@ -19,12 +19,9 @@
 // are never eliminated, so X is needed only on the shared unknowns and the backward pass stops after L_S' (the panels
 // are not needed in that direction). Without regularization rows Var = sigma^2 Z'Z (:784-843).
 //
-// The many-right-hand-side pieces are DMMA (mma.sync.m8n8k4.f64) kernels that take a tile of 32 right-hand sides:
-//   panels  Bs[tile][64-col block] -= Zf[tile][groups of the block] Y[groups][block]   one CTA per (block, tile)
-//   L_S     left-looking blocked solve, 64x64 blocks: every off-diagonal block of L_S is one GEMM against the tile,
-//           every diagonal block one GEMM with its stored inverse                       one CTA per tile
-// Each panel and each block of L_S is read once per tile instead of once per right-hand side. The 2x2 per point is
-// reduced by one warp in a fixed order: no atomics anywhere, two calls give bit-identical results.
+// The triangular solves are the structured factor's own (schur_solve_pieces(), factorization_schur.cu), which take
+// tiles of kSolveTile right-hand sides when there are many. The 2x2 per point is reduced by one warp in a fixed order:
+// no atomics anywhere, two calls give bit-identical results.
 #include <algorithm>
 
 #include "device_math.cuh"
@@ -33,17 +30,6 @@
 namespace mb200 {
 
 namespace {
-
-constexpr int TB = 64;     // block of L_S and of the panels
-constexpr int RT = 32;     // right-hand sides per tile
-constexpr int SLD = 68;    // shared-memory row stride of the staged tiles (doubles)
-constexpr size_t kTileSmem = (size_t)(RT + TB) * SLD * sizeof(double);
-
-__device__ __forceinline__ void dmma(double& c0, double& c1, double a, double b)
-{
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                 : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
 
 struct RowArgs
 {
@@ -56,15 +42,6 @@ struct RowArgs
     int Nelim;
     const double* scale;  // [Nstate] pack scales
 };
-
-// where state column c of right-hand side `row` lives in the pieces
-__device__ __forceinline__ double* slot(const NormalBuffers& N, double* Bf, int Nelim, double* Bs, double* Bi, int row, int c)
-{
-    if(c >= N.e0 && c < N.e1) return &Bf[(size_t)row * Nelim + (c - N.e0)];
-    const int r = N.reduced_index(c);
-    const int cc = N.cidx[r];
-    return cc >= 0 ? &Bs[(size_t)row * N.ldS + cc] : &Bi[(size_t)row * N.n_r + r];
-}
 
 // transform_point_rt(rt, p) and its gradient in r: R p + t, d(R p)/dr (3x3). rotation only: R p
 __device__ __forceinline__ void pose_apply(double out[3], double d_dr[3][3], const double R[9], const double dR[27], const double* t, const double p[3])
@@ -92,7 +69,7 @@ uncertainty_rows_kernel(DevProblem P, NormalBuffers N, RowArgs A, const double* 
     const double p[3] = {pcam[3 * i], pcam[3 * i + 1], pcam[3 * i + 2]};
     const double* intr = P.u_intr + (size_t)A.icam * P.Nintr;
     const int r0 = 2 * i;
-    auto put = [&](int row, int c, double v) { *slot(N, Bf, A.Nelim, Bs, Bi, row, c) = v * A.scale[c]; };
+    auto put = [&](int row, int c, double v) { *N.at(N.slot(c), Bf, A.Nelim, Bs, Bi, row) = v * A.scale[c]; };
     // intrinsics parameter k (of the model's Nintr) -> its state column, or -1
     auto intr_col = [&](int k) { const int j = k - A.intr_arg0; return (A.intr_col0 >= 0 && j >= 0 && j < P.Nintr_state) ? A.intr_col0 + j : -1; };
 
@@ -182,7 +159,7 @@ uncertainty_rows_kernel(DevProblem P, NormalBuffers N, RowArgs A, const double* 
                     for(int k = 0; k < 3; k++) v[3 + k] = inf ? 0. : dqr[a][k] * w;
                     for(int k = 0; k < 6; k++)
                     {
-                        double* s = slot(N, Bf, A.Nelim, Bs, Bi, r0 + a, c0 + k);
+                        double* s = N.at(N.slot(c0 + k), Bf, A.Nelim, Bs, Bi, r0 + a);
                         const double add = v[k] * A.scale[c0 + k];
                         *s = j == 0 ? add : *s + add;
                     }
@@ -221,162 +198,7 @@ __global__ void uncertainty_K_kernel(NormalBuffers N, int Nelim, const double* _
     double v = 0.;
 #pragma unroll
     for(int k = 0; k < 6; k++) v += G[(size_t)row * 6 + k] * K[(size_t)k * Nstate + c];
-    *slot(N, Bf, Nelim, Bs, Bi, row, c) += v;
-}
-
-// Forward panels: Bs[r][64 blk + col] -= sum over the groups g that reach block blk of  Zf[r][g] Y_g[blk][:, col].
-// One CTA per (block, tile of RT right-hand sides); the groups in index order, 8 per stage, each padded to 8 unknowns
-__global__ void __launch_bounds__(256)
-panels_forward_tiled_kernel(NormalBuffers N, const double* __restrict__ Bf, int Nelim, double* __restrict__ Bs, int Nrhs)
-{
-    extern __shared__ __align__(16) double dsm[];
-    double (*sA)[SLD] = reinterpret_cast<double (*)[SLD]>(dsm);
-    double (*sM)[SLD] = reinterpret_cast<double (*)[SLD]>(dsm + RT * SLD);
-    const int blk = blockIdx.x, r0 = blockIdx.y * RT;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int g8 = lane >> 2, t4 = lane & 3;
-    const int mt = warp >> 1, nt0 = (warp & 1) * 4;   // warp: rows mt*8.., n-tiles nt0..nt0+3
-    double acc[4][2] = {};
-    const unsigned* present = N.grp_present + (size_t)blk * N.gwords;
-    int gid[8], nb = 0;
-    auto stage = [&]()
-    {
-        for(int e = tid; e < RT * 64; e += 256)
-        {
-            const int r = e >> 6, kk = e & 63, q = kk >> 3, pp = kk & 7;
-            double v = 0.;
-            if(q < nb && r0 + r < Nrhs)
-            {
-                const int g = gid[q], ne = g < N.Nframe_groups ? 6 : 3;
-                const int col0 = g < N.Nframe_groups ? 6 * g : 6 * N.Nframe_groups + 3 * (g - N.Nframe_groups);
-                if(pp < ne) v = Bf[(size_t)(r0 + r) * Nelim + col0 + pp];
-            }
-            sA[r][kk] = v;
-        }
-        for(int e = tid; e < 64 * TB; e += 256)
-        {
-            const int kk = e >> 6, col = e & 63, q = kk >> 3, pp = kk & 7;
-            double v = 0.;
-            if(q < nb)
-            {
-                const int g = gid[q], ne = g < N.Nframe_groups ? 6 : 3;
-                if(pp < ne) v = N.Ypan[((size_t)g * N.nblk_max + blk) * kYpanel + pp * kYld + col];
-            }
-            sM[kk][col] = v;
-        }
-        __syncthreads();
-        const int ksteps = 2 * nb;
-        for(int ks = 0; ks < ksteps; ks++)
-        {
-            const double a = sA[mt * 8 + g8][ks * 4 + t4];
-#pragma unroll
-            for(int j = 0; j < 4; j++) dmma(acc[j][0], acc[j][1], a, sM[ks * 4 + t4][(nt0 + j) * 8 + g8]);
-        }
-        __syncthreads();
-        nb = 0;
-    };
-    for(int w = 0; w < N.gwords; w++)
-    {
-        unsigned m = present[w];
-        while(m)
-        {
-            gid[nb++] = 32 * w + __ffs(m) - 1;
-            m &= m - 1;
-            if(nb == 8) stage();
-        }
-    }
-    if(nb > 0) stage();
-    const int r = r0 + mt * 8 + g8;
-    if(r >= Nrhs) return;
-#pragma unroll
-    for(int j = 0; j < 4; j++)
-        for(int h = 0; h < 2; h++)
-        {
-            const int col = TB * blk + (nt0 + j) * 8 + 2 * t4 + h;
-            if(col < N.n_c) Bs[(size_t)r * N.ldS + col] -= acc[j][h];
-        }
-}
-
-// L y = b (BWD = false) or L' x = b (BWD = true) for a tile of RT right-hand sides B[r][0..ldb), in place, left-looking
-// over 64-blocks: block i takes the GEMM of every already-solved block k with L's block (i,k) (or (k,i)'), then the
-// GEMM with the stored inverse of its diagonal block. Unknowns >= nreal are treated as zero
-template <bool BWD>
-__global__ void __launch_bounds__(256)
-ls_solve_tiled_kernel(const double* __restrict__ L, int ld, const double* __restrict__ invL, double* __restrict__ B, int ldb,
-                      int Nrhs, int nblk, int nreal)
-{
-    extern __shared__ __align__(16) double dsm[];
-    double (*sA)[SLD] = reinterpret_cast<double (*)[SLD]>(dsm);
-    double (*sM)[SLD] = reinterpret_cast<double (*)[SLD]>(dsm + RT * SLD);
-    const int r0 = blockIdx.x * RT;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int g8 = lane >> 2, t4 = lane & 3;
-    const int mt = warp >> 1, nt0 = (warp & 1) * 4;
-    auto gemm = [&](double (&acc)[4][2], bool trans)
-    {
-#pragma unroll 4
-        for(int ks = 0; ks < TB / 4; ks++)
-        {
-            const double a = sA[mt * 8 + g8][ks * 4 + t4];
-#pragma unroll
-            for(int j = 0; j < 4; j++)
-            {
-                const int n = (nt0 + j) * 8 + g8, k = ks * 4 + t4;
-                dmma(acc[j][0], acc[j][1], a, trans ? sM[k][n] : sM[n][k]);
-            }
-        }
-    };
-    auto load_rhs = [&](int kb)
-    {
-        for(int e = tid; e < RT * TB; e += 256)
-        {
-            const int r = e >> 6, m = e & 63, c = kb * TB + m;
-            sA[r][m] = (r0 + r < Nrhs && c < nreal) ? B[(size_t)(r0 + r) * ldb + c] : 0.;
-        }
-    };
-    for(int step = 0; step < nblk; step++)
-    {
-        const int i = BWD ? nblk - 1 - step : step;
-        double acc[4][2] = {};
-        for(int s = 0; s < step; s++)
-        {
-            const int k = BWD ? nblk - 1 - s : s;
-            load_rhs(k);
-            // forward: sM[n][m] = L(i*64+n, k*64+m);  backward: sM[m][n] = L(k*64+m, i*64+n)
-            for(int e = tid; e < TB * TB; e += 256)
-            {
-                const int a = e >> 6, b = e & 63;
-                const int row = BWD ? k * TB + a : i * TB + a, col = BWD ? i * TB + b : k * TB + b;
-                sM[a][b] = (row < nreal && col < nreal) ? L[(size_t)row * ld + col] : 0.;
-            }
-            __syncthreads();
-            gemm(acc, BWD);
-            __syncthreads();
-        }
-        load_rhs(i);
-        for(int e = tid; e < TB * TB; e += 256) sM[e >> 6][e & 63] = invL[(size_t)i * TB * TB + e];
-        __syncthreads();
-#pragma unroll
-        for(int j = 0; j < 4; j++)
-        {
-            sA[mt * 8 + g8][(nt0 + j) * 8 + 2 * t4] -= acc[j][0];
-            sA[mt * 8 + g8][(nt0 + j) * 8 + 2 * t4 + 1] -= acc[j][1];
-            acc[j][0] = acc[j][1] = 0.;
-        }
-        __syncthreads();
-        // forward: y[n] = sum_m invL[n][m] b[m];  backward: x[n] = sum_m invL[m][n] b[m]
-        gemm(acc, BWD);
-        const int r = r0 + mt * 8 + g8;
-        if(r < Nrhs)
-#pragma unroll
-            for(int j = 0; j < 4; j++)
-                for(int h = 0; h < 2; h++)
-                {
-                    const int c = i * TB + (nt0 + j) * 8 + 2 * t4 + h;
-                    if(c < nreal) B[(size_t)r * ldb + c] = acc[j][h];
-                }
-        __syncthreads();
-    }
+    *N.at(N.slot(c), Bf, Nelim, Bs, Bi, row) += v;
 }
 
 // Var0 = Z'Z per point: one warp per point, lanes over the unknowns, then a butterfly (fixed order)
@@ -419,11 +241,10 @@ __global__ void finish_kernel(const NormalBuffers N, const double* __restrict__ 
         double a = 0., b = 0.;
         for(int e = rowptr[m]; e < rowptr[m + 1]; e++)
         {
-            const int c = Jcol[e];
-            if(c >= N.e0 && c < N.e1) { *bad = 1; continue; }
-            const int r = N.reduced_index(c), cc = N.cidx[r];
-            const double xa = cc >= 0 ? Bs[(size_t)(2 * pt) * N.ldS + cc] : Bi[(size_t)(2 * pt) * N.n_r + r];
-            const double xb = cc >= 0 ? Bs[(size_t)(2 * pt + 1) * N.ldS + cc] : Bi[(size_t)(2 * pt + 1) * N.n_r + r];
+            const NormalBuffers::Slot sl = N.slot(Jcol[e]);
+            if(sl.piece == 0) { *bad = 1; continue; }
+            const double xa = *N.at<const double>(sl, nullptr, 0, Bs, Bi, 2 * pt);
+            const double xb = *N.at<const double>(sl, nullptr, 0, Bs, Bi, 2 * pt + 1);
             a += Jval[e] * xa; b += Jval[e] * xb;
         }
         s00 += a * a; s01 += a * b; s11 += b * b;
@@ -532,9 +353,6 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
     if(method == MRCAL_B200_UNCERTAINTY_RRP_JFP && Ne > 1) { set_error("I only handle stationary cameras for now"); return false; }
 
     cudaStream_t s = P->stream;
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(panels_forward_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(ls_solve_tiled_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(ls_solve_tiled_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem));
     // 1-2. the Jacobian at the current state, and the structured factor
     DeviceArena mem;
     mrcal_b200_factorization F;   // its buffers only: it does not own P here
@@ -543,8 +361,6 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
     const int Nstate = L.Nstate;
     if(!schur_factor_build(P, &F)) return false;
     const NormalBuffers N = P->ws->N;
-    const double* Lfac = N.S;
-    const double* invLfac = P->ws->invL;
     const int Nelim = F.Nelim;
     const int nBi = N.n_r;
     // 3. K, if the method needs it (the Jacobian was evaluated above)
@@ -577,7 +393,7 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
     const size_t per_rhs = (size_t)(Nelim > 0 ? Nelim : 1) + N.ldS + (nBi > 0 ? nBi : 1);
     const size_t budget = (size_t)512 << 20;
     int chunk = (int)(budget / (2 * per_rhs * sizeof(double)));
-    chunk = chunk < RT ? RT : (chunk / RT) * RT;
+    chunk = chunk < kSolveTile ? kSolveTile : (chunk / kSolveTile) * kSolveTile;
     if(chunk > Npts) chunk = Npts;
     const int maxrhs = 2 * chunk;
     double *Bf, *Bs, *Bi, *G, *pts, *V, *out;
@@ -586,7 +402,6 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
        !mem.alloc(&pts, (size_t)3 * Npts) || !mem.alloc(&V, (size_t)3 * chunk) || !mem.alloc(&out, (size_t)4 * Npts))
         return false;
     MB200_CUDA_CHECK(cudaMemcpyAsync(pts, p_cam, (size_t)3 * Npts * sizeof(double), cudaMemcpyHostToDevice, s));
-    const int nblkS = N.ldS / TB;
     const bool reg = L.Nmeas_reg > 0;
     for(int p0 = 0; p0 < Npts; p0 += chunk)
     {
@@ -601,20 +416,10 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
             uncertainty_K_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, s>>>(N, Nelim, G, K, Nstate, c0K, nr, Bf, Bs, Bi);
         }
         // Z = inv(L) P dF'
-        if(N.Ngroups > 0)
-        {
-            schur_groups_tri(&F, Bf, nr, true, s);
-            panels_forward_tiled_kernel<<<dim3(nblkS, (nr + RT - 1) / RT), 256, kTileSmem, s>>>(N, Bf, Nelim, Bs, nr);
-        }
-        if(N.n_c > 0) ls_solve_tiled_kernel<false><<<(nr + RT - 1) / RT, 256, kTileSmem, s>>>(Lfac, N.ldS, invLfac, Bs, N.ldS, nr, nblkS, N.n_c);
-        schur_inactive_tri(&F, Bi, nr, true, s);
+        if(!schur_solve_pieces(&F, Bf, Bs, Bi, nr, true, BackSolve::none, s)) return false;
         ztz_kernel<<<(unsigned)((np * 32 + 255) / 256), 256, 0, s>>>(N, Bf, Nelim, Bs, Bi, nBi, np, V);
         // X on the shared unknowns = inv(L_S') Z_s, inv(L_I') Z_i
-        if(reg)
-        {
-            schur_inactive_tri(&F, Bi, nr, false, s);
-            if(N.n_c > 0) ls_solve_tiled_kernel<true><<<(nr + RT - 1) / RT, 256, kTileSmem, s>>>(Lfac, N.ldS, invLfac, Bs, N.ldS, nr, nblkS, N.n_c);
-        }
+        if(reg && !schur_solve_pieces(&F, Bf, Bs, Bi, nr, false, BackSolve::shared, s)) return false;
         finish_kernel<<<(unsigned)((np * 32 + 255) / 256), 256, 0, s>>>(N, Bs, Bi, P->d_rowptr, op.Jcol, op.Jval, L.m_reg0,
                                                                          reg ? L.m_reg0 + L.Nmeas_reg : L.m_reg0, np, V, sigma,
                                                                          out + 4 * (size_t)p0, bad);

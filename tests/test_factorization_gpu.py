@@ -37,15 +37,20 @@ def test_reference_known_answer():
     assert np.allclose(F.solve_xt_JtJ_bt(bt, sys="L"), np.linalg.solve(L, bt.T).T, rtol=1e-12)
 
 
-# n = 100: two 64-blocks; n = 8300: 130 of them
-@pytest.mark.parametrize("n,m,density", [(50, 200, 0.2), (64, 300, 0.1), (100, 400, 0.1), (200, 1500, 0.05), (700, 6000, 0.02),
-                                         (1100, 9000, 0.01), (8300, 9000, 0.0005)])
-def test_random_sparse(n, m, density):
+# n = 100: two 64-blocks; n = 8300: 130 of them. 3 right-hand sides take the per-block solve; 1100 the tiled one, which
+# takes over at 8 right-hand sides per 64-block
+_SPARSE = [(50, 200, 0.2), (64, 300, 0.1), (100, 400, 0.1), (200, 1500, 0.05), (700, 6000, 0.02), (1100, 9000, 0.01),
+           (8300, 9000, 0.0005)]
+
+
+@pytest.mark.parametrize("n,m,density,nrhs", [pytest.param(*c, 3, id="-".join(map(str, c))) for c in _SPARSE] +
+                         [pytest.param(8300, 9000, 0.0005, 1100, id="8300-9000-0.0005-1100rhs")])
+def test_random_sparse(n, m, density, nrhs):
     rng = np.random.default_rng(n)
     J = scipy.sparse.random(m, n, density=density, random_state=np.random.RandomState(n), format="csr")
     J = (J + scipy.sparse.vstack([scipy.sparse.eye(n) * 0.5, scipy.sparse.csr_matrix((m - n, n))])).tocsr()
     H = (J.T @ J).toarray()
-    bt = rng.normal(size=(3, n))
+    bt = rng.normal(size=(nrhs, n))
     F = mrcal_b200.CHOLMOD_factorization(J)
     xt = F.solve_xt_JtJ_bt(bt)
     r = (H @ xt.T).T - bt
@@ -75,14 +80,20 @@ def test_optimizer_callback_returns_factorization():
 def test_solve_systems():
     """solve_xt_JtJ_bt(sys=...) (mrcal-pywrap.c:467-493). With P = I and D = I the factor L is THE Cholesky factor
     of JtJ (unique), so 'L' and 'Lt' are pinned by numpy; the identities the reference's callers rely on
-    (mrcal/model_analysis.py:837-841: P, then L, then D, and A2 A3' = b' inv(JtJ) b) are checked as such."""
+    (mrcal/model_analysis.py:837-841: P, then L, then D, and A2 A3' = b' inv(JtJ) b) are checked as such.
+    n = 150 is three 64-blocks: 7 right-hand sides take the per-block solve, 100 (three full tiles and a partial one)
+    the tiled solve."""
     rng = np.random.default_rng(5)
     J = scipy.sparse.random(400, 150, density=0.08, random_state=7, format="csr") + \
         scipy.sparse.vstack((scipy.sparse.eye(150), scipy.sparse.csr_matrix((250, 150))))
     F = mrcal_b200.CHOLMOD_factorization(J)
     JtJ = (J.T @ J).toarray()
     L = np.linalg.cholesky(JtJ)
-    bt = rng.normal(size=(7, 150))
+    for bt in (rng.normal(size=(7, 150)), rng.normal(size=(100, 150))):
+        _check_solve_systems(F, JtJ, L, bt)
+
+
+def _check_solve_systems(F, JtJ, L, bt):
     tol = dict(rtol=0, atol=1e-9 * np.abs(bt).max())
     xA = F.solve_xt_JtJ_bt(bt)
     assert np.allclose(xA, np.linalg.solve(JtJ, bt.T).T, **tol)
@@ -111,7 +122,8 @@ def test_solve_systems():
     ("LENSMODEL_SPLINED_STEREOGRAPHIC_order=3_Nx=11_Ny=8_fov_x_deg=150", 3, 0),   # most knots uncoupled: the L_I part
     ("LENSMODEL_OPENCV8", 3, 9),                                                  # point groups next to frame groups
 ])
-def test_structured_factorization_of_a_problem(lensmodel, Ncameras, Npoints):
+@pytest.mark.parametrize("nrhs", [5, 100])   # the per-block and the tiled solve of L_S (100: a partial tile)
+def test_structured_factorization_of_a_problem(lensmodel, Ncameras, Npoints, nrhs):
     """optimizer_callback()'s factorization is built from the problem's structure (factorization_schur.cu); it must
     agree with the dense factorization of the same J for every system, up to its own (documented) permutation."""
     from mrcal_b200 import synthetic
@@ -122,7 +134,7 @@ def test_structured_factorization_of_a_problem(lensmodel, Ncameras, Npoints):
     Fd = mrcal_b200.CHOLMOD_factorization(J)          # dense, P = I
     JtJ = (J.T @ J).toarray()
     rng = np.random.default_rng(0)
-    bt = rng.normal(size=(5, J.shape[1]))
+    bt = rng.normal(size=(nrhs, J.shape[1]))
     # Two correct factorizations of the same matrix agree to eps*cond(JtJ), not better -- and these problems are not
     # well conditioned (barely-observed knots held by the regularization alone): forward gates scale with the
     # condition number, and every solve also passes a backward (residual) gate that does not
