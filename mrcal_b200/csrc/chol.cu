@@ -230,14 +230,16 @@ syrk_dmma_kernel(double* __restrict__ A, int ld, int n, int c0, int c1, int k0, 
 ////////////////////////////////////////////////////////////////////////////////
 // triangular solves, Nrhs right-hand sides stored as rows: B[rhs][n]
 ////////////////////////////////////////////////////////////////////////////////
-// y_k = invL_kk b_k  (transpose=false)  or  invL_kk' b_k (transpose=true); one CTA per rhs
+// y_k = invL_kk b_k  (transpose=false)  or  invL_kk' b_k (transpose=true); one CTA per rhs. Unknowns >= nreal are
+// read as zero: whatever the padding holds (NaN included) never reaches a real unknown, and the padding unknowns of
+// the solution come out zero in the backward direction
 __global__ void __launch_bounds__(64)
-solve_diag_kernel(const double* __restrict__ invL, double* __restrict__ B, int ldb, int k0, bool transpose)
+solve_diag_kernel(const double* __restrict__ invL, double* __restrict__ B, int ldb, int k0, int nreal, bool transpose)
 {
     __shared__ double b[NB];
     double* v = B + (size_t)blockIdx.x * ldb + k0;
     const int i = threadIdx.x;
-    b[i] = v[i];
+    b[i] = k0 + i < nreal ? v[i] : 0.;
     __syncthreads();
     double acc = 0.;
     if(!transpose) { for(int m = 0; m <= i; m++) acc += invL[i * NB + m] * b[m]; }
@@ -434,8 +436,8 @@ static bool syrk_update(double* A, int ld, int n, int c0, int c1, int k0, int k1
 // The multi-kernel factorization is ~3 short kernels per 64-column block, a solve 2 per block and direction, all with
 // launch-time-constant arguments: replaying a captured CUDA graph takes the host out of the loop (the host would
 // otherwise bound the rate at which the chain of tiny kernels is issued).
-// m: nreal (factorization) or ldb (solve); kind: 0 the factorization, else the solve's parts
-struct GraphKey { const void* a; const void* b; int npad, m, kind; };
+// m: ldb (solve; unused by the factorization); kind: 0 the factorization, else the solve's parts
+struct GraphKey { const void* a; const void* b; int npad, nreal, m, kind; };
 struct GraphEntry { GraphKey key; cudaGraphExec_t exec; int launches; unsigned long stamp; };
 static std::vector<GraphEntry> g_graphs;
 static unsigned long g_stamp = 0;
@@ -444,7 +446,8 @@ template <typename F>
 static bool run_graphed(const GraphKey& key, cudaStream_t s, int* nlaunch, F enqueue)
 {
     for(auto& e : g_graphs)
-        if(e.key.a == key.a && e.key.b == key.b && e.key.npad == key.npad && e.key.m == key.m && e.key.kind == key.kind)
+        if(e.key.a == key.a && e.key.b == key.b && e.key.npad == key.npad && e.key.nreal == key.nreal && e.key.m == key.m &&
+           e.key.kind == key.kind)
         {
             e.stamp = ++g_stamp;
             MB200_CUDA_CHECK(cudaGraphLaunch(e.exec, s));
@@ -488,7 +491,7 @@ void chol_forget_graphs(const void* A)
 bool chol_factor_blocked(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch)
 {
     if(!configure_kernels()) return false;
-    return run_graphed(GraphKey{A, d_info, npad, nreal, 0}, s, nlaunch, [&](int* n)
+    return run_graphed(GraphKey{A, d_info, npad, nreal, 0, 0}, s, nlaunch, [&](int* n)
     {
         MB200_CUDA_CHECK(cudaMemsetAsync(d_info, 0, sizeof(int), s));
         for(int K0 = 0; K0 < npad; K0 += NBO)
@@ -515,13 +518,14 @@ bool chol_factor_blocked(double* A, int npad, int nreal, double* invL, int* d_in
     });
 }
 
-static bool chol_solve_enqueue(const double* L, int npad, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s, int* nlaunch, int parts)
+static bool chol_solve_enqueue(const double* L, int npad, int nreal, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s,
+                               int* nlaunch, int parts)
 {
     const int nblk = npad / NB;
     for(int k = 0; k < nblk && (parts & 1); k++)
     {
         const int k0 = k * NB;
-        solve_diag_kernel<<<nrhs, NB, 0, s>>>(invL + (size_t)k * NB * NB, B, ldb, k0, false);
+        solve_diag_kernel<<<nrhs, NB, 0, s>>>(invL + (size_t)k * NB * NB, B, ldb, k0, nreal, false);
         if(nlaunch) (*nlaunch)++;
         const int below = npad - k0 - NB;
         if(below > 0)
@@ -533,7 +537,7 @@ static bool chol_solve_enqueue(const double* L, int npad, const double* invL, do
     for(int k = nblk - 1; k >= 0 && (parts & 2); k--)
     {
         const int k0 = k * NB;
-        solve_diag_kernel<<<nrhs, NB, 0, s>>>(invL + (size_t)k * NB * NB, B, ldb, k0, true);
+        solve_diag_kernel<<<nrhs, NB, 0, s>>>(invL + (size_t)k * NB * NB, B, ldb, k0, nreal, true);
         if(nlaunch) (*nlaunch)++;
         if(k0 > 0)
         {
@@ -552,9 +556,9 @@ static bool chol_solve_enqueue(const double* L, int npad, const double* invL, do
 constexpr int kTiledSolveRhsPerBlock = 8;
 
 bool chol_solve(const double* L, int npad, int nreal, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s,
-                int* nlaunch, int parts)
+                int* nlaunch, int parts, int kernels)
 {
-    if(nrhs >= kTiledSolveRhsPerBlock * (npad / NB))
+    if(kernels == 2 || (kernels == 0 && nrhs >= kTiledSolveRhsPerBlock * (npad / NB)))
     {
         if(!configure_kernels()) return false;
         const unsigned tiles = (unsigned)((nrhs + kSolveTile - 1) / kSolveTile);
@@ -564,9 +568,48 @@ bool chol_solve(const double* L, int npad, int nreal, const double* invL, double
         MB200_CUDA_CHECK(cudaGetLastError());
         return true;
     }
-    if(nrhs != 1) return chol_solve_enqueue(L, npad, invL, B, ldb, nrhs, s, nlaunch, parts);
-    return run_graphed(GraphKey{L, B, npad, ldb, parts}, s, nlaunch,
-                       [&](int* n) { return chol_solve_enqueue(L, npad, invL, B, ldb, 1, s, n, parts); });
+    if(nrhs != 1) return chol_solve_enqueue(L, npad, nreal, invL, B, ldb, nrhs, s, nlaunch, parts);
+    return run_graphed(GraphKey{L, B, npad, nreal, ldb, parts}, s, nlaunch,
+                       [&](int* n) { return chol_solve_enqueue(L, npad, nreal, invL, B, ldb, 1, s, n, parts); });
+}
+
+// Test aid (not on any product path): solve with a host factor (L: npad x npad, invL: npad/64 blocks of 64 x 64) for
+// nrhs host right-hand sides B[r][0..npad), in place. kernel: 0 chol_solve()'s own choice, 1 its per-block kernels,
+// 2 its tiled kernel, 3 chol_solve_backward() (nrhs = 1, parts = 2: the whole padded system)
+bool chol_debug_solve(const double* L, const double* invL, int npad, int nreal, double* B, int nrhs, int parts, int kernel)
+{
+    if(npad <= 0 || npad % NB != 0 || nreal < 0 || nreal > npad || nrhs <= 0 || parts < 1 || parts > 3 || kernel < 0 ||
+       kernel > 3 || (kernel == 3 && (nrhs != 1 || parts != 2)))
+    {
+        set_error("chol_debug_solve: bad arguments (npad %d, nreal %d, nrhs %d, parts %d, kernel %d)", npad, nreal, nrhs, parts, kernel);
+        return false;
+    }
+    double *dL = nullptr, *dinv = nullptr, *dB = nullptr; int* info = nullptr;
+    cudaStream_t s = nullptr;
+    CholScratch sc;
+    int h_info = 0;
+    bool ok = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaMalloc(&dL, (size_t)npad * npad * sizeof(double)) == cudaSuccess &&
+              cudaMalloc(&dinv, (size_t)npad * NB * sizeof(double)) == cudaSuccess &&
+              cudaMalloc(&dB, (size_t)nrhs * npad * sizeof(double)) == cudaSuccess && cudaMalloc(&info, sizeof(int)) == cudaSuccess &&
+              cudaMemcpyAsync(dL, L, (size_t)npad * npad * sizeof(double), cudaMemcpyHostToDevice, s) == cudaSuccess &&
+              cudaMemcpyAsync(dinv, invL, (size_t)npad * NB * sizeof(double), cudaMemcpyHostToDevice, s) == cudaSuccess &&
+              cudaMemcpyAsync(dB, B, (size_t)nrhs * npad * sizeof(double), cudaMemcpyHostToDevice, s) == cudaSuccess &&
+              cudaMemsetAsync(info, 0, sizeof(int), s) == cudaSuccess;
+    if(ok && kernel == 3)
+        ok = chol_scratch_create(&sc, npad) && chol_solve_backward(dL, npad, dinv, dB, info, s, nullptr, &sc);
+    else if(ok)
+        ok = chol_solve(dL, npad, nreal, dinv, dB, npad, nrhs, s, nullptr, parts, kernel);
+    ok = ok && cudaMemcpyAsync(B, dB, (size_t)nrhs * npad * sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaMemcpyAsync(&h_info, info, sizeof(int), cudaMemcpyDeviceToHost, s) == cudaSuccess && cudaStreamSynchronize(s) == cudaSuccess;
+    if(!ok) set_error("chol_debug_solve failed: %s", cudaGetErrorString(cudaGetLastError()));
+    else if(h_info != 0) { set_error("chol_debug_solve: the backward substitution reported %d", h_info); ok = false; }
+    if(s) cudaStreamSynchronize(s);
+    chol_forget_graphs(dL);   // one right-hand side: a graph keyed on dL and dB
+    chol_scratch_destroy(&sc);
+    cudaFree(dL); cudaFree(dinv); cudaFree(dB); cudaFree(info);
+    if(s) cudaStreamDestroy(s);
+    return ok;
 }
 
 __global__ void debug_fill_spd_kernel(double* A, int n)

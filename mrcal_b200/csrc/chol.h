@@ -54,15 +54,19 @@ constexpr int kSolveTile = 32, kSolveTileLd = 68;
 constexpr size_t kSolveTileSmem = (size_t)(kSolveTile + kCholBlock) * kSolveTileLd * sizeof(double);
 
 // chol.cu: solve L L' X = B in place for nrhs right-hand sides stored as rows B[r][0..npad); unknowns >= nreal are
-// padding. parts: 1 = only L Y = B, 2 = only L' X = B, 3 = both. The kernels are chosen by nrhs
+// padding, read as zero whatever B holds there. parts: 1 = only L Y = B, 2 = only L' X = B, 3 = both. The kernels are
+// chosen by nrhs; kernels (tests only): 1 forces the per-block kernels, 2 the tiled one
 bool chol_solve(const double* L, int npad, int nreal, const double* invL, double* B, int ldb, int nrhs, cudaStream_t s,
-                int* nlaunch, int parts = 3);
+                int* nlaunch, int parts = 3, int kernels = 0);
 
 // drop cached CUDA graphs that reference this buffer (call before freeing it)
 void chol_forget_graphs(const void* A);
 
 double chol_debug_time(int n, int reps, int what);
 bool chol_debug_potrf_stamps(long long* out64);
+// test aids: chol_dataflow.cu, chol.cu
+bool chol_debug_factor(const double* A0, int n, int nreal, int path, double* L_out, double* invL_out, int* info_out, int* grid_out);
+bool chol_debug_solve(const double* L, const double* invL, int npad, int nreal, double* B, int nrhs, int parts, int kernel);
 
 // d_out2[0] = min, d_out2[1] = max of diag(L)[0..nreal)
 bool chol_diag_minmax(const double* L, int npad, int nreal, double* d_out2, cudaStream_t s);

@@ -17,6 +17,7 @@
 // mrcal.c:6435); the reference has no counterpart of this structure.
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <vector>
 
 #include "chol.h"
 #include "potrf_block.cuh"
@@ -499,6 +500,33 @@ bool scratch_fits(const CholScratch* sc, int npad)
 }
 
 long long* g_debug_stamps = nullptr;   // set by chol_debug_spine_stamps() only
+int* g_debug_grid = nullptr;           // set by chol_debug_factor() only: the spine kernel's grid goes there
+
+// the persistent factorization (chol_factor up to npad = 8192)
+bool chol_factor_spine(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch,
+                       CholScratch* scratch, const int* d_run_if)
+{
+    const int num_sms = configure();
+    if(num_sms == 0) return false;
+    int nb = npad / T, ld = npad;
+    const int ntiles = nb * (nb + 1) / 2;
+    int* abort_flag = scratch->flags;
+    int* flags = abort_flag + 1;
+    int* pre = flags + ntiles;
+    WordFill clear;
+    clear.add(d_info, sizeof(int));
+    clear.add(abort_flag, (size_t)(1 + ntiles + nb) * sizeof(int));
+    if(!fill_words(clear, s)) return false;
+    long long* stamps = g_debug_stamps;
+    void* args[] = {&A, &ld, &nb, &nreal, &invL, &d_info, &flags, &pre, &abort_flag, &d_run_if, &stamps};
+    // the spine CTA and up to one helper CTA per helper task (see the kernel; none for nb <= 2) on the other SMs
+    const int nhelper_tasks = nb >= 3 ? (nb - 1) * nb / 2 - 1 : 0;
+    const int grid = 1 + (nhelper_tasks < num_sms - 1 ? nhelper_tasks : num_sms - 1);
+    MB200_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)chol_spine_kernel, dim3(grid), dim3(256), args, sizeof(DfSmem), s));
+    if(nlaunch) (*nlaunch)++;
+    if(g_debug_grid) *g_debug_grid = grid;
+    return true;
+}
 
 }  // namespace
 
@@ -533,25 +561,7 @@ bool chol_factor(double* A, int npad, int nreal, double* invL, int* d_info, cuda
     // against 187 ms at n = 19376 (DESIGN section 9). It ignores d_run_if: a factorization nobody asked for costs
     // time, not correctness
     if(npad > 8192) return chol_factor_blocked(A, npad, nreal, invL, d_info, s, nlaunch);
-    const int num_sms = configure();
-    if(num_sms == 0) return false;
-    int nb = npad / T, ld = npad;
-    const int ntiles = nb * (nb + 1) / 2;
-    int* abort_flag = scratch->flags;
-    int* flags = abort_flag + 1;
-    int* pre = flags + ntiles;
-    WordFill clear;
-    clear.add(d_info, sizeof(int));
-    clear.add(abort_flag, (size_t)(1 + ntiles + nb) * sizeof(int));
-    if(!fill_words(clear, s)) return false;
-    long long* stamps = g_debug_stamps;
-    void* args[] = {&A, &ld, &nb, &nreal, &invL, &d_info, &flags, &pre, &abort_flag, &d_run_if, &stamps};
-    // the spine CTA and up to one helper CTA per helper task (see the kernel; none for nb <= 2) on the other SMs
-    const int nhelper_tasks = nb >= 3 ? (nb - 1) * nb / 2 - 1 : 0;
-    const int grid = 1 + (nhelper_tasks < num_sms - 1 ? nhelper_tasks : num_sms - 1);
-    MB200_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)chol_spine_kernel, dim3(grid), dim3(256), args, sizeof(DfSmem), s));
-    if(nlaunch) (*nlaunch)++;
-    return true;
+    return chol_factor_spine(A, npad, nreal, invL, d_info, s, nlaunch, scratch, d_run_if);
 }
 
 bool chol_solve_backward(const double* L, int npad, const double* invL, double* B, int* d_info, cudaStream_t s, int* nlaunch,
@@ -603,6 +613,58 @@ bool chol_debug_spine_stamps(int n, long long* out, int nmax)
     chol_scratch_destroy(&sc);
     cudaFree(A); cudaFree(invL); cudaFree(info); cudaFree(st);
     cudaStreamDestroy(s);
+    return ok;
+}
+
+// Test aid (not on any product path): factor the lower triangle of the host n x n matrix A0 (row-major), padded to
+// npad = chol_padded(n) with 1 on the padding diagonal; pivots >= nreal are not reported. path: 0 what chol_factor
+// picks, 1 the spine kernel (npad <= 8192), 2 chol_factor_blocked. Out: L_out (npad x npad, the whole buffer),
+// invL_out (npad/64 blocks of 64 x 64), *info_out, grid_out[4] = {path that ran, CTAs of the spine kernel's cooperative
+// launch (0: not launched), SMs of the device, helper tasks of the spine kernel}
+bool chol_debug_factor(const double* A0, int n, int nreal, int path, double* L_out, double* invL_out, int* info_out, int* grid_out)
+{
+    const int npad = chol_padded(n), nb = npad / T;
+    if(n <= 0 || nreal < 0 || nreal > n || path < 0 || path > 2 || (path == 1 && npad > 8192))
+    {
+        set_error("chol_debug_factor: bad arguments (n %d, nreal %d, path %d)", n, nreal, path);
+        return false;
+    }
+    const int sms = configure();
+    if(sms == 0) return false;
+    std::vector<double> h((size_t)npad * npad, 0.);
+    for(int i = 0; i < npad; i++)
+        for(int j = 0; j <= i; j++) h[(size_t)i * npad + j] = i < n ? A0[(size_t)i * n + j] : (i == j ? 1. : 0.);
+    double *A = nullptr, *invL = nullptr; int* info = nullptr;
+    cudaStream_t s = nullptr;
+    CholScratch sc;
+    int grid = 0;
+    bool ok = cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) == cudaSuccess &&
+              cudaMalloc(&A, (size_t)npad * npad * sizeof(double)) == cudaSuccess &&
+              cudaMalloc(&invL, (size_t)npad * T * sizeof(double)) == cudaSuccess && cudaMalloc(&info, sizeof(int)) == cudaSuccess &&
+              chol_scratch_create(&sc, npad) &&
+              cudaMemcpyAsync(A, h.data(), h.size() * sizeof(double), cudaMemcpyHostToDevice, s) == cudaSuccess &&
+              cudaMemsetAsync(invL, 0xff, (size_t)npad * T * sizeof(double), s) == cudaSuccess;   // NaN: every entry must be written
+    if(ok)
+    {
+        g_debug_grid = &grid;
+        ok = path == 0 ? chol_factor(A, npad, nreal, invL, info, s, nullptr, &sc)
+           : path == 1 ? chol_factor_spine(A, npad, nreal, invL, info, s, nullptr, &sc, nullptr)
+                       : chol_factor_blocked(A, npad, nreal, invL, info, s, nullptr);
+        g_debug_grid = nullptr;
+    }
+    ok = ok && cudaMemcpyAsync(L_out, A, (size_t)npad * npad * sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaMemcpyAsync(invL_out, invL, (size_t)npad * T * sizeof(double), cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+         cudaMemcpyAsync(info_out, info, sizeof(int), cudaMemcpyDeviceToHost, s) == cudaSuccess && cudaStreamSynchronize(s) == cudaSuccess;
+    if(!ok) set_error("chol_debug_factor failed: %s", cudaGetErrorString(cudaGetLastError()));
+    grid_out[0] = grid > 0 ? 1 : 2;
+    grid_out[1] = grid;
+    grid_out[2] = sms;
+    grid_out[3] = nb >= 3 ? (nb - 1) * nb / 2 - 1 : 0;
+    if(s) cudaStreamSynchronize(s);
+    chol_forget_graphs(A);   // the blocked path caches a graph keyed on A
+    chol_scratch_destroy(&sc);
+    cudaFree(A); cudaFree(invL); cudaFree(info);
+    if(s) cudaStreamDestroy(s);
     return ok;
 }
 

@@ -177,3 +177,14 @@ extern "C" bool mrcal_b200_debug_potrf_stamps(long long* out64)
 {
     return chol_debug_potrf_stamps(out64);
 }
+// Test entry points of the dense Cholesky kernels (tests/test_cholesky_gpu.py); not declared in the public header
+extern "C" bool mrcal_b200_debug_cholesky(const double* A, int n, int nreal, int path, double* L_out, double* invL_out,
+                                          int* info_out, int* grid_out)
+{
+    return chol_debug_factor(A, n, nreal, path, L_out, invL_out, info_out, grid_out);
+}
+extern "C" bool mrcal_b200_debug_chol_solve(const double* L, const double* invL, int npad, int nreal, double* B, int nrhs,
+                                            int parts, int kernel)
+{
+    return chol_debug_solve(L, invL, npad, nreal, B, nrhs, parts, kernel);
+}

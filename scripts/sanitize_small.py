@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """A small end-to-end exercise of every kernel family, meant to be run under compute-sanitizer
 (memcheck / racecheck / synccheck): callback, solve (persistent Cholesky, potrf_block, Schur, assembly),
-factorization object, project/unproject, triangulated points."""
+factorization object, the dense Cholesky kernels on their own, project/unproject, triangulated points."""
 import sys
 sys.path.insert(0, ".")
 sys.path.insert(0, "tests")
@@ -25,6 +25,18 @@ P = mrcal_b200.Problem(**kw)
 print("solve", P.optimize(max_iterations=6)["Niterations"])
 for icam in (-1, 1):
     print("drt_cross_reprojection__dbpacked", icam, np.abs(mrcal_b200.drt_cross_reprojection__dbpacked(icam_intrinsics=icam, **kw)).max())
+# the dense Cholesky kernels directly (tests/test_cholesky_gpu.py's entry points): the spine kernel at 1 to 4 blocks
+# (its helper CTAs and pre tasks from 3 on, potrf_block's named barriers in every step), the blocked factorization,
+# and the solves of chol_solve() (both kernel families) and chol_solve_backward()
+import chol_np
+import test_cholesky_gpu as tc
+for n, path in ((64, 1), (128, 1), (192, 1), (250, 1), (250, 2)):
+    f = tc.factor(chol_np.spd_cond(n, 1e2, np.random.default_rng(n)), path)
+    B = np.random.default_rng(0).normal(size=(3, f.L.shape[0]))
+    for kernel in (1, 2):
+        tc.solve(f.L, f.invL, n, B, 3, kernel)
+    tc.solve(f.L, f.invL, n, B[:1], 2, 3)
+    print("cholesky", n, "path", f.path, "grid", f.grid, "info", f.info)
 intr = synthetic.true_intrinsics("LENSMODEL_OPENCV8", 1, np.random.default_rng(0))[0]
 q = mrcal_b200.project(np.array(((0.1, 0.2, 2.), (-.3, .1, 3.))), "LENSMODEL_OPENCV8", intr)
 print("unproject", mrcal_b200.unproject(q, "LENSMODEL_OPENCV8", intr))
