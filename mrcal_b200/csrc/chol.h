@@ -36,14 +36,14 @@ void chol_scratch_destroy(CholScratch* sc);
 // are padding (1 on the diagonal). On return the lower triangle holds L.
 // invL: [npad/64][64*64] inverses of the diagonal blocks of L.
 // d_info: device int; 0 if positive definite, else 1 + index of the first bad pivot.
-// scratch: the caller's, for at least npad. d_run_if: device flag; 0 there = do nothing (nullptr: always run)
+// scratch: the caller's, for at least npad
 bool chol_factor(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch,
-                 CholScratch* scratch, const int* d_run_if = nullptr);
+                 CholScratch* scratch);
 
 // Only the backward half, L' Z = B in place, one right-hand side B[0..npad). d_info (may be the factorization's): set
 // to -9 if the persistent kernel gave up waiting (never expected; the alternative would be to hang the GPU)
 bool chol_solve_backward(const double* L, int npad, const double* invL, double* B, int* d_info, cudaStream_t s, int* nlaunch,
-                         CholScratch* scratch, const int* d_run_if = nullptr);
+                         CholScratch* scratch);
 
 // chol.cu: the multi-kernel factorization, which chol_factor runs above npad = 8192 (same arguments; no scratch)
 bool chol_factor_blocked(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch);

@@ -234,11 +234,10 @@ __device__ __forceinline__ void tile_to_global(double* __restrict__ dst, size_t 
 // (registers capped -- no spills at 160 -- so that the small kernels of the Cauchy side fit next to a CTA of this one)
 __global__ void __maxnreg__(160)
 chol_spine_kernel(double* __restrict__ A, int ld, int nb, int nreal, double* __restrict__ invL, int* __restrict__ info,
-                  int* __restrict__ flags, int* __restrict__ pre, int* __restrict__ abort_flag, const int* __restrict__ run_if,
+                  int* __restrict__ flags, int* __restrict__ pre, int* __restrict__ abort_flag,
                   long long* __restrict__ stamps /* debugging aid: 8 clock64() values per spine step, or NULL */)
 {
 #define SPINE_STAMP(k) do { if(stamps != nullptr && tid == 0) stamps[8 * d + (k)] = clock64(); } while(0)
-    if(run_if != nullptr && *run_if == 0) return;
     extern __shared__ __align__(16) unsigned char dsm_raw[];
     DfSmem& sm = *reinterpret_cast<DfSmem*>(dsm_raw);
     const int tid = threadIdx.x;
@@ -400,10 +399,8 @@ chol_spine_kernel(double* __restrict__ A, int ld, int nb, int nreal, double* __r
 // the wait.
 __global__ void __launch_bounds__(256, 1)
 chol_backward_dataflow_kernel(const double* __restrict__ L, int ld, int nb, const double* __restrict__ invL,
-                              double* __restrict__ B, double* __restrict__ xbuf, int* __restrict__ abort_flag, int* __restrict__ info,
-                              const int* __restrict__ run_if)
+                              double* __restrict__ B, double* __restrict__ xbuf, int* __restrict__ abort_flag, int* __restrict__ info)
 {
-    if(run_if != nullptr && *run_if == 0) return;
     __shared__ double xs[T];
     __shared__ double red[4][T];
     __shared__ double tv[T];
@@ -504,7 +501,7 @@ int* g_debug_grid = nullptr;           // set by chol_debug_factor() only: the s
 
 // the persistent factorization (chol_factor up to npad = 8192)
 bool chol_factor_spine(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch,
-                       CholScratch* scratch, const int* d_run_if)
+                       CholScratch* scratch)
 {
     const int num_sms = configure();
     if(num_sms == 0) return false;
@@ -518,7 +515,7 @@ bool chol_factor_spine(double* A, int npad, int nreal, double* invL, int* d_info
     clear.add(abort_flag, (size_t)(1 + ntiles + nb) * sizeof(int));
     if(!fill_words(clear, s)) return false;
     long long* stamps = g_debug_stamps;
-    void* args[] = {&A, &ld, &nb, &nreal, &invL, &d_info, &flags, &pre, &abort_flag, &d_run_if, &stamps};
+    void* args[] = {&A, &ld, &nb, &nreal, &invL, &d_info, &flags, &pre, &abort_flag, &stamps};
     // the spine CTA and up to one helper CTA per helper task (see the kernel; none for nb <= 2) on the other SMs
     const int nhelper_tasks = nb >= 3 ? (nb - 1) * nb / 2 - 1 : 0;
     const int grid = 1 + (nhelper_tasks < num_sms - 1 ? nhelper_tasks : num_sms - 1);
@@ -554,18 +551,17 @@ void chol_scratch_destroy(CholScratch* sc)
 }
 
 bool chol_factor(double* A, int npad, int nreal, double* invL, int* d_info, cudaStream_t s, int* nlaunch,
-                 CholScratch* scratch, const int* d_run_if)
+                 CholScratch* scratch)
 {
     if(!scratch_fits(scratch, npad)) return false;
     // Above 8192 unknowns the multi-kernel factorization (chol.cu) is faster: 39 against 43 ms at n = 12000, 159
-    // against 187 ms at n = 19376 (DESIGN section 9). It ignores d_run_if: a factorization nobody asked for costs
-    // time, not correctness
+    // against 187 ms at n = 19376 (DESIGN section 9)
     if(npad > 8192) return chol_factor_blocked(A, npad, nreal, invL, d_info, s, nlaunch);
-    return chol_factor_spine(A, npad, nreal, invL, d_info, s, nlaunch, scratch, d_run_if);
+    return chol_factor_spine(A, npad, nreal, invL, d_info, s, nlaunch, scratch);
 }
 
 bool chol_solve_backward(const double* L, int npad, const double* invL, double* B, int* d_info, cudaStream_t s, int* nlaunch,
-                         CholScratch* scratch, const int* d_run_if)
+                         CholScratch* scratch)
 {
     const int num_sms = configure();
     if(num_sms == 0 || !scratch_fits(scratch, npad)) return false;
@@ -576,7 +572,7 @@ bool chol_solve_backward(const double* L, int npad, const double* invL, double* 
     clear.add(abort_flag, sizeof(int));
     if(!fill_words(clear, s)) return false;
     double* xbuf = scratch->xbuf;
-    void* args[] = {&L, &ld, &nb, &invL, &B, &xbuf, &abort_flag, &d_info, &d_run_if};
+    void* args[] = {&L, &ld, &nb, &invL, &B, &xbuf, &abort_flag, &d_info};
     const int grid = nb < num_sms ? nb : num_sms;
     MB200_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)chol_backward_dataflow_kernel, dim3(grid), dim3(256), args, 0, s));
     if(nlaunch) (*nlaunch)++;
@@ -648,7 +644,7 @@ bool chol_debug_factor(const double* A0, int n, int nreal, int path, double* L_o
     {
         g_debug_grid = &grid;
         ok = path == 0 ? chol_factor(A, npad, nreal, invL, info, s, nullptr, &sc)
-           : path == 1 ? chol_factor_spine(A, npad, nreal, invL, info, s, nullptr, &sc, nullptr)
+           : path == 1 ? chol_factor_spine(A, npad, nreal, invL, info, s, nullptr, &sc)
                        : chol_factor_blocked(A, npad, nreal, invL, info, s, nullptr);
         g_debug_grid = nullptr;
     }

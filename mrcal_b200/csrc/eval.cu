@@ -542,9 +542,7 @@ eval_regularization_kernel(DevProblem P, bool splined, double* __restrict__ x, d
 {
     __shared__ double red[32];
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    const int Ndist_rows   = (P.reg && P.opt_dist) ? P.Ncam_i * (P.Nintr - 4) : 0;
-    const int Ncenter_rows = (P.reg && P.opt_core) ? P.Ncam_i * 2 : 0;
-    const int Nunity_rows  = P.reg_unity ? 1 : 0;
+    const int Ndist_rows = P.Nreg_dist, Ncenter_rows = P.Nreg_center, Nunity_rows = P.Nreg_unity;
     const double nominal_pixel_error = 0.1;
     double err = 0.;
     if(t < Ndist_rows)
@@ -554,7 +552,7 @@ eval_regularization_kernel(DevProblem P, bool splined, double* __restrict__ x, d
         {
             // per knot: a radial row then a (10x heavier) tangential row (:5709-5786)
             const double scale = nominal_pixel_error / 10.0;
-            const int per_cam = P.Nintr - 4;
+            const int per_cam = P.Ndist_state;
             const int cam = t / per_cam, r = t - cam * per_cam;
             const int knot = r >> 1, which = r & 1;
             const int iy = knot / P.Nx, ix = knot - iy * P.Nx;
@@ -575,7 +573,7 @@ eval_regularization_kernel(DevProblem P, bool splined, double* __restrict__ x, d
             x[m] = err;
             if constexpr(WITH_J)
             {
-                const size_t j = (size_t)P.reg_j0 + 2 * (size_t)t;
+                const size_t j = reg_row_j0(P, true, t);
                 Jcol[j] = col;     Jval[j]     = g0 * kScaleDistortion;
                 Jcol[j + 1] = col + 1; Jval[j + 1] = g1 * kScaleDistortion;
             }
@@ -584,14 +582,14 @@ eval_regularization_kernel(DevProblem P, bool splined, double* __restrict__ x, d
         {
             // L2 on each distortion; the rational denominator terms of OPENCV8+ 5x heavier (:5787-5850)
             const double scale = nominal_pixel_error / 1.0;
-            const int per_cam = P.Nintr - 4;
+            const int per_cam = P.Ndist_state;
             const int cam = t / per_cam, j = t - cam * per_cam;
             const double scale_here = (P.opencv8plus && 5 <= j && j <= 7) ? scale * 5. : scale;
             err = scale_here * P.u_intr[(size_t)cam * P.Nintr + 4 + j];
             x[m] = err;
             if constexpr(WITH_J)
             {
-                const size_t jj = (size_t)P.reg_j0 + t;
+                const size_t jj = reg_row_j0(P, false, t);
                 Jcol[jj] = P.i_intr0 + cam * P.Nintr_state + P.Ncore_state + j;
                 Jval[jj] = scale_here * kScaleDistortion;
             }
@@ -609,7 +607,7 @@ eval_regularization_kernel(DevProblem P, bool splined, double* __restrict__ x, d
         x[P.m_reg0 + t] = err;
         if constexpr(WITH_J)
         {
-            const size_t jj = (size_t)P.reg_j0 + (size_t)(splined ? 2 : 1) * Ndist_rows + r;
+            const size_t jj = reg_row_j0(P, splined, t);
             Jcol[jj] = P.i_intr0 + cam * P.Nintr_state + 2 + k;
             Jval[jj] = scale * kScaleCenter;
         }
@@ -623,7 +621,7 @@ eval_regularization_kernel(DevProblem P, bool splined, double* __restrict__ x, d
         x[P.m_reg0 + t] = err;
         if constexpr(WITH_J)
         {
-            const size_t jj = (size_t)P.reg_j0 + (size_t)(splined ? 2 : 1) * Ndist_rows + Ncenter_rows;
+            const size_t jj = reg_row_j0(P, splined, t);
             for(int i = 0; i < 3; i++)
             {
                 Jcol[jj + i] = P.i_extr0 + 3 + i;
@@ -764,15 +762,7 @@ __global__ void fill_rowptr_kernel(DevProblem P, bool splined, int nnz_total, in
     else if(m < P.m_reg0)
         rowptr[m] = P.tri_j0[m - P.m_tri0];
     else
-    {
-        const int t = m - P.m_reg0;
-        const int Ndist_rows   = (P.reg && P.opt_dist) ? P.Ncam_i * (P.Nintr - 4) : 0;
-        const int Ncenter_rows = (P.reg && P.opt_core) ? P.Ncam_i * 2 : 0;
-        const int wd = splined ? 2 : 1;
-        if(t < Ndist_rows)                      rowptr[m] = P.reg_j0 + wd * t;
-        else if(t < Ndist_rows + Ncenter_rows)  rowptr[m] = P.reg_j0 + wd * Ndist_rows + (t - Ndist_rows);
-        else                                    rowptr[m] = P.reg_j0 + wd * Ndist_rows + Ncenter_rows;
-    }
+        rowptr[m] = reg_row_j0(P, splined, m - P.m_reg0);
 }
 
 template <int KIND>
@@ -790,16 +780,7 @@ static bool launch_kind(const DevProblem& dp, const EvalBuffers& out, bool with_
             int stride = row2;
             while((stride & 3) != 2) stride++;
             const size_t smem = (size_t)threads * stride * sizeof(double) + 16;
-            // cudaFuncSetAttribute is per device: one flag per (device, lens kind)
-            static bool configured[kMaxDevices][LENS_NKINDS] = {};
-            int dev = 0;
-            MB200_CUDA_CHECK(cudaGetDevice(&dev));
-            if(dev < 0 || dev >= kMaxDevices) { set_error("device index %d out of range", dev); return false; }
-            if(!configured[dev][KIND])
-            {
-                MB200_CUDA_CHECK(cudaFuncSetAttribute(eval_boards_kernel<KIND, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-                configured[dev][KIND] = true;
-            }
+            if(!set_max_dynamic_smem<eval_boards_kernel<KIND, true>>(200 * 1024)) return false;
             if(smem > 200 * 1024) { set_error("Jacobian rows of %d entries are too wide for the staging buffer", row2 / 2); return false; }
             eval_boards_kernel<KIND, true ><<<dp.Nobs_board, threads, smem, stream>>>(dp, out.x, out.Jval, out.Jcol, out.norm2);
         }
@@ -878,11 +859,7 @@ bool launch_evaluate(const DevProblem& dp, const EvalBuffers& out, bool with_jac
     }
     if(Jrowptr != nullptr)
     {
-        // nnz_total: after the last regularization entry
-        const int Ndist_rows   = (dp.reg && dp.opt_dist) ? dp.Ncam_i * (dp.Nintr - 4) : 0;
-        const int Ncenter_rows = (dp.reg && dp.opt_core) ? dp.Ncam_i * 2 : 0;
-        const int nnz_total = dp.reg_j0 + (splined ? 2 : 1) * Ndist_rows + Ncenter_rows + (dp.reg_unity ? 3 : 0);
-        fill_rowptr_kernel<<<(dp.Nmeas + 1 + 255) / 256, 256, 0, stream>>>(dp, splined, nnz_total, Jrowptr);
+        fill_rowptr_kernel<<<(dp.Nmeas + 1 + 255) / 256, 256, 0, stream>>>(dp, splined, reg_nnz_total(dp, splined), Jrowptr);
         (*nlaunch)++;
     }
     MB200_CUDA_CHECK(cudaGetLastError());

@@ -17,12 +17,12 @@
 //
 // The object OWNS the device problem it was made from (the one the last mrcal_optimizer_callback() call left in the
 // cache): mrcal_b200_factorization_create_from_last_callback().
+#include "comm.h"
 #include "dmma.cuh"
 #include "solver_internal.h"
 
 namespace mb200 {
 
-bool comm_active();
 mrcal_b200_problem_t* capi_steal_cached_problem();   // capi.cu
 
 namespace {
@@ -50,46 +50,19 @@ __global__ void inactive_blocks_kernel(DevProblem P, NormalBuffers N, const doub
     ia_first[r] = 0;
     if(N.cidx[r] >= 0) return;
     const int c = N.state_index(r);
-    const int n_intr = P.Ncam_i * P.Nintr_state;
-    double H = 0.;
-    if(P.reg && c < n_intr)
+    const UncoupledBlock u = uncoupled_block(P, N.splined, c, Jval, nullptr);
+    if(u.n == 2)
     {
-        const int cam = c / P.Nintr_state, k = c - cam * P.Nintr_state;
-        const int Ndist_rows = P.opt_dist ? P.Ncam_i * (P.Nintr - 4) : 0;
-        if(k >= P.Ncore_state)
-        {
-            const int j = k - P.Ncore_state;
-            if(N.splined)
-            {
-                const int knot = j >> 1, which = j & 1;
-                const int t0 = cam * (P.Nintr - 4) + 2 * knot;
-                const double* e0 = &Jval[(size_t)P.reg_j0 + 2 * (size_t)t0];
-                const double* e1 = e0 + 2;
-                const double Hxx = e0[0] * e0[0] + e1[0] * e1[0], Hyy = e0[1] * e0[1] + e1[1] * e1[1];
-                const double Hxy = e0[0] * e0[1] + e1[0] * e1[1];
-                const double l11 = sqrt(Hxx), l21 = Hxy / l11, d = Hyy - l21 * l21;
-                if(!(Hxx > 0.) || !(d > 0.)) { atomicExch(bad, 1); return; }
-                if(which == 0) { ia_first[r] = 1; ia_L[3 * r] = l11; ia_L[3 * r + 1] = l21; ia_L[3 * r + 2] = sqrt(d); }
-                else           { ia_first[r] = 2; ia_L[3 * r] = l11; ia_L[3 * r + 1] = l21; ia_L[3 * r + 2] = sqrt(d); }
-                return;
-            }
-            const double e = Jval[(size_t)P.reg_j0 + cam * (P.Nintr - 4) + j];
-            H = e * e;
-        }
-        else if(k >= 2)
-        {
-            const double e = Jval[(size_t)P.reg_j0 + (size_t)(N.splined ? 2 : 1) * Ndist_rows + 2 * cam + (k - 2)];
-            H = e * e;
-        }
+        const double l11 = sqrt(u.Hxx), l21 = u.Hxy / l11, d = u.Hyy - l21 * l21;
+        if(!(u.Hxx > 0.) || !(d > 0.)) { atomicExch(bad, 1); return; }
+        ia_first[r] = u.which == 0 ? 1 : 2;
+        ia_L[3 * r] = l11; ia_L[3 * r + 1] = l21; ia_L[3 * r + 2] = sqrt(d);
+        return;
     }
+    const double H = u.Hxx;
     if(!(H > 0.)) { atomicExch(bad, 1); return; }   // an unknown nothing constrains: JtJ is singular
     ia_first[r] = 3;
     ia_L[3 * r] = sqrt(H); ia_L[3 * r + 1] = 0.; ia_L[3 * r + 2] = 0.;
-}
-
-__device__ __forceinline__ int group_col0(const NormalBuffers& N, int grp)
-{
-    return grp < N.Nframe_groups ? 6 * grp : 6 * N.Nframe_groups + 3 * (grp - N.Nframe_groups);
 }
 
 // state-ordered right-hand sides <-> the three pieces of the permuted vector. bt, out: [Nrhs][Nstate]
@@ -173,8 +146,7 @@ panels_forward_tiled_kernel(NormalBuffers N, const double* __restrict__ Bf, int 
             if(q < nb && r0 + r < Nrhs)
             {
                 const int g = gid[q], ne = g < N.Nframe_groups ? 6 : 3;
-                const int col0 = g < N.Nframe_groups ? 6 * g : 6 * N.Nframe_groups + 3 * (g - N.Nframe_groups);
-                if(pp < ne) v = Bf[(size_t)(r0 + r) * Nelim + col0 + pp];
+                if(pp < ne) v = Bf[(size_t)(r0 + r) * Nelim + group_col0(N, g) + pp];
             }
             sA[r][kk] = v;
         }

@@ -19,7 +19,7 @@
 //      two dense products Dk'[Dk | Gx Gy ex ey] on the fp64 tensor pipe (DMMA 8x8x4) -- a quarter of the flops of
 //      the Gram matrix over the full row width that normal.cu's kernel computes from the stored Jacobian
 //   3. geometry x geometry (14 x 14) and J'x over the geometry: plain FMAs
-//   4. the blocks go out in the layout normal_det.cu consumes: A in the compact layout (normal.h, kCompactSlot: fx^2,
+//   4. the blocks go out in the layout normal_schur.cu consumes: A in the compact layout (normal.h, kCompactSlot: fx^2,
 //      fy^2, M = Dk'Dk once, the geometry rows, -J'x once), and B, D, gf
 //
 // Replaces, for this path: the board loop of optimizer_callback() (mrcal.c:4604-4900), libdogleg's Jt*x and what
@@ -485,16 +485,7 @@ sum_partials_to_kernel(const double* __restrict__ part, int n, double* __restric
 // N.active / N.stat for this evaluation and has unpacked the state (launch_unpack_state)
 bool launch_fused_boards(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& out, double* norm_part, cudaStream_t s, int* nlaunch)
 {
-    static bool configured[kMaxDevices] = {};
-    int dev = 0;
-    MB200_CUDA_CHECK(cudaGetDevice(&dev));
-    if(dev < 0 || dev >= kMaxDevices) { set_error("device index %d out of range", dev); return false; }
-    if(!configured[dev])
-    {
-        MB200_CUDA_CHECK(cudaFuncSetAttribute(fused_boards_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
-        MB200_CUDA_CHECK(cudaFuncSetAttribute(fused_boards_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
-        configured[dev] = true;
-    }
+    if(!set_max_dynamic_smem<fused_boards_kernel<4>>(110 * 1024) || !set_max_dynamic_smem<fused_boards_kernel<3>>(110 * 1024)) return false;
     const int NWH = dp.W * dp.H;
     if(NWH > 128) { set_error("internal error: the fused path needs W*H <= 128"); return false; }
     const int K = (NWH + 3) & ~3;

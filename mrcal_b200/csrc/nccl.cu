@@ -6,6 +6,7 @@
 // (torch.distributed in mrcal_b200/distributed.py).
 #include <dlfcn.h>
 
+#include "comm.h"
 #include "problem_impl.h"
 
 namespace mb200 {

@@ -1,29 +1,22 @@
-// Kernel family 2a: the normal equations. From the Jacobian strips written by
-// eval.cu, form JtJ in its block-diagonal + arrowhead structure, eliminate the
-// per-frame (6x6) and per-point (3x3) blocks (Schur complement), and leave the
-// small dense reduced system S, g' of the shared unknowns (all intrinsics, all
-// extrinsics, the board warp) for chol.cu:
+// The normal equations, first half: from the rows of the evaluation at an operating point, the per-item blocks that
+// normal_schur.cu sums into the small dense reduced system S, g' of the shared unknowns (all intrinsics, all
+// extrinsics, the board warp) for chol*.cu:
 //
 //     [ A  B ] [ds]     [gs]        S  = A  - sum_j B_j D_j^-1 B_j'
 //     [ B' D ] [df] = - [gf]        g' = gs - sum_j B_j D_j^-1 gf_j
 //                                   df_j = -D_j^-1 (gf_j + B_j' ds)
 //
-// This replaces what the reference gets from libdogleg/CHOLMOD (Jt*x, the
-// symbolic+numeric factorization of the whole sparse JtJ; call site
-// mrcal.c:6435). The unit of work is the OBSERVATION: one CTA per board
-// observation (or point observation) builds the Gram matrix of that
-// observation's rows over the few columns they touch, in shared memory, and
-// only the reduced result goes to global memory. For splined models the touched
-// knot columns are data-dependent (mrcal.c:2171-2185), so each CTA discovers
-// its own local column set every time.
+// This replaces what the reference gets from libdogleg/CHOLMOD (Jt*x, the symbolic+numeric factorization of the whole
+// sparse JtJ; call site mrcal.c:6435). The unit of work is the OBSERVATION (a work item): pass 1 finds the shared columns
+// each item's rows touch -- for splined models the touched knot columns are data-dependent (mrcal.c:2171-2185) -- and
+// numbers the touched ones compactly; pass 2, one CTA per item, builds the Gram matrix of the item's rows over those
+// columns and leaves its shared x shared block in the item's own block of a pool, and B, D, gf in the item's slots.
+#include <algorithm>
+
+#include "comm.h"
 #include "normal_items.cuh"
-#include "chol.h"
 
 namespace mb200 {
-
-bool comm_active();
-bool comm_allreduce_sum(double* d_buf, size_t count, cudaStream_t s);
-bool comm_allreduce_max_int(int* d_buf, size_t count, cudaStream_t s);
 
 // COMPACTION. Only the shared unknowns that some observation row touches are coupled to anything.
 // For the wide splined models most knots are never hit by a board corner and appear only in their
@@ -134,10 +127,75 @@ compact_scan_kernel(NormalBuffers N)
     if(tid == 1023) N.stat[0] = s_scan[1023];
 }
 
+// exclusive scan of lda^2 over the items [first, Nwi), behind the fixed slots of the first `first` (the board observations
+// of the fused evaluation, which place their compact blocks themselves): one CTA
+__global__ void __launch_bounds__(1024)
+item_offsets_kernel(NormalBuffers N, int first, int Nwi)
+{
+    __shared__ long long s_scan[1024];
+    const int tid = threadIdx.x;
+    const int per = (Nwi - first + 1023) / 1024;
+    const int lo = first + tid * per, hi = min(lo + per, Nwi);
+    long long cnt = 0;
+    for(int w = lo; w < hi; w++)
+    {
+        const int lda = (N.wi_nsh[w] + 2 + 1) & ~1;
+        N.wi_lda[w] = lda;
+        cnt += (long long)lda * lda;
+    }
+    s_scan[tid] = cnt;
+    __syncthreads();
+    for(int o = 1; o < 1024; o <<= 1)
+    {
+        const long long v = tid >= o ? s_scan[tid - o] : 0;
+        __syncthreads();
+        s_scan[tid] += v;
+        __syncthreads();
+    }
+    long long base = (long long)first * kCompactSlot + s_scan[tid] - cnt;
+    for(int w = lo; w < hi; w++)
+    {
+        N.wi_Aoff[w] = base;
+        base += (long long)N.wi_lda[w] * N.wi_lda[w];
+    }
+    if(tid == 1023)
+    {
+        // pool too small: normal_adopt_sizes() grows it and the items are placed again
+        const long long need = (long long)first * kCompactSlot + s_scan[1023];
+        *N.pool_need = need;
+        if(need > N.A_pool) N.stat[2] = 1;
+    }
+}
+
+// After the compaction: compact column of each local column, the two gradient rows, the first local column of
+// every 64-column block, the block presence bits. One warp per item
+__global__ void __launch_bounds__(256)
+item_prepare_kernel(NormalBuffers N, int Nwi, int n_c, int nblk)
+{
+    const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if(w >= Nwi) return;
+    const int nsh = N.wi_nsh[w];
+    const int* cols = N.wi_cols + (size_t)w * N.cap;
+    unsigned short* cc = N.wi_ccol + (size_t)w * N.capA;
+    unsigned short* seg = N.wi_segoff + (size_t)w * (N.nblk_max + 1);
+    const int n = nsh + 2;
+    for(int l = lane; l < n; l += 32)
+    {
+        const int c = l < nsh ? N.cidx[cols[l]] : n_c + (l - nsh);
+        cc[l] = (unsigned short)c;
+        const int blk = c >> 6;
+        const int prev = l == 0 ? -1 : ((l - 1 < nsh ? N.cidx[cols[l - 1]] : n_c + (l - 1 - nsh)) >> 6);
+        // blocks (prev, blk] start at local column l
+        for(int b = prev + 1; b <= blk; b++) seg[b] = (unsigned short)l;
+        if(blk != prev) atomicOr(&N.wi_present[(size_t)blk * N.wwords + (w >> 5)], 1u << (w & 31));
+        if(l == n - 1) for(int b = blk + 1; b <= nblk; b++) seg[b] = (unsigned short)n;
+    }
+}
+
 // Pass 2, one CTA per work item: the Gram matrix of the item's rows over its local columns. The tensor-pipe kernel below
 // takes the items up to kDmmaMaxCols local columns; this one the wider ones (splined observations that touch many knots).
 // Like that kernel, it leaves the shared x shared block and -J'x in the item's own block of the pool and B, D, gf in the
-// item's slots; normal_det.cu sums the blocks into S in a fixed order
+// item's slots; normal_schur.cu sums the blocks into S in a fixed order
 __global__ void __launch_bounds__(256, 1)
 assemble_items_kernel(DevProblem P, NormalBuffers N, int gram_cap, const double* __restrict__ x,
                       const double* __restrict__ Jval, const int* __restrict__ Jcol, int w0)
@@ -448,7 +506,7 @@ assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double*
     // ---- write out from the accumulators. Lane holds G[8 ti + g][8 tj + 2t + {0,1}]
     double* B = N.wi_B + (size_t)w * 6 * N.cap;
     // the shared x shared block and the gradient go to this item's own block of the pool (every entry of the lower
-    // triangle exactly once, zeros included); normal_det.cu sums the blocks into S in a fixed order
+    // triangle exactly once, zeros included); normal_schur.cu sums the blocks into S in a fixed order
     double* Aw = N.wi_A + N.wi_Aoff[w];
     const int lda = N.wi_lda[w];
 #pragma unroll
@@ -511,7 +569,6 @@ __global__ void inactive_step_kernel(DevProblem P, NormalBuffers N, double lambd
     if(P.reg && c < n_intr)
     {
         const int cam = c / P.Nintr_state, k = c - cam * P.Nintr_state;
-        const int Ndist_rows = P.opt_dist ? P.Ncam_i * (P.Nintr - 4) : 0;
         if(k >= P.Ncore_state)
         {
             const int j = k - P.Ncore_state;
@@ -519,7 +576,7 @@ __global__ void inactive_step_kernel(DevProblem P, NormalBuffers N, double lambd
             {
                 // rows (radial, tangential) of this knot; entries [d/dx, d/dy] each (eval.cu)
                 const int knot = j >> 1, which = j & 1;
-                const int t0 = cam * (P.Nintr - 4) + 2 * knot;
+                const int t0 = cam * P.Ndist_state + 2 * knot;
                 const double* e0 = &Jval[(size_t)P.reg_j0 + 2 * (size_t)t0];
                 const double* e1 = e0 + 2;
                 const double x0 = x[P.m_reg0 + t0], x1 = x[P.m_reg0 + t0 + 1];
@@ -532,7 +589,7 @@ __global__ void inactive_step_kernel(DevProblem P, NormalBuffers N, double lambd
             }
             else
             {
-                const int t = cam * (P.Nintr - 4) + j;
+                const int t = cam * P.Ndist_state + j;
                 const double e = Jval[(size_t)P.reg_j0 + t];
                 const double H = e * e + lambda;
                 if(H > 0.) step = -e * x[P.m_reg0 + t] / H;
@@ -540,8 +597,8 @@ __global__ void inactive_step_kernel(DevProblem P, NormalBuffers N, double lambd
         }
         else if(k >= 2)
         {
-            const int t = Ndist_rows + 2 * cam + (k - 2);
-            const double e = Jval[(size_t)P.reg_j0 + (size_t)(N.splined ? 2 : 1) * Ndist_rows + 2 * cam + (k - 2)];
+            const int t = P.Nreg_dist + 2 * cam + (k - 2);
+            const double e = Jval[(size_t)P.reg_j0 + (size_t)(N.splined ? 2 : 1) * P.Nreg_dist + 2 * cam + (k - 2)];
             const double H = e * e + lambda;
             if(H > 0.) step = -e * x[P.m_reg0 + t] / H;
         }
@@ -552,17 +609,10 @@ __global__ void inactive_step_kernel(DevProblem P, NormalBuffers N, double lambd
 // One-time, per-device kernel attributes
 static bool configure_kernels()
 {
-    static bool configured[kMaxDevices] = {};
-    int dev = 0;
-    MB200_CUDA_CHECK(cudaGetDevice(&dev));
-    if(dev < 0 || dev >= kMaxDevices) { set_error("device index %d out of range", dev); return false; }
-    if(configured[dev]) return true;
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(assemble_items_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute((assemble_items_dmma_kernel<kDmmaClassTiles[0], 0, kDmmaClassT[0]>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute((assemble_items_dmma_kernel<kDmmaClassTiles[1], kDmmaClassT[0], kDmmaClassT[1]>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute((assemble_items_dmma_kernel<kDmmaClassTiles[2], kDmmaClassT[1], kDmmaClassT[2]>), cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
-    configured[dev] = true;
-    return true;
+    return set_max_dynamic_smem<assemble_items_kernel>(200 * 1024) &&
+           set_max_dynamic_smem<assemble_items_dmma_kernel<kDmmaClassTiles[0], 0, kDmmaClassT[0]>>(100 * 1024) &&
+           set_max_dynamic_smem<assemble_items_dmma_kernel<kDmmaClassTiles[1], kDmmaClassT[0], kDmmaClassT[1]>>(100 * 1024) &&
+           set_max_dynamic_smem<assemble_items_dmma_kernel<kDmmaClassTiles[2], kDmmaClassT[1], kDmmaClassT[2]>>(100 * 1024);
 }
 
 static bool launch_gram_dmma(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, int Nwi, int max_ntot,
@@ -628,6 +678,31 @@ __global__ void marks_unstage_kernel(int* __restrict__ active, int n_r, double* 
     else if(i == n_r && rider != nullptr) *rider = stage[i];
 }
 
+// the column marks and the sizes of an evaluation, into the caller's fill
+static void marks_to_clear(const NormalBuffers& N, WordFill* f)
+{
+    f->add(N.active, (size_t)(N.n_r > 0 ? N.n_r : 1) * sizeof(int));
+    f->add(N.stat, 4 * sizeof(int));
+}
+
+static bool clear_marks(NormalBuffers& N, cudaStream_t s)
+{
+    WordFill f;
+    marks_to_clear(N, &f);
+    return fill_words(f, s);
+}
+
+// where each item's block goes: the full-layout blocks of items [first, Nwi), behind the `first` fixed compact slots
+static bool place_items(const DevProblem& dp, NormalBuffers& N, int first, cudaStream_t s, int* nlaunch)
+{
+    const int Nwi = dp.Nobs_board + dp.Nobs_point;
+    if(Nwi - first <= 0) return true;
+    item_offsets_kernel<<<1, 1024, 0, s>>>(N, first, Nwi);
+    (*nlaunch)++;
+    MB200_CUDA_CHECK(cudaGetLastError());
+    return true;
+}
+
 bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, cudaStream_t s, int* nlaunch, bool boards_done,
                     double* rider, bool* rider_summed, bool copy_sizes)
 {
@@ -643,7 +718,7 @@ bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& o
     const int Nwi = dp.Nobs_board + dp.Nobs_point;
     // boards_done: the fused evaluation (fused_eval.cu) has already listed the board observations' columns and marked
     // them, into buffers the caller cleared before it ran
-    if(!boards_done && !normal_clear_marks(N, s)) return false;
+    if(!boards_done && !clear_marks(N, s)) return false;
     const int w0 = boards_done ? dp.Nobs_board : 0;
     if(Nwi - w0 > 0) { item_columns_kernel<<<Nwi - w0, 256, lmap_bytes, s>>>(dp, N, op.Jcol, w0); (*nlaunch)++; }
     if(dp.reg_unity) { mark_reg_active_kernel<<<1, 32, 0, s>>>(dp, N); (*nlaunch)++; }
@@ -665,23 +740,10 @@ bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& o
     compact_scan_kernel<<<1, 1024, 0, s>>>(N);
     (*nlaunch)++;
     // (the fused evaluation placed the board observations' blocks at their fixed slots)
-    if(!normal_det_item_offsets(dp, N, w0, s, nlaunch)) return false;
+    if(!place_items(dp, N, w0, s, nlaunch)) return false;
     if(copy_sizes) MB200_CUDA_CHECK(cudaMemcpyAsync(N.h_stat, N.stat, 4 * sizeof(int), cudaMemcpyDeviceToHost, s));
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;
-}
-
-void normal_marks_to_clear(const NormalBuffers& N, WordFill* f)
-{
-    f->add(N.active, (size_t)(N.n_r > 0 ? N.n_r : 1) * sizeof(int));
-    f->add(N.stat, 4 * sizeof(int));
-}
-
-bool normal_clear_marks(NormalBuffers& N, cudaStream_t s)
-{
-    WordFill f;
-    normal_marks_to_clear(N, &f);
-    return fill_words(f, s);
 }
 
 // After the stream was synchronised: take over what normal_prepare() found. If the items' blocks outgrew the pool (wide
@@ -728,7 +790,7 @@ bool normal_assemble(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& 
     return normal_adopt_sizes(N, s) && normal_finish(dp, N, op, d_rowptr, lambda, s, nlaunch, false);
 }
 
-// Pass 2: Gram matrices, Schur elimination, regularization, right-hand side: S, g', J'x
+// Pass 2: the Gram matrices of the items, then their sum into S, g', J'x (normal_schur.cu)
 bool normal_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
                    double lambda, cudaStream_t s, int* nlaunch, bool boards_done, double* also_clear, int also_clear_n)
 {
@@ -739,18 +801,26 @@ bool normal_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op
     const int max_ntot = N.max_ntot;
     if(N.replace_items)
     {
-        if(!normal_det_item_offsets(dp, N, w0, s, nlaunch)) return false;
+        if(!place_items(dp, N, w0, s, nlaunch)) return false;
         N.replace_items = false;
     }
-    // every accumulator and counter of the assembly (and the caller's scalars) zeroed in one launch
+    // every accumulator and counter of the assembly (and the caller's scalars) zeroed in one launch: with the presence
+    // bitmaps and the tiles' arrival counters
+    const int nblk = N.ldS / kCholBlock;
     WordFill clear;
     clear.add(N.g_full, (size_t)dp.Nstate * sizeof(double));
     clear.add(N.info, sizeof(int));
     if(also_clear) clear.add(also_clear, (size_t)also_clear_n * sizeof(double));
-    normal_det_to_clear(N, &clear);
+    clear.add(N.wi_present, (size_t)nblk * N.wwords * sizeof(unsigned));
+    if(N.Ngroups > 0) clear.add(N.grp_present, (size_t)nblk * N.gwords * sizeof(unsigned));
+    clear.add(N.part_arrive, (size_t)(nblk * (nblk + 1) / 2) * sizeof(int));
     if(!fill_words(clear, s)) return false;
 
-    if(!normal_det_item_prepare(dp, N, s, nlaunch)) return false;
+    if(Nwi > 0)
+    {
+        item_prepare_kernel<<<(Nwi * 32 + 255) / 256, 256, 0, s>>>(N, Nwi, N.n_c, nblk);
+        (*nlaunch)++;
+    }
     if(((max_ntot + 1 + 7) / 8) * 8 <= kDmmaMaxCols)
     {
         if(!launch_gram_dmma(dp, N, op, Nwi, max_ntot, lmap_bytes, s, nlaunch, w0)) return false;
@@ -763,10 +833,8 @@ bool normal_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op
         assemble_items_kernel<<<Nwi - w0, 256, lmap_bytes + (gram_doubles + 2) * sizeof(double), s>>>(dp, N, gram_cap, op.x, op.Jval, op.Jcol, w0);
         (*nlaunch)++;
     }
-    if(!normal_det_finish(dp, N, op, d_rowptr, lambda, s, nlaunch)) return false;
-    if(!normal_det_rhs(N, s, nlaunch)) return false;
     MB200_CUDA_CHECK(cudaGetLastError());
-    return true;
+    return normal_schur_sum(dp, N, op, d_rowptr, lambda, s, nlaunch);
 }
 
 // y (the forward-substituted right-hand side) out of row n_c of the factor; padding 0
@@ -802,9 +870,125 @@ bool normal_expand_step(const DevProblem& dp, const NormalBuffers& N, const Eval
         inactive_step_kernel<<<(N.n_r + 255) / 256, 256, 0, s>>>(dp, N, lambda, op.x, op.Jval, step_full);
         (*nlaunch)++;
     }
-    if(!normal_det_backsub(N, sol, step_full, s, nlaunch)) return false;
     MB200_CUDA_CHECK(cudaGetLastError());
+    return normal_schur_backsub(N, sol, step_full, s, nlaunch);
+}
+
+bool normal_evaluate(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, cudaStream_t s, int* nlaunch)
+{
+    if(!N.fused) return launch_evaluate(dp, op, true, nullptr, s, nlaunch);
+    // boards: residuals and normal-equation blocks in one pass, no Jacobian; the rest (points, regularization) as usual
+    WordFill clear;   // the cost and the marks of the columns, in one launch
+    clear.add(op.norm2, sizeof(double));
+    marks_to_clear(N, &clear);
+    return fill_words(clear, s) && launch_unpack_state(dp, op.p, s, nlaunch) && launch_fused_boards(dp, N, op, N.norm_part, s, nlaunch) &&
+           launch_evaluate(dp, op, true, nullptr, s, nlaunch, false);
+}
+
+bool normal_buffers_create(NormalBuffers* Np, const mrcal_b200_problem* P, DeviceArena& A)
+{
+    NormalBuffers& N = *Np;
+    const Layout& L = P->L;
+    const bool elim = L.sel.do_optimize_frames && (L.i_frame0 >= 0 || L.i_point0 >= 0);
+    N.e0 = elim ? (L.i_frame0 >= 0 ? L.i_frame0 : L.i_point0) : L.Nstate;
+    N.e1 = elim ? N.e0 + (L.i_frame0 >= 0 ? 6 * L.d.Nframes : 0) + (L.i_point0 >= 0 ? 3 * L.Npoints_variable : 0) : L.Nstate;
+    N.n_r = L.Nstate - (N.e1 - N.e0);
+    N.ldS_max = chol_padded(N.n_r + 2);
+    N.ldS = N.ldS_max;
+    N.n_c = N.n_r;
+    N.splined = L.splined;
+    N.cap = L.Nintr_state + 8;
+    N.Nframe_groups = (elim && L.i_frame0 >= 0) ? L.d.Nframes : 0;
+    const int Npoint_groups = (elim && L.i_point0 >= 0) ? L.Npoints_variable : 0;
+    N.Ngroups = N.Nframe_groups + Npoint_groups;
+    const int Nwi = L.d.Nobs_board + L.d.Nobs_point;
+
+    // group -> work items (board observations are sorted by frame; point observations are bucketed)
+    std::vector<int> ptr(N.Ngroups + 1, 0), items;
+    {
+        std::vector<std::vector<int>> buckets(N.Ngroups);
+        if(N.Nframe_groups)
+            for(int w = 0; w < L.d.Nobs_board; w++) buckets[P->h_obs_board[3 * w + 2]].push_back(w);
+        if(Npoint_groups)
+            for(int o = 0; o < L.d.Nobs_point; o++)
+            {
+                const int ip = P->h_obs_point[3 * o + 2];
+                if(ip < L.Npoints_variable) buckets[N.Nframe_groups + ip].push_back(L.d.Nobs_board + o);
+            }
+        for(int g = 0; g < N.Ngroups; g++)
+        {
+            ptr[g] = (int)items.size();
+            items.insert(items.end(), buckets[g].begin(), buckets[g].end());
+        }
+        ptr[N.Ngroups] = (int)items.size();
+    }
+
+    bool ok = A.alloc(&N.S, (size_t)N.ldS_max * N.ldS_max) && A.alloc(&N.gs, (size_t)N.ldS_max, true) && A.alloc(&N.g_full, L.Nstate, true) &&
+              A.alloc(&N.info, 4, true) && A.alloc(&N.active, N.n_r, true) && A.alloc(&N.cidx, N.n_r, true) &&
+              A.alloc(&N.cinv, N.ldS_max, true) && A.alloc(&N.stat, 4, true) &&
+              A.alloc(&N.wi_nsh, Nwi, true) && A.alloc(&N.wi_cols, (size_t)Nwi * N.cap) &&
+              A.alloc(&N.wi_B, (size_t)Nwi * 6 * N.cap) && A.alloc(&N.wi_D, (size_t)Nwi * 36) && A.alloc(&N.wi_gf, (size_t)Nwi * 6) &&
+              A.alloc(&N.grp_ptr, (size_t)N.Ngroups + 1) && A.alloc(&N.grp_items, items.size());
+    if(!ok) return false;
+    // The pool of per-item blocks is sized for the items the problem has in the common case; wider ones (splined boards
+    // that touch more knots) make it grow (normal_adopt_sizes)
+    N.nblk_max = N.ldS_max / kCholBlock;
+    N.capA = N.cap + 2;
+    {
+        auto even = [](int v) { return (v + 1) & ~1; };
+        const int lda_board = even(std::min(N.capA, (L.splined ? 160 : L.Nintr_state + 8) + 2));
+        const int lda_point = even(std::min(N.capA, (L.splined ? 2 * 16 + 4 + 6 : L.Nintr_state + 6) + 2));
+        // (a splined model's boards may also take the fused evaluation's fixed compact slots)
+        const long long board_block = L.splined ? std::max((long long)lda_board * lda_board, kCompactSlot) : (long long)lda_board * lda_board;
+        N.A_pool = (long long)L.d.Nobs_board * board_block + (long long)L.d.Nobs_point * lda_point * lda_point;
+    }
+    // (schur_tiles_kernel addresses the pool with 32-bit element offsets: 4 G doubles = 34 GB)
+    if(N.A_pool >= (1ll << 32)) { set_error("the observations' normal-equation blocks need %lld doubles: at most 2^32 are supported", N.A_pool); return false; }
+    N.gwords = (N.Ngroups + 31) / 32; if(N.gwords < 1) N.gwords = 1;
+    N.wwords = (Nwi + 31) / 32;
+    N.bwords = (N.nblk_max + 31) / 32;
+    MB200_CUDA_CHECK(cudaMalloc(&N.wi_A, (size_t)(N.A_pool > 0 ? N.A_pool : 1) * sizeof(double)));   // (not in the arena: it may grow)
+    const NormalSchurSizes z = normal_schur_sizes(N.nblk_max);
+    ok = A.alloc(&N.pool_need, 1, true) && A.alloc(&N.wi_Aoff, Nwi, true) && A.alloc(&N.wi_lda, Nwi, true) &&
+         A.alloc(&N.wi_ccol, (size_t)Nwi * N.capA, true) && A.alloc(&N.wi_segoff, (size_t)Nwi * (N.nblk_max + 1), true) &&
+         A.alloc(&N.Ypan, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * N.nblk_max * kYpanel) &&
+         A.alloc(&N.grp_present, (size_t)N.nblk_max * N.gwords, true) && A.alloc(&N.wi_present, (size_t)N.nblk_max * N.wwords, true) &&
+         A.alloc(&N.grp_blkmask, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * N.bwords, true) &&
+         A.alloc(&N.grp_Linv, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * 36, true) && A.alloc(&N.grp_h, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * 6, true) &&
+         A.alloc(&N.part_scratch, z.part_scratch_doubles) && A.alloc(&N.part_arrive, z.part_arrive_ints, true) &&
+         // (always there: the communicator may be created after these buffers)
+         A.alloc(&N.S_packed, z.packed_doubles);
+    if(!ok) return false;
+    // the fused evaluation (fused_eval.cu): splined models with the core locked, boards of at most 128 corners
+    N.fused = L.splined && !L.sel.do_optimize_intrinsics_core && L.sel.do_optimize_intrinsics_distortions &&
+              L.sel.do_optimize_frames && L.i_frame0 >= 0 && L.d.Nobs_board > 0 && L.d.W * L.d.H <= 128;
+    // (the fused kernel places each board observation's block itself: fixed slots of kCompactSlot doubles, normal.h)
+    if(N.fused && !(A.alloc(&N.norm_part, L.d.Nobs_board, true) && A.alloc(&N.qf_part, L.d.Nobs_board, true))) return false;
+    MB200_CUDA_CHECK(cudaEventCreateWithFlags(&N.ev_fork, cudaEventDisableTiming));
+    for(int k = 0; k < 2; k++)
+    {
+        MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&N.s_side[k], cudaStreamNonBlocking));
+        MB200_CUDA_CHECK(cudaEventCreateWithFlags(&N.ev_join[k], cudaEventDisableTiming));
+    }
+    MB200_CUDA_CHECK(cudaMemcpyAsync(N.grp_ptr, ptr.data(), ptr.size() * sizeof(int), cudaMemcpyHostToDevice, P->stream));
+    if(!items.empty())
+        MB200_CUDA_CHECK(cudaMemcpyAsync(N.grp_items, items.data(), items.size() * sizeof(int), cudaMemcpyHostToDevice, P->stream));
+    MB200_CUDA_CHECK(cudaStreamSynchronize(P->stream));
     return true;
+}
+
+void normal_buffers_destroy(NormalBuffers* N)
+{
+    if(N->wi_A) cudaFree(N->wi_A);
+    for(int k = 0; k < 2; k++)
+    {
+        if(N->s_side[k]) cudaStreamDestroy(N->s_side[k]);
+        if(N->ev_join[k]) cudaEventDestroy(N->ev_join[k]);
+    }
+    if(N->ev_fork) cudaEventDestroy(N->ev_fork);
+    N->wi_A = nullptr;
+    N->s_side[0] = N->s_side[1] = nullptr;
+    N->ev_join[0] = N->ev_join[1] = N->ev_fork = nullptr;
 }
 
 }  // namespace mb200

@@ -1,7 +1,9 @@
-// Internal: normal-equation assembly + Schur elimination (normal.cu)
+// Internal: the normal equations of the trust-region step, reduced to the shared unknowns by Schur elimination.
+// normal.cu: which shared unknowns the rows touch, and the per-item blocks; normal_schur.cu: their sum into S, and the
+// back-substitution of the eliminated unknowns
 #pragma once
-#include "problem.h"
 #include "chol.h"
+#include "problem_impl.h"
 
 namespace mb200 {
 
@@ -58,11 +60,11 @@ struct NormalBuffers
     int*    grp_ptr;    // [Ngroups+1]
     int*    grp_items;  // work item ids
 
-    // ---- the assembly without atomics (normal_det.cu): every entry of S is summed by ONE thread in a fixed order
+    // ---- the sum into S (normal_schur.cu): every entry of S is summed by ONE thread in a fixed order
     bool    fused;        // the board rows are evaluated by fused_eval.cu: blocks straight from the projection, no J
     double* norm_part;    // [Nobs_board] per-observation |x|^2
     double* qf_part;      // [Nobs_board] per-observation g'(J'J)g
-    cudaStream_t s_side[2];               // forked streams of the Gram kernel's size classes (owned by the workspace)
+    cudaStream_t s_side[2];               // forked streams: the Gram kernel's size classes; [0] also the step's Cauchy sums
     cudaEvent_t  ev_fork, ev_join[2];
     int     capA;         // most local columns (incl. the two gradient rows) an item may have in the A pool
     double* wi_A;         // pool of per-item Gram blocks over the shared columns, in one of two layouts (wi_lda says which):
@@ -110,11 +112,59 @@ struct NormalBuffers
     }
 };
 
+// The first eliminated column of group grp, relative to e0
+__host__ __device__ inline int group_col0(const NormalBuffers& N, int grp)
+{
+    return grp < N.Nframe_groups ? 6 * grp : 6 * N.Nframe_groups + 3 * (grp - N.Nframe_groups);
+}
+
+// The regularization block of an uncoupled shared unknown (state column c), the only rows that touch it: H = J'J over
+// its 1 or 2 columns and, if x is given, J'x. n = 0: no row touches c
+struct UncoupledBlock { int n, which; double Hxx, Hyy, Hxy, gx, gy; };
+__device__ __forceinline__ UncoupledBlock uncoupled_block(const DevProblem& P, bool splined, int c, const double* __restrict__ Jval,
+                                                          const double* __restrict__ x)
+{
+    UncoupledBlock u{};
+    const int b = reg_block_of_column(P, splined, c, &u.which);
+    if(b < 0) return u;
+    const RegBlock rb = reg_block(P, splined, b);
+    u.n = rb.ncol;
+    if(rb.ncol == 2)
+    {
+        // rows (radial, tangential) of the knot; entries [d/dx, d/dy] each
+        const double* e0 = &Jval[rb.j0];
+        const double* e1 = e0 + 2;
+        u.Hxx = e0[0] * e0[0] + e1[0] * e1[0];
+        u.Hyy = e0[1] * e0[1] + e1[1] * e1[1];
+        u.Hxy = e0[0] * e0[1] + e1[0] * e1[1];
+        if(x != nullptr)
+        {
+            const double x0 = x[rb.m0], x1 = x[rb.m0 + 1];
+            u.gx = e0[0] * x0 + e1[0] * x1;
+            u.gy = e0[1] * x0 + e1[1] * x1;
+        }
+    }
+    else
+    {
+        const double e = Jval[rb.j0];
+        u.Hxx = e * e;
+        if(x != nullptr) u.gx = e * x[rb.m0];
+    }
+    return u;
+}
+
+// The buffers of the normal equations of problem P (its layout, its observations): allocated in `arena`, except for
+// what may grow or is not memory (the pool of the items' blocks, the side streams and their events), which
+// normal_buffers_destroy() releases. N.h_stat is the caller's to set
+bool normal_buffers_create(NormalBuffers* N, const mrcal_b200_problem* P, DeviceArena& arena);
+void normal_buffers_destroy(NormalBuffers* N);
+
+// The evaluation at `op` that the assembly needs: the fused one when N.fused (the board observations' blocks straight
+// from the projection, the other rows as usual), the stored-Jacobian one otherwise. normal_prepare() comes next
+bool normal_evaluate(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, cudaStream_t s, int* nlaunch);
 // The same in pieces, for a caller that wants to pick its own moment to wait for the device:
 // prepare (device work + an async copy of the sizes) -> [synchronise the stream] -> adopt_sizes -> finish
 // (copy_sizes = false: the caller copies stat[] to h_stat itself, together with its own scalars)
-bool normal_clear_marks(NormalBuffers& N, cudaStream_t s);
-void normal_marks_to_clear(const NormalBuffers& N, WordFill* f);   // the same buffers, into the caller's fill
 bool normal_prepare(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, cudaStream_t s, int* nlaunch, bool boards_done,
                     double* rider = nullptr, bool* rider_summed = nullptr, bool copy_sizes = true);
 bool normal_adopt_sizes(NormalBuffers& N, cudaStream_t s);   // (s: the stream the pool is used on, when it grows)
@@ -135,17 +185,13 @@ bool normal_extract_y(const NormalBuffers& N, double* rhs, cudaStream_t s, int* 
 bool normal_expand_step(const DevProblem& dp, const NormalBuffers& N, const EvalBuffers& op, double lambda,
                         const double* sol, double* step_full, cudaStream_t s, int* nlaunch);
 
-// normal_det.cu: the stages after the per-item Gram matrices, without atomics
-bool normal_det_finish(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
-                       double lambda, cudaStream_t s, int* nlaunch);
-bool normal_det_item_prepare(const DevProblem& dp, NormalBuffers& N, cudaStream_t s, int* nlaunch);   // after the compaction
-void normal_det_to_clear(const NormalBuffers& N, WordFill* f);   // before item_prepare: what it and det_finish expect zeroed
-// before it: the full-layout blocks of items [first, Nwi), behind the `first` fixed compact slots
-bool normal_det_item_offsets(const DevProblem& dp, NormalBuffers& N, int first, cudaStream_t s, int* nlaunch);
-size_t normal_det_part_scratch_doubles(int nblk_max);
-int normal_det_part_arrive_ints(int nblk_max);
-size_t normal_det_packed_doubles(int nblk_max);
-bool normal_det_rhs(const NormalBuffers& N, cudaStream_t s, int* nlaunch);   // after the cross-rank reduction of S
-bool normal_det_backsub(const NormalBuffers& N, const double* sol_compact, double* step_full, cudaStream_t s, int* nlaunch);
+// normal_schur.cu. S, g' and J'x from the items' blocks at `op` (normal_finish() runs it)
+bool normal_schur_sum(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& op, const int* d_rowptr,
+                      double lambda, cudaStream_t s, int* nlaunch);
+// the eliminated unknowns of the step from the compact solution (normal_expand_step() runs it)
+bool normal_schur_backsub(const NormalBuffers& N, const double* sol_compact, double* step_full, cudaStream_t s, int* nlaunch);
+// what its buffers need for a system of up to nblk_max 64-column blocks
+struct NormalSchurSizes { size_t part_scratch_doubles; int part_arrive_ints; size_t packed_doubles; };
+NormalSchurSizes normal_schur_sizes(int nblk_max);
 
 }  // namespace mb200

@@ -1,4 +1,4 @@
-// Internal: what the assembly kernels of normal.cu and normal_det.cu share.
+// Internal: what the assembly kernels of normal.cu, normal_schur.cu and fused_eval.cu share.
 #pragma once
 #include "normal.h"
 

@@ -16,13 +16,11 @@
 // thread walks the pairs of one point in the reference's order; points are
 // independent of each other. Sharded solves: the sums and the "found" flag are
 // all-reduced, every rank marks its own frames.
+#include "comm.h"
 #include "device_math.cuh"
 #include "problem_impl.h"
 
 namespace mb200 {
-
-bool comm_active();
-bool comm_allreduce_sum(double* d_buf, size_t count, cudaStream_t s);
 
 constexpr double kOutlierK0 = 4.0, kOutlierK1 = 5.0;
 // Fixed, not derived from the SM count: the number of partial sums sets the order of the additions, and so

@@ -204,7 +204,7 @@ mrcal_b200_problem_create_triangulated(const double* intrinsics, const mrcal_pos
     }
 
     tri_set_obs0.push_back(Nobservations_point_triangulated);
-    // the pairs of each camera, in order: what the assembly's owner of an extrinsics entry walks (normal_det.cu)
+    // the pairs of each camera, in order: what the assembly's owner of an extrinsics entry walks (normal_schur.cu)
     std::vector<int> tri_cam_ptr(Ncameras_extrinsics + 1, 0), tri_cam_rows;
     for(int e = 0; e < Ncameras_extrinsics; e++)
     {
@@ -355,6 +355,7 @@ mrcal_b200_problem_create_triangulated(const double* intrinsics, const mrcal_pos
     dp.obs_board = d_obs_board; dp.obs_board_pool = P->d_pool_board;
     dp.obs_point = d_obs_point; dp.obs_point_pool = P->d_pool_point;
     dp.board_j0 = d_board_j0; dp.point_j0 = d_point_j0; dp.reg_j0 = reg_j0;
+    dp.Nreg_dist = L.Nreg_dist; dp.Nreg_center = L.Nreg_center; dp.Nreg_unity = L.Nreg_unity;
     dp.m_tri0 = L.m_tri0; dp.Ntri = d.Nmeas_tri;
     dp.tri_px = d_tri_px; dp.tri_cam_e = d_tri_cam_e; dp.tri_outlier = d_tri_outlier; dp.tri_pairs = d_tri_pairs; dp.tri_j0 = d_tri_j0;
     dp.Ntri_sets = (int)tri_set_m0.size(); dp.tri_set_obs0 = d_tri_set_obs0; dp.tri_set_m0 = d_tri_set_m0;

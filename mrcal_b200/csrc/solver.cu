@@ -12,15 +12,10 @@
 #include <algorithm>
 #include <cmath>
 
+#include "comm.h"
 #include "solver_internal.h"
 
 namespace mb200 {
-
-bool comm_active();                                                             // nccl.cu
-bool comm_allreduce_sum(double* d_buf, size_t count, cudaStream_t s);           // nccl.cu
-int  comm_rank();
-long comm_collective_count();
-// the per-rank partial sums of the Cauchy phase sit in slots [6..8] (eliminated range) and [9..10] (row sums): one call
 
 static void delete_ws(SolverWorkspace* w) { delete w; }
 static bool build_workspace(mrcal_b200_problem* P);
@@ -101,31 +96,6 @@ dots_kernel(const double* __restrict__ a, const double* __restrict__ b, int e0, 
     }
 }
 
-// step = cg g + cn gn ; p_new = p + step
-__global__ void combine_step_kernel(int n, double cg, const double* __restrict__ g, double cn, const double* __restrict__ gn,
-                                    const double* __restrict__ p, double* __restrict__ step, double* __restrict__ p_new)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if(i >= n) return;
-    const double s = cg * g[i] + (cn != 0. ? cn * gn[i] : 0.);
-    step[i] = s;
-    p_new[i] = p[i] + s;
-}
-
-// rhs = -g' (reduced) ; padding = 0
-__global__ void negate_kernel(int n, int npad, const double* __restrict__ in, double* __restrict__ out)
-{
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if(i < npad) out[i] = i < n ? -in[i] : 0.;
-}
-
-// shared part of the full-length GN step, from the reduced solution
-__global__ void scatter_shared_kernel(NormalBuffers N, const double* __restrict__ ds, double* __restrict__ step_full)
-{
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if(r < N.n_r) step_full[N.state_index(r)] = ds[r];
-}
-
 // number of board corners with weight < 0 (mrcal.c:6420-6425). Integer atomics: order-independent
 __global__ void count_negative_kernel(const double* __restrict__ pool, long n, int* __restrict__ out)
 {
@@ -148,90 +118,11 @@ static bool build_workspace(mrcal_b200_problem* P)
     NormalBuffers& N = ws->N;
     DeviceArena& A = ws->arena;
 
-    const bool elim = L.sel.do_optimize_frames && (L.i_frame0 >= 0 || L.i_point0 >= 0);
-    N.e0 = elim ? (L.i_frame0 >= 0 ? L.i_frame0 : L.i_point0) : L.Nstate;
-    N.e1 = elim ? N.e0 + (L.i_frame0 >= 0 ? 6 * L.d.Nframes : 0) + (L.i_point0 >= 0 ? 3 * L.Npoints_variable : 0) : L.Nstate;
-    N.n_r = L.Nstate - (N.e1 - N.e0);
-    N.ldS_max = chol_padded(N.n_r + 2);
-    N.ldS = N.ldS_max;
-    N.n_c = N.n_r;
-    N.splined = L.splined;
-    N.cap = L.Nintr_state + 8;
-    N.Nframe_groups = (elim && L.i_frame0 >= 0) ? L.d.Nframes : 0;
-    const int Npoint_groups = (elim && L.i_point0 >= 0) ? L.Npoints_variable : 0;
-    N.Ngroups = N.Nframe_groups + Npoint_groups;
-    const int Nwi = L.d.Nobs_board + L.d.Nobs_point;
-
-    // group -> work items (board observations are sorted by frame; point observations are bucketed)
-    std::vector<int> ptr(N.Ngroups + 1, 0), items;
-    {
-        std::vector<std::vector<int>> buckets(N.Ngroups);
-        if(N.Nframe_groups)
-            for(int w = 0; w < L.d.Nobs_board; w++) buckets[P->h_obs_board[3 * w + 2]].push_back(w);
-        if(Npoint_groups)
-            for(int o = 0; o < L.d.Nobs_point; o++)
-            {
-                const int ip = P->h_obs_point[3 * o + 2];
-                if(ip < L.Npoints_variable) buckets[N.Nframe_groups + ip].push_back(L.d.Nobs_board + o);
-            }
-        for(int g = 0; g < N.Ngroups; g++)
-        {
-            ptr[g] = (int)items.size();
-            items.insert(items.end(), buckets[g].begin(), buckets[g].end());
-        }
-        ptr[N.Ngroups] = (int)items.size();
-    }
-
-    bool ok = A.alloc(&N.S, (size_t)N.ldS_max * N.ldS_max) && A.alloc(&N.gs, (size_t)N.ldS_max, true) && A.alloc(&N.g_full, L.Nstate, true) &&
-              A.alloc(&N.info, 4, true) && A.alloc(&N.active, N.n_r, true) && A.alloc(&N.cidx, N.n_r, true) &&
-              A.alloc(&N.cinv, N.ldS_max, true) && A.alloc(&N.stat, 4, true) &&
-              A.alloc(&N.wi_nsh, Nwi, true) && A.alloc(&N.wi_cols, (size_t)Nwi * N.cap) &&
-              A.alloc(&N.wi_B, (size_t)Nwi * 6 * N.cap) && A.alloc(&N.wi_D, (size_t)Nwi * 36) && A.alloc(&N.wi_gf, (size_t)Nwi * 6) &&
-              A.alloc(&N.grp_ptr, (size_t)N.Ngroups + 1) && A.alloc(&N.grp_items, items.size()) &&
-              A.alloc(&ws->invL, (size_t)N.ldS_max * kCholBlock) && A.alloc(&ws->rhs, N.ldS_max, true) &&
-              A.alloc(&ws->step_gn, L.Nstate, true) && A.alloc(&ws->step, L.Nstate, true) && A.alloc(&ws->scal, 64, true) &&
-              A.alloc(&ws->ictl, 8, true);
+    if(!normal_buffers_create(&N, P, A)) return false;
+    const bool ok = A.alloc(&ws->invL, (size_t)N.ldS_max * kCholBlock) && A.alloc(&ws->rhs, N.ldS_max, true) &&
+                    A.alloc(&ws->step_gn, L.Nstate, true) && A.alloc(&ws->step, L.Nstate, true) && A.alloc(&ws->scal, 64, true) &&
+                    A.alloc(&ws->ictl, 8, true);
     if(!ok) return false;
-    // the assembly without atomics (normal_det.cu). Its pool of per-item blocks is sized for the items the problem has in
-    // the common case; wider ones (splined boards that touch more knots) make it grow (normal_adopt_sizes)
-    N.nblk_max = N.ldS_max / kCholBlock;
-    N.capA = N.cap + 2;
-    {
-        auto even = [](int v) { return (v + 1) & ~1; };
-        const int lda_board = even(std::min(N.capA, (L.splined ? 160 : L.Nintr_state + 8) + 2));
-        const int lda_point = even(std::min(N.capA, (L.splined ? 2 * 16 + 4 + 6 : L.Nintr_state + 6) + 2));
-        // (a splined model's boards may also take the fused evaluation's fixed compact slots)
-        const long long board_block = L.splined ? std::max((long long)lda_board * lda_board, kCompactSlot) : (long long)lda_board * lda_board;
-        N.A_pool = (long long)L.d.Nobs_board * board_block + (long long)L.d.Nobs_point * lda_point * lda_point;
-    }
-    // (schur_tiles_kernel addresses the pool with 32-bit element offsets: 4 G doubles = 34 GB)
-    if(N.A_pool >= (1ll << 32)) { set_error("the observations' normal-equation blocks need %lld doubles: at most 2^32 are supported", N.A_pool); return false; }
-    N.gwords = (N.Ngroups + 31) / 32; if(N.gwords < 1) N.gwords = 1;
-    N.wwords = (Nwi + 31) / 32;
-    N.bwords = (N.nblk_max + 31) / 32;
-    MB200_CUDA_CHECK(cudaMalloc(&N.wi_A, (size_t)(N.A_pool > 0 ? N.A_pool : 1) * sizeof(double)));   // (owned by the workspace: it may grow)
-    ok = A.alloc(&N.pool_need, 1, true) && A.alloc(&N.wi_Aoff, Nwi, true) && A.alloc(&N.wi_lda, Nwi, true) &&
-         A.alloc(&N.wi_ccol, (size_t)Nwi * N.capA, true) && A.alloc(&N.wi_segoff, (size_t)Nwi * (N.nblk_max + 1), true) &&
-         A.alloc(&N.Ypan, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * N.nblk_max * kYpanel) &&
-         A.alloc(&N.grp_present, (size_t)N.nblk_max * N.gwords, true) && A.alloc(&N.wi_present, (size_t)N.nblk_max * N.wwords, true) &&
-         A.alloc(&N.grp_blkmask, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * N.bwords, true) &&
-         A.alloc(&N.grp_Linv, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * 36, true) && A.alloc(&N.grp_h, (size_t)(N.Ngroups > 0 ? N.Ngroups : 1) * 6, true) &&
-         A.alloc(&N.part_scratch, normal_det_part_scratch_doubles(N.nblk_max)) && A.alloc(&N.part_arrive, normal_det_part_arrive_ints(N.nblk_max), true) &&
-         // (always there: the communicator may be created after this workspace)
-         A.alloc(&N.S_packed, normal_det_packed_doubles(N.nblk_max));
-    if(!ok) return false;
-    // the fused evaluation (fused_eval.cu): splined models with the core locked, boards of at most 128 corners
-    N.fused = L.splined && !L.sel.do_optimize_intrinsics_core && L.sel.do_optimize_intrinsics_distortions &&
-              L.sel.do_optimize_frames && L.i_frame0 >= 0 && L.d.Nobs_board > 0 && L.d.W * L.d.H <= 128 &&
-              getenv("MRCAL_B200_NO_FUSED") == nullptr;
-    // (the fused kernel places each board observation's block itself: fixed slots of kCompactSlot doubles, normal.h)
-    if(N.fused && !(A.alloc(&N.norm_part, L.d.Nobs_board, true) && A.alloc(&N.qf_part, L.d.Nobs_board, true))) return false;
-    MB200_CUDA_CHECK(cudaEventCreateWithFlags(&N.ev_fork, cudaEventDisableTiming));
-    for(int k = 0; k < 2; k++)
-    {
-        MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&N.s_side[k], cudaStreamNonBlocking));
-        MB200_CUDA_CHECK(cudaEventCreateWithFlags(&N.ev_join[k], cudaEventDisableTiming));
-    }
     MB200_CUDA_CHECK(cudaMallocHost(&ws->h_scal, 64 * sizeof(double)));
     MB200_CUDA_CHECK(cudaMallocHost(&ws->h_info, 16 * sizeof(int)));
     N.h_stat = ws->h_info + 4;
@@ -239,10 +130,6 @@ static bool build_workspace(mrcal_b200_problem* P)
     MB200_CUDA_CHECK(cudaHostGetDevicePointer((void**)&ws->h_scal_dev, ws->h_scal, 0));
     MB200_CUDA_CHECK(cudaHostGetDevicePointer((void**)&ws->h_info_dev, ws->h_info, 0));
     if(!chol_scratch_create(&ws->chol, N.ldS_max)) return false;
-    MB200_CUDA_CHECK(cudaMemcpyAsync(N.grp_ptr, ptr.data(), ptr.size() * sizeof(int), cudaMemcpyHostToDevice, P->stream));
-    if(!items.empty())
-        MB200_CUDA_CHECK(cudaMemcpyAsync(N.grp_items, items.data(), items.size() * sizeof(int), cudaMemcpyHostToDevice, P->stream));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(P->stream));
     P->ws = std::move(ws);
     return true;
 }
@@ -299,7 +186,7 @@ struct PhaseTimer
 //   11..19 dots of (gn, g) by range: gn.gn, g.g, gn.g
 //   22     |x|^2 at the trial point
 //   32 cg  33 cn  34 update_lensq  35 edge  36 cauchy_lensq  37 gn_lensq  38 kc  39 expected improvement
-// ictl[]: 0 need_gn (the factorization kernels run only if set)  1 zero gradient
+// ictl[]: 0 need_gn (the Cauchy point is inside the trust region)  1 zero gradient
 enum { SC_CG = 32, SC_CN, SC_UPDATE, SC_EDGE, SC_CAUCHY2, SC_GN2, SC_KC, SC_EXPECTED, SC_N = 48 };
 
 // Sharded solves: the per-rank partial sums among the scalars -- [6..10] (eliminated part of |g|^2, the row sums of
@@ -419,18 +306,7 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
     auto evaluate = [&](int which) -> bool
     {
         const int a = T->mark();
-        if(N.fused)
-        {
-            // boards: residuals and normal-equation blocks in one pass, no Jacobian; the rest (points, regularization) as usual
-            const EvalBuffers& o = P->op[which];
-            WordFill clear;   // the cost and the marks of the columns, in one launch
-            clear.add(o.norm2, sizeof(double));
-            normal_marks_to_clear(N, &clear);
-            if(!fill_words(clear, s) || !launch_unpack_state(P->dp, o.p, s, nl) ||
-               !launch_fused_boards(P->dp, N, o, N.norm_part, s, nl) ||
-               !launch_evaluate(P->dp, o, true, nullptr, s, nl, false)) return false;
-        }
-        else if(!problem_evaluate(P, which, true, false)) return false;
+        if(!normal_evaluate(P->dp, N, P->op[which], s, nl)) return false;
         T->spans[0].push_back({a, T->mark()});
         info->Nevaluations++;
         const int b = T->mark();
@@ -528,17 +404,12 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
             // idle). The price: whether the Cauchy point already leaves the trust region -- and the Gauss-Newton step is
             // unnecessary -- is only known afterwards, so every new operating point is factored; the rare unnecessary
             // factorization (the first few steps of a solve) costs less than those sums on the critical path of every step
-            const bool overlap = N.s_side[0] != nullptr && getenv("MRCAL_B200_NO_OVERLAP") == nullptr;
             if(!have_cauchy)
             {
                 // (scal[0..31] were cleared by the assembly, which always comes right before)
-                cudaStream_t sc = s;
-                if(overlap)
-                {
-                    sc = N.s_side[0];
-                    MB200_CUDA_CHECK(cudaEventRecord(N.ev_fork, s));
-                    MB200_CUDA_CHECK(cudaStreamWaitEvent(sc, N.ev_fork, 0));
-                }
+                cudaStream_t sc = N.s_side[0];
+                MB200_CUDA_CHECK(cudaEventRecord(N.ev_fork, s));
+                MB200_CUDA_CHECK(cudaStreamWaitEvent(sc, N.ev_fork, 0));
                 dots_kernel<<<3, 1024, 0, sc>>>(N.g_full, nullptr, e0, e1, Nstate, ws->scal + 0);
                 const int nsm = std::max(1, device_sm_count());
                 if(N.fused)
@@ -551,55 +422,38 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
                 else
                     jv_kernel<<<nsm * 16, 256, 0, sc>>>(P->d_rowptr, cur.Jcol, cur.Jval, N.g_full, cur.x, 0, Nrows_mine, ws->scal + 9);
                 *nl += 2;
-                if(overlap) MB200_CUDA_CHECK(cudaEventRecord(N.ev_join[0], sc));
+                MB200_CUDA_CHECK(cudaEventRecord(N.ev_join[0], sc));
                 // eliminated-range dots and the row sums are per-rank partial sums. Sharded: they wait for the partial sums
                 // of the Gauss-Newton dots and go through ONE reduction with them (below)
                 have_cauchy = true;
             }
-            const bool sharded = comm_active();
-            if(have_gn)
-            {
-                // (same operating point, smaller trust region: everything is there)
-                cauchy_decide_kernel<<<1, 32, 0, s>>>(ws->scal, ws->ictl, trustregion);
-                (*nl)++;
-            }
+            // (have_gn: same operating point, smaller trust region: everything is there)
             bool factored_now = false;
             if(!have_gn)
             {
-                // ---- Gauss-Newton step: factor the reduced system, solve, back-substitute. Without the overlap (and not
-                // sharded) the kernels look at ictl[0] and do nothing if the Cauchy point is outside the trust region
-                const int* run_if = nullptr;
-                if(!sharded && !overlap)
-                {
-                    cauchy_decide_kernel<<<1, 32, 0, s>>>(ws->scal, ws->ictl, trustregion);
-                    (*nl)++;
-                    run_if = ws->ictl;
-                }
+                // ---- Gauss-Newton step: factor the reduced system, solve, back-substitute
                 const int a = T->mark();
-                if(!chol_factor(N.S, N.ldS, N.n_c, ws->invL, N.info + 1, s, nl, &ws->chol, run_if)) return false;
+                if(!chol_factor(N.S, N.ldS, N.n_c, ws->invL, N.info + 1, s, nl, &ws->chol)) return false;
                 T->spans[2].push_back({a, T->mark()});
                 const int b = T->mark();
                 if(!normal_extract_y(N, ws->rhs, s, nl)) return false;
-                if(N.n_c > 0 && !chol_solve_backward(N.S, N.ldS, ws->invL, ws->rhs, N.info + 1, s, nl, &ws->chol, run_if)) return false;
+                if(N.n_c > 0 && !chol_solve_backward(N.S, N.ldS, ws->invL, ws->rhs, N.info + 1, s, nl, &ws->chol)) return false;
                 if(!normal_expand_step(P->dp, N, P->op[P->cur], *lambda, ws->rhs, ws->step_gn, s, nl)) return false;
                 dots_kernel<<<3, 1024, 0, s>>>(ws->step_gn, N.g_full, e0, e1, Nstate, ws->scal + 11);
                 (*nl)++;
-                if(overlap) MB200_CUDA_CHECK(cudaStreamWaitEvent(s, N.ev_join[0], 0));
-                if(sharded)
+                MB200_CUDA_CHECK(cudaStreamWaitEvent(s, N.ev_join[0], 0));
+                if(comm_active())
                 {
                     stage_partials_kernel<<<1, 32, 0, s>>>(ws->scal, true);
                     if(!comm_allreduce_sum(ws->scal + 50, 8, s)) return false;
                     stage_partials_kernel<<<1, 32, 0, s>>>(ws->scal, false);
                     *nl += 2;
                 }
-                if(sharded || overlap)
-                {
-                    cauchy_decide_kernel<<<1, 32, 0, s>>>(ws->scal, ws->ictl, trustregion);
-                    (*nl)++;
-                }
                 T->spans[3].push_back({b, T->mark()});
                 factored_now = true;
             }
+            cauchy_decide_kernel<<<1, 32, 0, s>>>(ws->scal, ws->ictl, trustregion);
+            (*nl)++;
             // ---- take the step
             select_step_kernel<<<1, 32, 0, s>>>(ws->scal, ws->ictl, trustregion, *lambda);
             combine_step_dev_kernel<<<(Nstate + 255) / 256, 256, 0, s>>>(Nstate, ws->scal, N.g_full, ws->step_gn, cur.p, ws->step, nxt.p);
@@ -619,7 +473,7 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
                     return false;
                 }
                 // (sharded: a frame block that is singular on ONE rank has been reported to every rank with the reduced system
-                // itself, normal_det.cu:unpack_extras_kernel, and the factorization is replicated)
+                // itself, normal_schur.cu:unpack_extras_kernel, and the factorization is replicated)
                 if(bad)
                 {
                     // singular JtJ: add lambda I "from now on", as libdogleg does (1e-10, then x10), and do this operating point again
@@ -810,11 +664,7 @@ extern "C" bool mrcal_b200_problem_reduced_system_fused(mrcal_b200_problem_t* P,
     cudaStream_t s = P->stream;
     int* nl = &P->launches;
     const EvalBuffers& o = P->op[P->cur];
-    WordFill clear;
-    clear.add(o.norm2, sizeof(double));
-    normal_marks_to_clear(N, &clear);
-    if(!fill_words(clear, s) || !launch_unpack_state(P->dp, o.p, s, nl) || !launch_fused_boards(P->dp, N, o, N.norm_part, s, nl) ||
-       !launch_evaluate(P->dp, o, true, nullptr, s, nl, false) || !normal_prepare(P->dp, N, o, s, nl, true)) return false;
+    if(!normal_evaluate(P->dp, N, o, s, nl) || !normal_prepare(P->dp, N, o, s, nl, true)) return false;
     MB200_CUDA_CHECK(cudaStreamSynchronize(s));
     if(!normal_adopt_sizes(N, s)) return false;
     if(N.h_stat[3] != 0)

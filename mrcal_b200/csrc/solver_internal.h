@@ -28,13 +28,7 @@ struct SolverWorkspace
     ~SolverWorkspace()
     {
         chol_forget_graphs(N.S);
-        if(N.wi_A) cudaFree(N.wi_A);
-        for(int k = 0; k < 2; k++)
-        {
-            if(N.s_side[k]) cudaStreamDestroy(N.s_side[k]);
-            if(N.ev_join[k]) cudaEventDestroy(N.ev_join[k]);
-        }
-        if(N.ev_fork) cudaEventDestroy(N.ev_fork);
+        normal_buffers_destroy(&N);
         if(h_scal) cudaFreeHost(h_scal);
         if(h_info) cudaFreeHost(h_info);
         chol_scratch_destroy(&chol);

@@ -10,7 +10,7 @@ Generators:
     minor_failure(S, p, d)   S with its trailing block [p:, p:] changed so that pivot p becomes -d: the leading p x p
                              block is S's, bit for bit, so every earlier pivot is unchanged
     with_nan(A, i, j)        one NaN (and its mirror)
-    augmented(S, b)          the solver's augmented layout (normal_det.cu): rows < nreal: S; row nreal: b' with 1 on
+    augmented(S, b)          the solver's augmented layout (normal_schur.cu): rows < nreal: S; row nreal: b' with 1 on
                              the diagonal; row nreal+1: g' (zero by default) with 1 on the diagonal
 """
 import numpy as np

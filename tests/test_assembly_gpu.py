@@ -1,4 +1,4 @@
-"""The reduced normal equations are assembled without atomics for every problem (normal.cu, normal_det.cu): the same
+"""The reduced normal equations are assembled without atomics for every problem (normal.cu, normal_schur.cu): the same
 problem gives the same system, bit for bit. Also the problems at the edges of that assembly: board
 observations wider than the tensor-pipe Gram kernel takes (more than 160 local columns, and more than 255), and
 problems with no board or point observations at all."""

@@ -326,7 +326,7 @@ def test_not_positive_definite_factorization_object(p):
 
 @pytest.mark.parametrize("n_c,path", [(62, 1), (63, 1), (64, 1), (127, 1), (1268, 1), (127, 2)])
 def test_augmented_row(n_c, path, record_property):
-    """The solver factors S with the right-hand side b' as an extra row n_c (normal_det.cu) and reads its forward
+    """The solver factors S with the right-hand side b' as an extra row n_c (normal_schur.cu) and reads its forward
     substitution from row n_c of L. That row must equal inv(L) b; its pivot, 1 - |inv(L) b|^2, is negative here and
     must stay unreported (only pivots < nreal count)"""
     rng = np.random.default_rng(n_c)
