@@ -9,9 +9,8 @@
 // shared memory; each thread evaluates its corner's projection and gradients
 // in registers and writes its two fixed-width Jacobian rows. Row positions are
 // analytic (fixed nnz per row class), so there is no serial fill pointer.
-#include "device_math.cuh"
+#include "observation.cuh"
 #include "triangulated.cuh"
-#include "problem.h"
 
 namespace mb200 {
 
@@ -145,19 +144,13 @@ __device__ __forceinline__ int emit_intrinsics(double* __restrict__ jv, int* __r
     return n;
 }
 
-struct ObsGeometry   // per observation, in shared memory
-{
-    double Rf[9], dRf[27], tf[3];
-    double Rc[9], dRc[27], tc[3];
-};
-
 // One CTA per board observation, one thread per corner (strided if W*H > blockDim)
 template <int KIND, bool WITH_J>
 __global__ void __maxnreg__(160)   // 3 CTAs of 128 threads per SM
 eval_boards_kernel(DevProblem P, double* __restrict__ x, double* __restrict__ Jval, int* __restrict__ Jcol,
                    double* __restrict__ norm2)
 {
-    __shared__ ObsGeometry G;
+    __shared__ ObsPoses G;
     __shared__ double red[32];
     __shared__ int s_ivar0[256];   // per corner: where its spline window starts (the only data-dependent column index)
     __shared__ __align__(8) int s_pat[2 * 256]; // per entry of a corner's two rows: its column for a window at 0, and whether the window's
@@ -175,22 +168,7 @@ eval_boards_kernel(DevProblem P, double* __restrict__ x, double* __restrict__ Jv
     const int iframe = P.obs_board[3 * iobs + 2];
     const bool cam_identity = icam_e < 0;
 
-    if(threadIdx.x < 36)
-    {
-        const double v = P.u_rot_frame[36 * iframe + threadIdx.x];
-        if(threadIdx.x < 9) G.Rf[threadIdx.x] = v; else G.dRf[threadIdx.x - 9] = v;
-    }
-    else if(threadIdx.x < 39) G.tf[threadIdx.x - 36] = P.u_rtframe[6 * iframe + 3 + threadIdx.x - 36];
-    if(!cam_identity)
-    {
-        if(threadIdx.x >= 64 && threadIdx.x < 100)
-        {
-            const int k = threadIdx.x - 64;
-            const double v = P.u_rot_cam[36 * icam_e + k];
-            if(k < 9) G.Rc[k] = v; else G.dRc[k - 9] = v;
-        }
-        else if(threadIdx.x >= 40 && threadIdx.x < 43) G.tc[threadIdx.x - 40] = P.u_rtcam[6 * icam_e + 3 + threadIdx.x - 40];
-    }
+    load_obs_poses(G, P, iframe, icam_e, threadIdx.x);
     __syncthreads();
 
     const double* __restrict__ intr = &P.u_intr[(size_t)icam_i * P.Nintr];
@@ -249,29 +227,8 @@ eval_boards_kernel(DevProblem P, double* __restrict__ x, double* __restrict__ Jv
       const int ipt = ipt0 + threadIdx.x;
       if(ipt < NWH)
       {
-        const int cx = ipt % P.W, cy = ipt / P.W;
-        // the board point, with the parabolic warp (mrcal.c:2794-2819)
-        double pt[3] = {(double)cx * P.spacing, (double)cy * P.spacing, 0.};
-        double dz[2] = {0., 0.};
-        if(P.have_warp)
-        {
-            const double xr = (double)cx / (double)(P.W - 1);
-            const double yr = (double)cy / (double)(P.H - 1);
-            dz[0] = 4. * xr * (1. - xr);
-            dz[1] = 4. * yr * (1. - yr);
-            pt[2] += wx2 * dz[0];
-            pt[2] += wy2 * dz[1];
-        }
-        // v = Rf pt + tf (reference coords); p = Rc v + tc (camera coords)
-        double v[3], p[3];
-        mat3_vec(v, G.Rf, pt);
-        v[0] += G.tf[0]; v[1] += G.tf[1]; v[2] += G.tf[2];
-        if(cam_identity) { p[0] = v[0]; p[1] = v[1]; p[2] = v[2]; }
-        else
-        {
-            mat3_vec(p, G.Rc, v);
-            p[0] += G.tc[0]; p[1] += G.tc[1]; p[2] += G.tc[2];
-        }
+        double pt[3], dz[2], v[3], p[3];
+        board_corner(pt, dz, v, p, P, G, cam_identity, ipt % P.W, ipt / P.W, wx2, wy2);
 
         double q[2], dq_dp[2][3];
         double ddist[2][LensTraits<KIND>::NDIST > 0 ? LensTraits<KIND>::NDIST : 1];

@@ -9,7 +9,7 @@
 // mrcal-calibrate-cameras:641-643; every BASELINE splined config).
 //
 // One CTA per board observation, one thread per corner:
-//   1. project the corner (same device functions as eval.cu): residuals, the B-spline basis (wx, wy) of its window,
+//   1. project the corner (its point from observation.cuh): residuals, the B-spline basis (wx, wy) of its window,
 //      and the 14 "geometric" entries of each of its two rows (camera r,t | frame r,t | warp)
 //   2. the knots the observation touches form a patch of the control-point grid; the x row of a corner touches the
 //      x surface with values  w b fx, the y row the y surface with  w b fy,  b = wx (x) wy THE SAME for both rows.
@@ -24,8 +24,8 @@
 //
 // Replaces, for this path: the board loop of optimizer_callback() (mrcal.c:4604-4900), libdogleg's Jt*x and what
 // CHOLMOD's A*A' does with those rows.
-#include "device_math.cuh"
 #include "normal_items.cuh"
+#include "observation.cuh"
 
 namespace mb200 {
 
@@ -35,8 +35,6 @@ constexpr int FLDK = 68;    // row stride of Dk [K][<=64 knots]: 4 (mod 16), con
 constexpr int FLDG = 36;    // row stride of G  [K][32]
 constexpr int FMAXK = kCompactMaxKnots;   // most knots of one observation's patch that are touched
 constexpr int FMAXPATCH = 400;   // bounding box of the patch (knots)
-
-struct FusedGeom { double Rf[9], dRf[27], tf[3], Rc[9], dRc[27], tc[3]; };
 
 }  // namespace
 
@@ -50,7 +48,7 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
     double* Gs = Dk + (size_t)K * FLDK;      // [K][FLDG]
     double* Cs = Gs + (size_t)K * FLDG;      // [FMAXK][33]  Dk'[Gx Gy ex ey]
     double* GG = Cs + FMAXK * 33;            // [14][14] + gv[14]
-    __shared__ FusedGeom G;
+    __shared__ ObsPoses G;
     __shared__ short s_kidx[FMAXPATCH];
     __shared__ unsigned char s_touched[FMAXPATCH];
     __shared__ int s_win[128];               // per corner: window origin (wy0 << 16 | wx0)
@@ -64,13 +62,7 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
     const bool emit_cam = P.opt_extr && !cam_identity;
     const int NWH = P.W * P.H;
 
-    if(tid < 36) { const double v = P.u_rot_frame[36 * iframe + tid]; if(tid < 9) G.Rf[tid] = v; else G.dRf[tid - 9] = v; }
-    else if(tid < 39) G.tf[tid - 36] = P.u_rtframe[6 * iframe + 3 + tid - 36];
-    if(!cam_identity)
-    {
-        if(tid >= 64 && tid < 100) { const int k = tid - 64; const double v = P.u_rot_cam[36 * icam_e + k]; if(k < 9) G.Rc[k] = v; else G.dRc[k - 9] = v; }
-        else if(tid >= 40 && tid < 43) G.tc[tid - 40] = P.u_rtcam[6 * icam_e + 3 + tid - 40];
-    }
+    load_obs_poses(G, P, iframe, icam_e, tid);
     if(tid == 0) { s_box[0] = 1 << 30; s_box[1] = -1; s_box[2] = 1 << 30; s_box[3] = -1; s_bad = 0; }
     for(int e = tid; e < K * FLDK; e += 128) Dk[e] = 0.;
     for(int e = tid; e < K * FLDG; e += 128) Gs[e] = 0.;
@@ -89,21 +81,8 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
     {
         const int ipt = tid;
         const int cx = ipt % P.W, cy = ipt / P.W;
-        double pt[3] = {(double)cx * P.spacing, (double)cy * P.spacing, 0.};
-        double dz[2] = {0., 0.};
-        if(P.have_warp)
-        {
-            const double xr = (double)cx / (double)(P.W - 1), yr = (double)cy / (double)(P.H - 1);
-            dz[0] = 4. * xr * (1. - xr);
-            dz[1] = 4. * yr * (1. - yr);
-            pt[2] += wx2 * dz[0];
-            pt[2] += wy2 * dz[1];
-        }
-        double v[3], p[3];
-        mat3_vec(v, G.Rf, pt);
-        v[0] += G.tf[0]; v[1] += G.tf[1]; v[2] += G.tf[2];
-        if(cam_identity) { p[0] = v[0]; p[1] = v[1]; p[2] = v[2]; }
-        else { mat3_vec(p, G.Rc, v); p[0] += G.tc[0]; p[1] += G.tc[1]; p[2] += G.tc[2]; }
+        double pt[3], dz[2], v[3], p[3];
+        board_corner(pt, dz, v, p, P, G, cam_identity, cx, cy, wx2, wy2);
 
         double q[2], dq_dp[2][3], wxb[4], wyb[4], upd[2];
         int ivar0;
