@@ -20,15 +20,16 @@
 //
 // Stands in for cholmod_factorize / cholmod_solve as the reference calls them (mrcal.c:6435, mrcal-pywrap.c:196-212,
 // 557). Storage: row-major npad x npad, lower triangle, npad a multiple of 64 (the caller puts 1 on the padding
-// diagonal). Rows are K-contiguous, which is what mma.sync.m8n8k4.row.col.f64 wants for both operands of  C -= P P'.
+// diagonal). Rows are K-contiguous, which is what dmma() (ptx.cuh, row x col) wants for both operands of  C -= P P'.
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <vector>
 
 #include "chol.h"
-#include "dmma.cuh"
 #include "potrf_block.cuh"
 #include "problem.h"
+#include "ptx.cuh"
+#include "reduce.cuh"
 
 namespace mb200 {
 
@@ -118,15 +119,6 @@ trsm_kernel(double* __restrict__ A, int ld, int k0, const double* __restrict__ i
 // Operands staged through shared memory with cp.async, 3 stages of BK=16.
 ////////////////////////////////////////////////////////////////////////////////
 constexpr int BM = 128, BK = 16, LDS = BK + 4, STAGES = 3;
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid)
-{
-    const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-    const int sz = valid ? 16 : 0;   // src-size 0: zero-fill
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem), "r"(sz));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
 // TILE = 128: 8 warps as 4 x 2, warp tile 32 x 64 (4 x 8 DMMA tiles)   -- large trailing matrices
 // TILE =  64: 8 warps as 4 x 2, warp tile 16 x 32 (2 x 4 DMMA tiles)   -- small ones: 4x the CTAs, so the
@@ -258,9 +250,7 @@ solve_update_fwd_kernel(const double* __restrict__ L, int ld, int n, double* __r
     for(int r = 0; r < nrhs; r++)
     {
         const double* y = B + (size_t)r * ldb + k0;
-        double acc = l0 * y[lane] + l1 * y[32 + lane];
-#pragma unroll
-        for(int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+        const double acc = warp_sum(l0 * y[lane] + l1 * y[32 + lane]);
         if(lane == 0) B[(size_t)r * ldb + i] -= acc;
     }
 }
@@ -396,22 +386,11 @@ static const size_t kPotrfSmem = sizeof(PotrfSmem);
 
 static bool configure_kernels()
 {
-    // cudaFuncSetAttribute is per device
-    static bool configured_dev[kMaxDevices] = {};
-    int dev = 0;
-    MB200_CUDA_CHECK(cudaGetDevice(&dev));
-    if(dev < 0 || dev >= kMaxDevices) { set_error("device index %d out of range", dev); return false; }
-    bool& configured = configured_dev[dev];
-    if(configured) return true;
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(syrk_dmma_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyrkSmem));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(syrk_dmma_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSyrkSmem));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(trsm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBlockSmem));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(potrf_diag_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(potrf_diag_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPotrfSmem));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(ls_solve_tiled_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveTileSmem));
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(ls_solve_tiled_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveTileSmem));
-    configured = true;
-    return true;
+    return set_max_dynamic_smem<syrk_dmma_kernel<128>>((int)kSyrkSmem) && set_max_dynamic_smem<syrk_dmma_kernel<64>>((int)kSyrkSmem) &&
+           set_max_dynamic_smem<trsm_kernel>((int)kBlockSmem) &&
+           set_max_dynamic_smem<potrf_diag_kernel<false>>((int)kPotrfSmem) && set_max_dynamic_smem<potrf_diag_kernel<true>>((int)kPotrfSmem) &&
+           set_max_dynamic_smem<ls_solve_tiled_kernel<false>>((int)kSolveTileSmem) &&
+           set_max_dynamic_smem<ls_solve_tiled_kernel<true>>((int)kSolveTileSmem);
 }
 
 static bool syrk_update(double* A, int ld, int n, int c0, int c1, int k0, int k1, cudaStream_t s, int* nlaunch)

@@ -49,13 +49,6 @@ __device__ __forceinline__ void st_release(int* p, int v)
 {
     asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
-__device__ __forceinline__ void cp16(void* smem, const void* gmem)
-{
-    const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
-}
-__device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-__device__ __forceinline__ void cp_wait_all() { asm volatile("cp.async.wait_group 0;\n" ::); }
 
 // 64x64 tile, row stride ld in global -> [64][PLD] in shared. 2048 16-byte chunks, 8 per thread
 __device__ __forceinline__ void tile_to_smem(double* dst, const double* src, size_t ld)
@@ -64,7 +57,7 @@ __device__ __forceinline__ void tile_to_smem(double* dst, const double* src, siz
     for(int q = 0; q < 8; q++)
     {
         const int chunk = threadIdx.x + q * 256, r = chunk >> 5, c = (chunk & 31) * 2;
-        cp16(&dst[r * PLD + c], &src[(size_t)r * ld + c]);
+        cp_async16(&dst[r * PLD + c], &src[(size_t)r * ld + c]);
     }
 }
 
@@ -111,7 +104,7 @@ __device__ __forceinline__ void tile_mma(double (&acc)[2][4][2], const double* A
 #pragma unroll
         for(int i = 0; i < 2; i++)
 #pragma unroll
-            for(int j = 0; j < 4; j++) pb_dmma(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+            for(int j = 0; j < 4; j++) dmma(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
     }
 }
 __device__ __forceinline__ void acc_zero(double (&acc)[2][4][2])
@@ -156,7 +149,7 @@ __device__ __forceinline__ void tile_trsm(const double* C, const double* W, doub
 #pragma unroll
         for(int j = 0; j < 8; j++)
             if(ks * 4 < 8 * (j + 1))
-                pb_dmma(acc[j][0], acc[j][1], af, W[(j * 8 + g) * PLD + ks * 4 + t]);
+                dmma(acc[j][0], acc[j][1], af, W[(j * 8 + g) * PLD + ks * 4 + t]);
     }
 #pragma unroll
     for(int j = 0; j < 8; j++)
@@ -196,8 +189,8 @@ __device__ __forceinline__ void tile_syrk_lower_sub(double* C, const double* D, 
 #pragma unroll
             for(int m = 0; m < 5; m++)
                 if(m < 4 || five)
-                    pb_dmma(acc[m][h][0], acc[m][h][1], A[(gr[m] * 8 + g) * PLD + (ks + h * (T / 8)) * 4 + t],
-                            A[(gc[m] * 8 + g) * PLD + (ks + h * (T / 8)) * 4 + t]);
+                    dmma(acc[m][h][0], acc[m][h][1], A[(gr[m] * 8 + g) * PLD + (ks + h * (T / 8)) * 4 + t],
+                         A[(gc[m] * 8 + g) * PLD + (ks + h * (T / 8)) * 4 + t]);
     }
 #pragma unroll
     for(int m = 0; m < 5; m++)
@@ -247,8 +240,8 @@ chol_spine_kernel(double* __restrict__ A, int ld, int nb, int nreal, double* __r
     {
         ////////////////////////////// the spine
         tile_to_smem(sm.pb.L, A, ld);
-        cp_commit();
-        cp_wait_all();
+        cp_async_commit();
+        cp_async_wait<0>();
         for(int d = 0; d < nb; d++)
         {
             double* Add = A + (size_t)d * T * ld + (size_t)d * T;
@@ -281,7 +274,7 @@ chol_spine_kernel(double* __restrict__ A, int ld, int nb, int nreal, double* __r
                 {
                     tile_to_smem(sm.C2, A + (size_t)(d + 1) * T * ld + (size_t)d * T, ld);
                     tile_to_smem(sm.opB, A + (size_t)(d + 1) * T * ld + (size_t)(d + 1) * T, ld);
-                    cp_commit();
+                    cp_async_commit();
                 }
             }
             SPINE_STAMP(4);
@@ -303,13 +296,13 @@ chol_spine_kernel(double* __restrict__ A, int ld, int nb, int nreal, double* __r
                 if(!wait_flags(sm, pre + d + 1, nullptr, abort_flag, info)) return;
                 tile_to_smem(sm.C2, A + (size_t)(d + 1) * T * ld + (size_t)d * T, ld);
                 tile_to_smem(sm.opB, A + (size_t)(d + 1) * T * ld + (size_t)(d + 1) * T, ld);
-                cp_commit();
-                cp_wait_all();
+                cp_async_commit();
+                cp_async_wait<0>();
                 __syncthreads();
             }
             else
             {
-                cp_wait_all();
+                cp_async_wait<0>();
                 __syncthreads();
                 if(tid == 255) st_release(flags + tile_flag(d, d, nb), 1);
             }
@@ -333,14 +326,14 @@ chol_spine_kernel(double* __restrict__ A, int ld, int nb, int nreal, double* __r
             const int i = rem == 0 ? j + 2 : j + 1 + rem;
             double* Aij = A + (size_t)i * T * ld + (size_t)j * T;
             tile_to_smem(sm.C2, Aij, ld);
-            cp_commit();
+            cp_async_commit();
             for(int k = 0; k < j; k++)
             {
                 if(!wait_flags(sm, flags + tile_flag(i, k, nb), flags + tile_flag(j, k, nb), abort_flag, info)) return;
                 tile_to_smem(sm.opA, A + (size_t)i * T * ld + (size_t)k * T, ld);
                 tile_to_smem(sm.opB, A + (size_t)j * T * ld + (size_t)k * T, ld);
-                cp_commit();
-                cp_wait_all();
+                cp_async_commit();
+                cp_async_wait<0>();
                 __syncthreads();
                 acc_zero(acc);
                 tile_mma(acc, sm.opA, sm.opB);
@@ -349,8 +342,8 @@ chol_spine_kernel(double* __restrict__ A, int ld, int nb, int nreal, double* __r
             }
             if(!wait_flags(sm, flags + tile_flag(j, j, nb), nullptr, abort_flag, info)) return;
             tile_to_smem(sm.opB, invL + (size_t)j * T * T, T);
-            cp_commit();
-            cp_wait_all();
+            cp_async_commit();
+            cp_async_wait<0>();
             __syncthreads();
             tile_trsm(sm.C2, sm.opB, Aij, ld, nullptr);
             __threadfence();
@@ -365,14 +358,14 @@ chol_spine_kernel(double* __restrict__ A, int ld, int nb, int nreal, double* __r
             double* Add = A + (size_t)d * T * ld + (size_t)d * T;
             tile_to_smem(sm.C2, Aij, ld);
             tile_to_smem(sm.pb.L, Add, ld);
-            cp_commit();
+            cp_async_commit();
             for(int k = 0; k <= d - 2; k++)
             {
                 if(!wait_flags(sm, flags + tile_flag(d, k, nb), flags + tile_flag(d - 1, k, nb), abort_flag, info)) return;
                 tile_to_smem(sm.opA, A + (size_t)d * T * ld + (size_t)k * T, ld);
                 tile_to_smem(sm.opB, A + (size_t)(d - 1) * T * ld + (size_t)k * T, ld);
-                cp_commit();
-                cp_wait_all();
+                cp_async_commit();
+                cp_async_wait<0>();
                 __syncthreads();
                 acc_zero(acc);
                 tile_mma(acc, sm.opA, sm.opB);

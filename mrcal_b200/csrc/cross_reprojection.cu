@@ -24,6 +24,7 @@
 // Accepts what the reference accepts and refuses what it refuses (uncertainty.c:944-989).
 #include "device_math.cuh"
 #include "problem_impl.h"
+#include "reduce.cuh"
 
 namespace mb200 {
 
@@ -133,16 +134,9 @@ cross_observations_kernel(DevProblem P, const double* __restrict__ b, const doub
 #pragma unroll
             for(int i = 0; i < 6; i++) { Gtc[2 * i] += v[i] * jc[0]; Gtc[2 * i + 1] += v[i] * jc[1]; }
     }
-#pragma unroll
-    for(int ofs = 16; ofs > 0; ofs >>= 1)
-    {
-#pragma unroll
-        for(int i = 0; i < 21; i++) Gtt[i] += __shfl_xor_sync(0xffffffffu, Gtt[i], ofs);
-#pragma unroll
-        for(int i = 0; i < 36; i++) Gtf[i] += __shfl_xor_sync(0xffffffffu, Gtf[i], ofs);
-#pragma unroll
-        for(int i = 0; i < 12; i++) Gtc[i] += __shfl_xor_sync(0xffffffffu, Gtc[i], ofs);
-    }
+    warp_sum(Gtt);
+    warp_sum(Gtf);
+    warp_sum(Gtc);
     if(lane != 0) return;
 
     // ---- 2. the transform

@@ -25,6 +25,7 @@
 #include "device_math.cuh"
 #include "lens_dispatch.cuh"
 #include "problem_impl.h"
+#include "reduce.cuh"
 
 namespace mb200 {
 namespace {
@@ -119,15 +120,14 @@ __device__ __forceinline__ void residual(double* f, double J[NP], double U[NP][3
     }
 }
 
-// Block-wide sum of NS per-thread values in a fixed order. The result is valid in thread 0 only
+// Block-wide sum of NS per-thread values in a fixed order: warp_sum(), then thread 0 adds the other warps' sums to its
+// own in warp order, ((w0 + w1) + w2) + ... (no zero in front: block_sum_by_warps() would add a +0 first, and thread 0
+// needs all NS sums). The result is valid in thread 0 only
 template <int NS>
-__device__ __forceinline__ void block_sum(double acc[NS], double (*red)[NS])
+__device__ __forceinline__ void block_sum(double (&acc)[NS], double (*red)[NS])
 {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for(int j = 0; j < NS; j++)
-#pragma unroll
-        for(int o = 16; o > 0; o >>= 1) acc[j] += __shfl_down_sync(0xffffffffu, acc[j], o);
+    warp_sum(acc);
     if(lane == 0)
 #pragma unroll
         for(int j = 0; j < NS; j++) red[warp][j] = acc[j];
@@ -180,7 +180,7 @@ __global__ void __launch_bounds__(kFitThreads) implied_fit_kernel(FitArgs A)
     __shared__ double R[9], dR[27], t[3];
     // thread 0's iteration state: the parameters, the sums at them, the step being tried, the damped system
     __shared__ double x[NP], cur[NS], step[NP], xt[NP], H[NP * NP];
-    __shared__ int s_done, s_count[kFitWarps];
+    __shared__ int s_done, s_count[1][kFitWarps];
     const int fit = blockIdx.x, tid = threadIdx.x;
     const double* p0 = A.p0 + fit * A.p0_stride;
     const double* v1 = A.v1 + fit * A.v1_stride;
@@ -189,13 +189,10 @@ __global__ void __launch_bounds__(kFitThreads) implied_fit_kernel(FitArgs A)
     // the focus region must hold at least 3 points (model_analysis.py:213-217)
     int count = 0;
     for(int i = tid; i < A.N; i += kFitThreads) count += kept(A, i);
-    for(int o = 16; o > 0; o >>= 1) count += __shfl_down_sync(0xffffffffu, count, o);
-    if((tid & 31) == 0) s_count[tid >> 5] = count;
-    __syncthreads();
+    int v[1] = {count};
+    const int total = block_sum_by_warps(v, s_count);
     if(tid == 0)
     {
-        int total = 0;
-        for(int w = 0; w < kFitWarps; w++) total += s_count[w];
         A.status[fit] = total < 3 ? FIT_TOO_FEW_POINTS : FIT_OK;
         s_done = total < 3;
     }

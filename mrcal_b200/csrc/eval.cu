@@ -10,6 +10,7 @@
 // in registers and writes its two fixed-width Jacobian rows. Row positions are
 // analytic (fixed nnz per row class), so there is no serial fill pointer.
 #include "observation.cuh"
+#include "ptx.cuh"
 #include "triangulated.cuh"
 
 namespace mb200 {
@@ -330,12 +331,9 @@ eval_boards_kernel(DevProblem P, double* __restrict__ x, double* __restrict__ Jv
             // this corner's 2 rows: one bulk copy, shared -> global, issued by the thread that wrote them. The fence makes
             // the generic-proxy writes above visible to the async proxy that reads them
             {
-                double* gdst = Jval + (size_t)P.board_j0[iobs] + (size_t)ipt * row2;
-                const unsigned ssrc = (unsigned)__cvta_generic_to_shared(stage_v + (size_t)threadIdx.x * stride);
-                asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-                asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;\n"
-                             ::"l"(gdst), "r"(ssrc), "r"(row2 * 8) : "memory");
-                asm volatile("cp.async.bulk.commit_group;\n" ::: "memory");
+                fence_proxy_async();
+                bulk_store(Jval + (size_t)P.board_j0[iobs] + (size_t)ipt * row2, stage_v + (size_t)threadIdx.x * stride, row2 * 8);
+                bulk_commit();
             }
         }
       }
@@ -357,7 +355,7 @@ eval_boards_kernel(DevProblem P, double* __restrict__ x, double* __restrict__ Jv
             }
         }
         // the staging buffer is reused by the next chunk of corners: wait until the TMA has READ it
-        asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory");
+        bulk_wait_read();
         __syncthreads();
       }
     }

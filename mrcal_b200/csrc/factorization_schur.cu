@@ -18,7 +18,8 @@
 // The object OWNS the device problem it was made from (the one the last mrcal_optimizer_callback() call left in the
 // cache): mrcal_b200_factorization_create_from_last_callback().
 #include "comm.h"
-#include "dmma.cuh"
+#include "ptx.cuh"
+#include "reduce.cuh"
 #include "solver_internal.h"
 
 namespace mb200 {
@@ -211,10 +212,7 @@ panels_backward_kernel(NormalBuffers N, double* __restrict__ Bf, int Nelim, cons
 #pragma unroll
         for(int p = 0; p < 6; p++) t[p] += Yg[(size_t)b * kYpanel + p * kYld + lane] * d0 + Yg[(size_t)b * kYpanel + p * kYld + 32 + lane] * d1;
     }
-#pragma unroll
-    for(int p = 0; p < 6; p++)
-#pragma unroll
-        for(int o = 16; o > 0; o >>= 1) t[p] += __shfl_xor_sync(0xffffffffu, t[p], o);
+    warp_sum(t);
     const int nelim = grp < N.Nframe_groups ? 6 : 3;
     if(lane < nelim) Bf[(size_t)rhs * Nelim + group_col0(N, grp) + lane] -= t[lane];
 }
@@ -361,7 +359,7 @@ bool schur_factor_build(mrcal_b200_problem* P, mrcal_b200_factorization* F)
     if(comm_active() || P->sharded) { set_error("structured factorization: not available for sharded problems"); return false; }
     if(!solver_build_workspace(P)) return false;
     // every solve with the factor takes the forward panels' tiles (schur_solve_pieces): more than 48 KB of shared memory
-    MB200_CUDA_CHECK(cudaFuncSetAttribute(panels_forward_tiled_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSolveTileSmem));
+    if(!set_max_dynamic_smem<panels_forward_tiled_kernel>((int)kSolveTileSmem)) return false;
     SolverWorkspace* ws = P->ws.get();
     NormalBuffers& N = ws->N;
     cudaStream_t s = P->stream;

@@ -52,7 +52,7 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
     __shared__ short s_kidx[FMAXPATCH];
     __shared__ unsigned char s_touched[FMAXPATCH];
     __shared__ int s_win[128];               // per corner: window origin (wy0 << 16 | wx0)
-    __shared__ int s_box[4], s_scan[128], s_nk, s_bad;
+    __shared__ int s_box[4], s_scan[128], s_bad;
     __shared__ double s_red[4];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -155,8 +155,7 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
         g[28] = e0; g[29] = e1;
     }
     // |x|^2 of this observation: one partial per CTA, summed in a fixed order later
-#pragma unroll
-    for(int o = 16; o > 0; o >>= 1) sumsq += __shfl_xor_sync(0xffffffffu, sumsq, o);
+    sumsq = warp_sum(sumsq);
     if(lane == 0) s_red[warp] = sumsq;
     __syncthreads();
     if(tid == 0) norm_part[iobs] = (s_red[0] + s_red[1]) + (s_red[2] + s_red[3]);
@@ -178,27 +177,17 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
             for(int ix = 0; ix < RUN; ix++) s_touched[(wy0 - by0 + iy) * pw + (wx0 - bx0 + ix)] = 1;
     }
     __syncthreads();
+    int nk;
     {
         // rank of each touched knot among the touched, in grid (= state) order
         const int per = (npk + 127) / 128;
         const int lo = tid * per, hi = min(lo + per, npk);
         int cnt = 0;
         for(int i = lo; i < hi; i++) cnt += s_touched[i];
-        s_scan[tid] = cnt;
-        __syncthreads();
-        for(int o = 1; o < 128; o <<= 1)
-        {
-            const int vv = tid >= o ? s_scan[tid - o] : 0;
-            __syncthreads();
-            s_scan[tid] += vv;
-            __syncthreads();
-        }
-        int base = s_scan[tid] - cnt;
+        int base = block_exclusive_scan<int, 128>(cnt, s_scan, nk);
         for(int i = lo; i < hi; i++) s_kidx[i] = s_touched[i] ? (short)(base++) : (short)-1;
-        if(tid == 127) s_nk = s_scan[127];
         __syncthreads();
     }
-    const int nk = s_nk;
     const int ncam = emit_cam ? 6 : 0, nwarp = P.opt_warp ? 2 : 0;
     const int nsh = 2 * nk + ncam + nwarp;
     if(nk > FMAXK || nsh + 2 > N.capA)
@@ -265,10 +254,7 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
             sym[u] = qq < nsym;
             if(sym[u])
             {
-                int a = (int)((sqrtf(8.f * qq + 1.f) - 1.f) * 0.5f);
-                while(a * (a + 1) / 2 > qq) a--;
-                while((a + 1) * (a + 2) / 2 <= qq) a++;
-                ti[u] = a; tj[u] = qq - a * (a + 1) / 2;
+                tri_row_col(qq, ti[u], tj[u]);
                 pb[u] = Dk + 8 * tj[u] + g + (size_t)t * FLDK; ldb[u] = FLDK;
             }
             else
@@ -283,7 +269,7 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
         for(int ks = 0; ks < ksteps; ks++)
 #pragma unroll
             for(int u = 0; u < 4; u++)
-                dmma884(acc[u][0], acc[u][1], pa[u][(size_t)ks * 4 * FLDK], pb[u][(size_t)ks * 4 * ldb[u]]);
+                dmma(acc[u][0], acc[u][1], pa[u][(size_t)ks * 4 * FLDK], pb[u][(size_t)ks * 4 * ldb[u]]);
 #pragma unroll
         for(int u = 0; u < 4; u++)
         {
@@ -311,13 +297,7 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
     if(tid < 105 + 14)
     {
         int i, j;
-        if(tid < 105)
-        {
-            i = (int)((sqrtf(8.f * tid + 1.f) - 1.f) * 0.5f);
-            while(i * (i + 1) / 2 > tid) i--;
-            while((i + 1) * (i + 2) / 2 <= tid) i++;
-            j = tid - i * (i + 1) / 2;
-        }
+        if(tid < 105) tri_row_col(tid, i, j);
         else { i = tid - 105; j = -1; }
         double s = 0.;
         for(int k = 0; k < NWH; k++)
@@ -373,21 +353,6 @@ fused_boards_kernel(DevProblem P, NormalBuffers N, double* __restrict__ x, doubl
     }
 }
 
-// sum of the per-observation partial |x|^2, in index order (one block; deterministic)
-__global__ void __launch_bounds__(256)
-sum_norm_partials_kernel(const double* __restrict__ part, int n, double* __restrict__ norm2)
-{
-    __shared__ double s[256];
-    const int tid = threadIdx.x;
-    const int per = (n + 255) / 256;
-    double a = 0.;
-    for(int i = tid * per; i < min(n, (tid + 1) * per); i++) a += part[i];
-    s[tid] = a;
-    __syncthreads();
-    for(int o = 128; o > 0; o >>= 1) { if(tid < o) s[tid] += s[tid + o]; __syncthreads(); }
-    if(tid == 0) *norm2 += s[0];
-}
-
 // |J g|^2 over the board rows from the blocks: g_w' [A B'; B D] g_w per observation. part[w] = that. One CTA per item, one
 // entry of the lower triangle of A per thread and step (all loads independent); the per-thread sums are added in a fixed tree.
 // A is in the compact layout (normal.h); each entry is formed as the full layout holds it, the zeros across the two
@@ -411,10 +376,8 @@ quadform_items_kernel(DevProblem P, NormalBuffers N, const double* __restrict__ 
     const int nent = nsh * (nsh + 1) / 2;
     for(int e = tid; e < nent; e += 128)
     {
-        int i = (int)((sqrtf(8.f * e + 1.f) - 1.f) * 0.5f);
-        while(i * (i + 1) / 2 > e) i--;
-        while((i + 1) * (i + 2) / 2 <= e) i++;
-        const int j = e - i * (i + 1) / 2;
+        int i, j;
+        tri_row_col(e, i, j);
         double a;
         if(i >= 2 * nk)     a = Ag[(size_t)(i - 2 * nk) * nsh + j];
         else if((i ^ j) & 1) a = 0.;
@@ -441,23 +404,8 @@ quadform_items_kernel(DevProblem P, NormalBuffers N, const double* __restrict__ 
                 for(int rr = 0; rr < 6; rr++) q += gf[p] * D[p * 6 + rr] * gf[rr];
         }
     }
-    s_red[tid] = q;
-    __syncthreads();
-    for(int o = 64; o > 0; o >>= 1) { if(tid < o) s_red[tid] += s_red[tid + o]; __syncthreads(); }
+    tree_sum<128>(s_red, q);
     if(tid == 0) part[w] = s_red[0];
-}
-__global__ void __launch_bounds__(256)
-sum_partials_to_kernel(const double* __restrict__ part, int n, double* __restrict__ out)
-{
-    __shared__ double s[256];
-    const int tid = threadIdx.x;
-    const int per = (n + 255) / 256;
-    double a = 0.;
-    for(int i = tid * per; i < min(n, (tid + 1) * per); i++) a += part[i];
-    s[tid] = a;
-    __syncthreads();
-    for(int o = 128; o > 0; o >>= 1) { if(tid < o) s[tid] += s[tid + o]; __syncthreads(); }
-    if(tid == 0) *out += s[0];
 }
 
 // The board observations of the evaluation at `out`: x, |x|^2, and the per-item blocks. The caller has cleared
@@ -471,7 +419,7 @@ bool launch_fused_boards(const DevProblem& dp, NormalBuffers& N, const EvalBuffe
     const size_t smem = ((size_t)K * (FLDK + FLDG) + FMAXK * 33 + 14 * 14 + 14 + 2) * sizeof(double);
     if(dp.lens_kind == LENS_SPLINED3) fused_boards_kernel<4><<<dp.Nobs_board, 128, smem, s>>>(dp, N, out.x, norm_part, K);
     else                              fused_boards_kernel<3><<<dp.Nobs_board, 128, smem, s>>>(dp, N, out.x, norm_part, K);
-    sum_norm_partials_kernel<<<1, 256, 0, s>>>(norm_part, dp.Nobs_board, out.norm2);
+    sum_partials_kernel<256><<<1, 256, 0, s>>>(norm_part, dp.Nobs_board, out.norm2);
     *nlaunch += 2;
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;
@@ -481,7 +429,7 @@ bool launch_quadform_boards(const DevProblem& dp, const NormalBuffers& N, const 
 {
     if(dp.Nobs_board <= 0) return true;
     quadform_items_kernel<<<dp.Nobs_board, 128, 0, s>>>(dp, N, g_full, dp.Nobs_board, part);
-    sum_partials_to_kernel<<<1, 256, 0, s>>>(part, dp.Nobs_board, out);
+    sum_partials_kernel<256><<<1, 256, 0, s>>>(part, dp.Nobs_board, out);
     *nlaunch += 2;
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;

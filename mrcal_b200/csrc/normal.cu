@@ -53,16 +53,8 @@ item_columns_kernel(DevProblem P, NormalBuffers N, const int* __restrict__ Jcol,
     const int lo = tid * per, hi = min(lo + per, d.clen);
     int cnt = 0;
     for(int i = lo; i < hi; i++) cnt += lmap[i];
-    s_scan[tid] = cnt;
-    __syncthreads();
-    for(int o = 1; o < 256; o <<= 1)
-    {
-        const int v = tid >= o ? s_scan[tid - o] : 0;
-        __syncthreads();
-        s_scan[tid] += v;
-        __syncthreads();
-    }
-    int base = s_scan[tid] - cnt;
+    int nloc;
+    int base = block_exclusive_scan<int, 256>(cnt, s_scan, nloc);
     int* cols = N.wi_cols + (size_t)w * N.cap;
     for(int i = lo; i < hi; i++)
         if(lmap[i])
@@ -71,7 +63,6 @@ item_columns_kernel(DevProblem P, NormalBuffers N, const int* __restrict__ Jcol,
             cols[base++] = r;
             N.active[r] = 1;
         }
-    const int nloc = s_scan[255];
     if(tid < ncam)  { const int r = N.reduced_index(d.cam0 + tid);  cols[nloc + tid] = r;        N.active[r] = 1; }
     if(tid < nwarp) { const int r = N.reduced_index(d.warp0 + tid); cols[nloc + ncam + tid] = r; N.active[r] = 1; }
     if(tid == 0)
@@ -109,22 +100,14 @@ compact_scan_kernel(NormalBuffers N)
     const int lo = tid * per, hi = min(lo + per, N.n_r);
     int cnt = 0;
     for(int i = lo; i < hi; i++) cnt += N.active[i] ? 1 : 0;
-    s_scan[tid] = cnt;
-    __syncthreads();
-    for(int o = 1; o < 1024; o <<= 1)
-    {
-        const int v = tid >= o ? s_scan[tid - o] : 0;
-        __syncthreads();
-        s_scan[tid] += v;
-        __syncthreads();
-    }
-    int base = s_scan[tid] - cnt;
+    int total;
+    int base = block_exclusive_scan<int, 1024>(cnt, s_scan, total);
     for(int i = lo; i < hi; i++)
     {
         if(N.active[i]) { N.cidx[i] = base; N.cinv[base] = i; base++; }
         else            N.cidx[i] = -1;
     }
-    if(tid == 1023) N.stat[0] = s_scan[1023];
+    if(tid == 1023) N.stat[0] = total;
 }
 
 // exclusive scan of lda^2 over the items [first, Nwi), behind the fixed slots of the first `first` (the board observations
@@ -143,16 +126,8 @@ item_offsets_kernel(NormalBuffers N, int first, int Nwi)
         N.wi_lda[w] = lda;
         cnt += (long long)lda * lda;
     }
-    s_scan[tid] = cnt;
-    __syncthreads();
-    for(int o = 1; o < 1024; o <<= 1)
-    {
-        const long long v = tid >= o ? s_scan[tid - o] : 0;
-        __syncthreads();
-        s_scan[tid] += v;
-        __syncthreads();
-    }
-    long long base = (long long)first * kCompactSlot + s_scan[tid] - cnt;
+    long long total;
+    long long base = (long long)first * kCompactSlot + block_exclusive_scan<long long, 1024>(cnt, s_scan, total);
     for(int w = lo; w < hi; w++)
     {
         N.wi_Aoff[w] = base;
@@ -161,7 +136,7 @@ item_offsets_kernel(NormalBuffers N, int first, int Nwi)
     if(tid == 1023)
     {
         // pool too small: normal_adopt_sizes() grows it and the items are placed again
-        const long long need = (long long)first * kCompactSlot + s_scan[1023];
+        const long long need = (long long)first * kCompactSlot + total;
         *N.pool_need = need;
         if(need > N.A_pool) N.stat[2] = 1;
     }
@@ -226,12 +201,10 @@ assemble_items_kernel(DevProblem P, NormalBuffers N, int gram_cap, const double*
     for(int i = tid; i < d.clen; i += 256) lmap[i] = -1;
     for(int e = tid; e < kMaxRowNnz * (kMaxRowNnz + 1) / 2; e += 256)
     {
-        // decode pair index e -> (a >= b)
-        int a = (int)((sqrtf(8.f * e + 1.f) - 1.f) * 0.5f);
-        while(a * (a + 1) / 2 > e) a--;
-        while((a + 1) * (a + 2) / 2 <= e) a++;
+        int a, b;
+        tri_row_col(e, a, b);
         s_pa[e] = (unsigned char)a;
-        s_pb[e] = (unsigned char)(e - a * (a + 1) / 2);
+        s_pb[e] = (unsigned char)b;
     }
     for(int i = tid; i < ngram + ntot; i += 256) gram[i] = 0.;
     if(big) for(int i = tid; i < nsh * lda; i += 256) Aw[i] = 0.;
@@ -400,11 +373,10 @@ assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double*
     for(int q = tid; q < ntiles; q += 256)
     {
         // tile q -> (ti >= tj); warp q%8 owns it as its (q/8)-th tile
-        int ti = (int)((sqrtf(8.f * q + 1.f) - 1.f) * 0.5f);
-        while(ti * (ti + 1) / 2 > q) ti--;
-        while((ti + 1) * (ti + 2) / 2 <= q) ti++;
+        int ti, tj;
+        tri_row_col(q, ti, tj);
         s_ti[q] = (unsigned char)ti;
-        s_tj[q] = (unsigned char)(q - ti * (ti + 1) / 2);
+        s_tj[q] = (unsigned char)tj;
     }
     __syncthreads();
     for(int l = tid; l < nloc; l += 256) lmap[cols[l] - d.cbase] = (short)l;
@@ -491,7 +463,7 @@ assemble_items_dmma_kernel(DevProblem P, NormalBuffers N, int ldD, const double*
 #pragma unroll
                 for(int u = 0; u < 4; u++)
                     if(i0 + u < kDmmaMaxTiles)
-                        dmma884(acc[i0 + u][0], acc[i0 + u][1], Da[u][ks * 4 * ldD], Db[u][ks * 4 * ldD]);
+                        dmma(acc[i0 + u][0], acc[i0 + u][1], Da[u][ks * 4 * ldD], Db[u][ks * 4 * ldD]);
         }
         __syncthreads();
         // un-scatter: cheaper than clearing the whole chunk

@@ -1,6 +1,8 @@
 // Internal: what the assembly kernels of normal.cu, normal_schur.cu and fused_eval.cu share.
 #pragma once
 #include "normal.h"
+#include "ptx.cuh"
+#include "reduce.cuh"
 
 namespace mb200 {
 
@@ -58,11 +60,13 @@ __device__ __forceinline__ ItemDesc describe_item(const DevProblem& P, int w, in
 
 __device__ __forceinline__ int tri(int a, int b) { return a * (a + 1) / 2 + b; }   // a >= b
 
-
-__device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b)
+// the inverse of tri(): q -> (r >= c) with tri(r, c) == q. The float square root is a first guess, corrected exactly
+__device__ __forceinline__ void tri_row_col(int q, int& r, int& c)
 {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-                 : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
+    r = (int)((sqrtf(8.f * q + 1.f) - 1.f) * 0.5f);
+    while(r * (r + 1) / 2 > q) r--;
+    while((r + 1) * (r + 2) / 2 <= q) r++;
+    c = q - r * (r + 1) / 2;
 }
 
 }  // namespace mb200

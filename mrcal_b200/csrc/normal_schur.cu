@@ -224,46 +224,11 @@ __device__ __forceinline__ void build_worklist(TileCommon& sm, const unsigned* r
     if(tid == 0) sm.count = sm.scan[0] + sm.scan[1];
     __syncthreads();
 }
-// ---- mbarrier / bulk-copy (TMA) plumbing of phase S
-__device__ __forceinline__ unsigned smem_u32(const void* p) { return (unsigned)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long* bar, int count)
-{
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" :: "r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(unsigned long long* bar, unsigned bytes)
-{
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long* bar, unsigned parity)
-{
-    unsigned ok;
-    do
-    {
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
-                     : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-    } while(!ok);
-}
-// global -> shared, `bytes` (a multiple of 16) contiguous; completion is counted on `bar`
-__device__ __forceinline__ void bulk_load(void* smem, const void* gmem, unsigned bytes, unsigned long long* bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
-                 :: "r"(smem_u32(smem)), "l"(gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
-
 constexpr int kPackedExtras = 8;      // doubles behind the packed tiles (sharded solves)
 constexpr int kMaxParts = 64;         // a tile's contributors may be split over this many CTAs
 constexpr int kCtasPerTile = 4;       // the grid: this many CTAs per tile on average (kernel_ctas()); parts are cut to fit
 // (at least kMaxParts: the one tile of a small system, which every observation reaches, may be split as far as a tile can be)
 __host__ __device__ inline int kernel_ctas(int ntiles) { return kCtasPerTile * ntiles > kMaxParts ? kCtasPerTile * ntiles : kMaxParts; }
-
-__device__ __forceinline__ void tile_row_col(int itile, int& r, int& c)
-{
-    r = (int)((sqrtf(8.f * itile + 1.f) - 1.f) * 0.5f);
-    while(r * (r + 1) / 2 > itile) r--;
-    while((r + 1) * (r + 2) / 2 <= itile) r++;
-    c = itile - r * (r + 1) / 2;
-}
 
 // What each tile has to sum, and over how many CTAs: plan[itile] = (items, groups, parts, -), then the numbers of items
 // and of groups in each stretch of 64 bitmap words (kPlanStretches + kPlanGroupStretches ints; a tile CTA walks past the
@@ -276,7 +241,7 @@ tile_plan_kernel(NormalBuffers N, int nblk, int ns_per_item, int ns_per_group, i
     const int itile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if(itile >= nblk * (nblk + 1) / 2) return;
     int r, c;
-    tile_row_col(itile, r, c);
+    tri_row_col(itile, r, c);
     const unsigned* wiA = N.wi_present + (size_t)r * N.wwords;
     const unsigned* wiB = N.wi_present + (size_t)c * N.wwords;
     int n_items = 0, n_groups = 0;
@@ -285,8 +250,7 @@ tile_plan_kernel(NormalBuffers N, int nblk, int ns_per_item, int ns_per_group, i
     {
         int cnt = 0;
         for(int w = 64 * st + lane; w < min(64 * st + 64, N.wwords); w += 32) cnt += __popc(wiA[w] & wiB[w]);
-#pragma unroll
-        for(int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        cnt = warp_sum(cnt);
         if(lane == 0 && st < kPlanStretches) mine[4 + st] = cnt;
         n_items += cnt;
     }
@@ -298,8 +262,7 @@ tile_plan_kernel(NormalBuffers N, int nblk, int ns_per_item, int ns_per_group, i
         {
             int cnt = 0;
             for(int w = 64 * st + lane; w < min(64 * st + 64, N.gwords); w += 32) cnt += __popc(grA[w] & grB[w]);
-#pragma unroll
-            for(int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+            cnt = warp_sum(cnt);
             if(lane == 0 && st < kPlanGroupStretches) mine[4 + kPlanStretches + st] = cnt;
             n_groups += cnt;
         }
@@ -329,9 +292,7 @@ tile_slots_kernel(int ntiles, int* __restrict__ plan, int* __restrict__ cta)
     // if the tiles wish for more extra parts than there is room for, every wish is scaled down alike
     long wish = 0;
     for(int k = tid; k < ntiles; k += 1024) wish += plan[(size_t)k * kPlanInts + 2] - 1;
-    s_scan[tid] = (int)wish;
-    __syncthreads();
-    for(int o = 512; o > 0; o >>= 1) { if(tid < o) s_scan[tid] += s_scan[tid + o]; __syncthreads(); }
+    tree_sum<1024>(s_scan, (int)wish);
     const long wish_total = s_scan[0];
     __syncthreads();
     for(int k0 = 0; k0 < ntiles; k0 += 1024)
@@ -340,17 +301,9 @@ tile_slots_kernel(int ntiles, int* __restrict__ plan, int* __restrict__ cta)
         const int itile = ntiles - 1 - k;
         int extra = k < ntiles ? plan[(size_t)itile * kPlanInts + 2] - 1 : 0;
         if(wish_total > nctas_max - ntiles) extra = (int)((long)extra * (nctas_max - ntiles) / wish_total);
-        // the extra parts, granted in launch order while there is room: inclusive scan of the wishes
-        s_scan[tid] = extra;
-        __syncthreads();
-        for(int o = 1; o < 1024; o <<= 1)
-        {
-            const int v = tid >= o ? s_scan[tid - o] : 0;
-            __syncthreads();
-            s_scan[tid] += v;
-            __syncthreads();
-        }
-        const int before = s_scan[tid] - extra;        // extra parts wished for by the tiles ahead of this one in the chunk
+        // the extra parts, granted in launch order while there is room
+        int wished;                                    // by the tiles of the chunk
+        const int before = block_exclusive_scan<int, 1024>(extra, s_scan, wished);   // by the tiles ahead of this one
         const int room = s_room;
         const int granted = max(0, min(extra, room - before));
         // slots: the tiles ahead took (their 1 + granted): granted_before = min(before, room)
@@ -364,7 +317,7 @@ tile_slots_kernel(int ntiles, int* __restrict__ plan, int* __restrict__ cta)
         __syncthreads();
         if(tid == 1023)
         {
-            const int used = min(s_scan[1023], room);
+            const int used = min(wished, room);
             s_carry += min(1024, ntiles - k0) + used;
             s_room = room - used;
         }
@@ -394,7 +347,7 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
     const int* pl = plan + (size_t)itile * kPlanInts;
     const int n_items = pl[0], n_groups = pl[1], parts = pl[2], slot0 = pl[3];
     int r, c;
-    tile_row_col(itile, r, c);
+    tri_row_col(itile, r, c);
     const bool diag = r == c;
     const unsigned* wiA = N.wi_present + (size_t)r * N.wwords;
     const unsigned* wiB = N.wi_present + (size_t)c * N.wwords;
@@ -404,7 +357,7 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
     {
         mbar_init(&sc.bar[0], 1);
         mbar_init(&sc.bar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+        fence_mbar_init();
     }
     const int item_lo = (int)((long)n_items * part / parts), item_hi = (int)((long)n_items * (part + 1) / parts);
     const int grp_lo = (int)((long)n_groups * part / parts), grp_hi = (int)((long)n_groups * (part + 1) / parts);
@@ -646,7 +599,7 @@ schur_tiles_kernel(NormalBuffers N, double lambda, int n_c, int nblk, bool add_l
 #pragma unroll
                 for(int a = 0; a < 2; a++)
 #pragma unroll
-                    for(int b = 0; b < 4; b++) dmma884(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
+                    for(int b = 0; b < 4; b++) dmma(acc[a][b][0], acc[a][b][1], af[a], bf[b]);
             }
             __syncthreads();   // this buffer is staged again two chunks from now
         }
@@ -739,13 +692,7 @@ __global__ void __launch_bounds__(256)
 unpack_tiles_kernel(NormalBuffers N, const double* __restrict__ packed, double lambda, int n_c, int nblk)
 {
     int r, c;
-    {
-        const int q = (int)blockIdx.x;
-        r = (int)((sqrtf(8.f * q + 1.f) - 1.f) * 0.5f);
-        while(r * (r + 1) / 2 > q) r--;
-        while((r + 1) * (r + 2) / 2 <= q) r++;
-        c = q - r * (r + 1) / 2;
-    }
+    tri_row_col((int)blockIdx.x, r, c);
     const double* src = packed + (size_t)blockIdx.x * (TB * TB);
     for(int e = threadIdx.x; e < TB * TB; e += 256)
     {
@@ -823,13 +770,7 @@ tri_rows_kernel(DevProblem P, NormalBuffers N, int n_c, const double* __restrict
     const int t = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
     const int ntri = nx * (nx + 1) / 2;
     int ka, kb = -1;   // kb < 0: the gradient entry of column ka
-    if(t < ntri)
-    {
-        ka = (int)((sqrtf(8.f * t + 1.f) - 1.f) * 0.5f);
-        while(ka * (ka + 1) / 2 > t) ka--;
-        while((ka + 1) * (ka + 2) / 2 <= t) ka++;
-        kb = t - ka * (ka + 1) / 2;
-    }
+    if(t < ntri) tri_row_col(t, ka, kb);
     else ka = t - ntri;
     const int ca = P.i_extr0 + ka, cb = P.i_extr0 + (kb >= 0 ? kb : 0);
     const int ia = N.cidx[N.reduced_index(ca)], ib = N.cidx[N.reduced_index(cb)];
@@ -848,8 +789,7 @@ tri_rows_kernel(DevProblem P, NormalBuffers N, int n_c, const double* __restrict
         }
         sum += kb >= 0 ? va * vb : va * x[m];
     }
-#pragma unroll
-    for(int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    sum = warp_sum(sum);
     if(lane == 0) s_part[tid >> 5] = sum;
     __syncthreads();
     if(tid != 0) return;
@@ -893,13 +833,10 @@ backsub_panels_kernel(NormalBuffers N, const double* __restrict__ sol, double* _
         for(int p = 0; p < 6; p++)
             tsum[p] += Yg[(size_t)b * kYpanel + p * kYld + lane] * d0 + Yg[(size_t)b * kYpanel + p * kYld + 32 + lane] * d1;
     }
+    warp_sum(tsum);
+    if(lane == 0)
 #pragma unroll
-    for(int p = 0; p < 6; p++)
-    {
-#pragma unroll
-        for(int o = 16; o > 0; o >>= 1) tsum[p] += __shfl_xor_sync(0xffffffffu, tsum[p], o);
-        if(lane == 0) s_part[warp][p] = tsum[p];
-    }
+        for(int p = 0; p < 6; p++) s_part[warp][p] = tsum[p];
     __syncthreads();
     if(threadIdx.x < nelim)
     {

@@ -19,6 +19,7 @@
 #include "comm.h"
 #include "device_math.cuh"
 #include "problem_impl.h"
+#include "reduce.cuh"
 
 namespace mb200 {
 
@@ -36,33 +37,19 @@ __global__ void __launch_bounds__(256)
 outlier_board_stats_kernel(const double* __restrict__ pool, const double* __restrict__ x, long Nfeat, double* __restrict__ part)
 {
     __shared__ double sh[3][8];
-    double s = 0., ni = 0., no = 0.;
+    double v[3] = {0., 0., 0.};   // sum x^2 of inliers, inliers, outliers
     // contiguous chunk per block, strided by threads inside: the order of the additions is fixed
     const long per = (Nfeat + gridDim.x - 1) / gridDim.x;
     const long i0 = (long)blockIdx.x * per, i1 = min(Nfeat, i0 + per);
     for(long i = i0 + threadIdx.x; i < i1; i += blockDim.x)
     {
-        if(pool[3 * i + 2] <= 0.0) { no += 1.; continue; }   // mrcal.c:4116
+        if(pool[3 * i + 2] <= 0.0) { v[2] += 1.; continue; }   // mrcal.c:4116
         const double dx = x[2 * i], dy = x[2 * i + 1];
-        s += dx * dx + dy * dy;
-        ni += 1.;
+        v[0] += dx * dx + dy * dy;
+        v[1] += 1.;
     }
-#pragma unroll
-    for(int o = 16; o > 0; o >>= 1)
-    {
-        s += __shfl_xor_sync(0xffffffffu, s, o);
-        ni += __shfl_xor_sync(0xffffffffu, ni, o);
-        no += __shfl_xor_sync(0xffffffffu, no, o);
-    }
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if(lane == 0) { sh[0][w] = s; sh[1][w] = ni; sh[2][w] = no; }
-    __syncthreads();
-    if(threadIdx.x < 3)
-    {
-        double t = 0.;
-        for(int k = 0; k < 8; k++) t += sh[threadIdx.x][k];
-        part[3 * blockIdx.x + threadIdx.x] = t;
-    }
+    const double t = block_sum_by_warps(v, sh);
+    if(threadIdx.x < 3) part[3 * blockIdx.x + threadIdx.x] = t;
 }
 
 // Do the rays of a pair converge? The value part of mrcal_triangulate_leecivera_mid2()

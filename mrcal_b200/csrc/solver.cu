@@ -13,6 +13,7 @@
 #include <cmath>
 
 #include "comm.h"
+#include "reduce.cuh"
 #include "solver_internal.h"
 
 namespace mb200 {
@@ -72,28 +73,14 @@ dots_kernel(const double* __restrict__ a, const double* __restrict__ b, int e0, 
     // slots: head 0..2, tail 3..5, eliminated 6..8 -- the per-rank partial sums (eliminated range) come last, next to
     // the row sums the caller keeps behind them, so that ONE cross-rank reduction covers both
     out += blockIdx.x == 0 ? 0 : (blockIdx.x == 1 ? 6 : 3);
-    double s0 = 0., s1 = 0., s2 = 0.;
+    double s[3] = {0., 0., 0.};
     for(int i = i0 + threadIdx.x; i < i1; i += blockDim.x)
     {
         const double x = a[i], y = b ? b[i] : 0.;
-        s0 += x * x; s1 += y * y; s2 += x * y;
+        s[0] += x * x; s[1] += y * y; s[2] += x * y;
     }
-#pragma unroll
-    for(int o = 16; o > 0; o >>= 1)
-    {
-        s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-        s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-    }
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if(lane == 0) { r[0][w] = s0; r[1][w] = s1; r[2][w] = s2; }
-    __syncthreads();
-    if(threadIdx.x < 3)
-    {
-        double t = 0.;
-        for(int i = 0; i < (int)(blockDim.x >> 5); i++) t += r[threadIdx.x][i];
-        out[threadIdx.x] = t;
-    }
+    const double t = block_sum_by_warps(s, r, (int)(blockDim.x >> 5));
+    if(threadIdx.x < 3) out[threadIdx.x] = t;
 }
 
 // number of board corners with weight < 0 (mrcal.c:6420-6425). Integer atomics: order-independent
@@ -102,7 +89,7 @@ __global__ void count_negative_kernel(const double* __restrict__ pool, long n, i
     int c = 0;
     for(long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x)
         if(pool[3 * i + 2] < 0.0) c++;
-    for(int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    c = warp_sum(c);
     if((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
 }
 

@@ -25,6 +25,7 @@
 #include <algorithm>
 
 #include "device_math.cuh"
+#include "reduce.cuh"
 #include "solver_internal.h"
 
 namespace mb200 {
@@ -207,23 +208,17 @@ __global__ void ztz_kernel(const NormalBuffers N, const double* __restrict__ Bf,
 {
     const int pt = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if(pt >= Npts) return;
-    double s00 = 0., s01 = 0., s11 = 0.;
+    double s[3] = {0., 0., 0.};
     auto acc = [&](const double* a, const double* b, int n)
     {
-        for(int c = lane; c < n; c += 32) { const double x = a[c], y = b[c]; s00 += x * x; s01 += x * y; s11 += y * y; }
+        for(int c = lane; c < n; c += 32) { const double x = a[c], y = b[c]; s[0] += x * x; s[1] += x * y; s[2] += y * y; }
     };
     const size_t ra = 2 * (size_t)pt, rb = ra + 1;
     acc(Bf + ra * Nelim, Bf + rb * Nelim, Nelim);
     acc(Bs + ra * N.ldS, Bs + rb * N.ldS, N.n_c);
     acc(Bi + ra * nBi, Bi + rb * nBi, nBi);
-#pragma unroll
-    for(int o = 16; o > 0; o >>= 1)
-    {
-        s00 += __shfl_xor_sync(0xffffffffu, s00, o);
-        s01 += __shfl_xor_sync(0xffffffffu, s01, o);
-        s11 += __shfl_xor_sync(0xffffffffu, s11, o);
-    }
-    if(lane == 0) { V[3 * pt] = s00; V[3 * pt + 1] = s01; V[3 * pt + 2] = s11; }
+    warp_sum(s);
+    if(lane == 0) { V[3 * pt] = s[0]; V[3 * pt + 1] = s[1]; V[3 * pt + 2] = s[2]; }
 }
 
 // Var = sigma^2 (Var0 - (Jr X)'(Jr X)): one warp per point, lanes over the regularization rows. X lives in Bs / Bi
@@ -235,7 +230,7 @@ __global__ void finish_kernel(const NormalBuffers N, const double* __restrict__ 
 {
     const int pt = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if(pt >= Npts) return;
-    double s00 = 0., s01 = 0., s11 = 0.;
+    double s[3] = {0., 0., 0.};
     for(int m = m0 + lane; m < m1; m += 32)
     {
         double a = 0., b = 0.;
@@ -247,18 +242,12 @@ __global__ void finish_kernel(const NormalBuffers N, const double* __restrict__ 
             const double xb = *N.at<const double>(sl, nullptr, 0, Bs, Bi, 2 * pt + 1);
             a += Jval[e] * xa; b += Jval[e] * xb;
         }
-        s00 += a * a; s01 += a * b; s11 += b * b;
+        s[0] += a * a; s[1] += a * b; s[2] += b * b;
     }
-#pragma unroll
-    for(int o = 16; o > 0; o >>= 1)
-    {
-        s00 += __shfl_xor_sync(0xffffffffu, s00, o);
-        s01 += __shfl_xor_sync(0xffffffffu, s01, o);
-        s11 += __shfl_xor_sync(0xffffffffu, s11, o);
-    }
+    warp_sum(s);
     if(lane != 0) return;
     const double s2 = sigma[0] * sigma[0];
-    const double v00 = (V[3 * pt] - s00) * s2, v01 = (V[3 * pt + 1] - s01) * s2, v11 = (V[3 * pt + 2] - s11) * s2;
+    const double v00 = (V[3 * pt] - s[0]) * s2, v01 = (V[3 * pt + 1] - s[1]) * s2, v11 = (V[3 * pt + 2] - s[2]) * s2;
     out[4 * pt] = v00; out[4 * pt + 1] = v01; out[4 * pt + 2] = v01; out[4 * pt + 3] = v11;
 }
 
@@ -271,13 +260,7 @@ __global__ void __launch_bounds__(256) sigma_kernel(const double* __restrict__ x
     double s = 0.;
     for(int i = threadIdx.x; i < Nboard; i += 256) s += x[m_board0 + i] * x[m_board0 + i];
     for(int i = threadIdx.x; i < Npoint; i += 256) s += x[m_point0 + i] * x[m_point0 + i];
-    part[threadIdx.x] = s;
-    __syncthreads();
-    for(int o = 128; o > 0; o >>= 1)
-    {
-        if(threadIdx.x < o) part[threadIdx.x] += part[threadIdx.x + o];
-        __syncthreads();
-    }
+    tree_sum<256>(part, s);
     if(threadIdx.x == 0)
     {
         const double n = (double)(Nboard + Npoint);
