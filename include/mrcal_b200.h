@@ -612,6 +612,29 @@ bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* problem, in
                                                bool atinfinity, const mrcal_point3_t* p_cam, int N,
                                                double observed_pixel_uncertainty, double* Var, double* sigma_used);
 
+/* The same for several cameras from ONE evaluation and factorization of the problem: camera icam_intrinsics[c] gets
+   N[c] points; p_cam and Var [sum N][2][2] hold every camera's points, camera after camera. Each camera's Var is what
+   mrcal_b200_problem_projection_uncertainty() gives for it alone, bit for bit: the same kernels run in the same order.
+   The observed-pixel uncertainty is estimated once (or given) and shared. False + mrcal_b200_last_error() if the
+   method or any camera is refused, or on failure */
+bool mrcal_b200_problem_projection_uncertainty_cameras(mrcal_b200_problem_t* problem, const int* icam_intrinsics,
+                                                       const int* N, int Ncameras, int method, bool atinfinity,
+                                                       const mrcal_point3_t* p_cam, double observed_pixel_uncertainty,
+                                                       double* Var, double* sigma_used);
+
+/* Residual statistics binned by imager cell, as mrcal.calibration._report_regional_statistics() computes them
+   (mrcal/calibration.py:1720-1866), for the cameras icam_intrinsics [Ncameras] in one launch. q_cell_center
+   [Ncameras][gridn_height][gridn_width][2]: each camera's cell centres (mrcal.sample_imager()); rcell [Ncameras][2]:
+   each camera's cell half-size. A board corner counts in a cell when its observation is of that camera, its weight
+   is > 0 and its observed pixel q has |q - centre| < rcell on both axes; its weighted x and y residuals both count.
+   stats [Ncameras][gridn_height][gridn_width][3] = (mean, population stdev, count), (0, 0, count) where count <= 5.
+   evaluate: evaluate the residuals at the problem's current state first; false: use those of the last evaluation
+   (the last callback, solve or projection-uncertainty call). x [Nmeasurements] (may be NULL) receives the residuals
+   used. Sums in a fixed order: two calls give the same bits. False + mrcal_b200_last_error() on refusal or failure */
+bool mrcal_b200_problem_regional_statistics(mrcal_b200_problem_t* problem, const int* icam_intrinsics, int Ncameras,
+                                            int gridn_width, int gridn_height, const double* q_cell_center,
+                                            const double* rcell, bool evaluate, double* stats, double* x);
+
 /* The transformation implied by two cameras' intrinsics, as mrcal.implied_Rt10__from_unprojections() fits it
    (mrcal/model_analysis.py:27-395): Rt10 [4][3] (R then t; t = 0 if atinfinity) minimizing the huber-robust sum over the
    points (m, i) in the focus region (|q0[i] - focus_center|^2 < focus_radius^2) of (w[m][i] th2)^2, th2 = 2 (1 -
@@ -672,6 +695,13 @@ bool mrcal_b200_image_transformation_map(float* mapxy, int W_to, int H_to,
                                          const double* Rt_to_from, const double* distance,
                                          const double* plane_n, double plane_d,
                                          const mrcal_point2_t* region, int Nregion);
+
+/* Which of the points q [N] lie strictly inside the closed polygon region [Nregion], as
+   mrcal.is_within_valid_intrinsics_region() (shapely's Polygon.contains()) decides it: mask[i] is false for a point
+   on an edge or a vertex (an exact test for integer coordinates), for a NaN point, and for every point if Nregion is
+   0; otherwise the even-odd rule decides. Any number of vertices. One thread per point on the device. False +
+   mrcal_b200_last_error() on failure */
+bool mrcal_b200_is_within_region(bool* mask, const mrcal_point2_t* q, int N, const mrcal_point2_t* region, int Nregion);
 
 /* An image remapped through a map, as mrcal.transform_image() (cv2.remap()) computes it, pixel for pixel: out
    [H_out][W_out][channels] (packed) from image [H][W][channels] (rows image_stride bytes apart) and mapxy

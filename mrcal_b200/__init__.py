@@ -29,6 +29,11 @@ from .image_transforms import (  # noqa: F401
     INTER_NEAREST, INTER_LINEAR, BORDER_CONSTANT, BORDER_TRANSPARENT,
 )
 from .cameramodel import cameramodel, CameramodelParseException  # noqa: F401
+from .regions import (  # noqa: F401
+    measurements_board, measurements_point, residuals_board, residuals_chessboard, residuals_point,
+    close_contour, imagergrid_using, is_within_valid_intrinsics_region, valid_intrinsics_regions,
+    _report_regional_statistics, _compute_valid_intrinsics_region,
+)
 from ._capi import lib as _lib
 
 

@@ -120,7 +120,8 @@ EXPORTED_SYMBOLS = (
     "mrcal_b200_problem_time_callback",
     "mrcal_b200_problem_triangulated_outliers",
     "mrcal_b200_problem_drt_cross_reprojection__dbpacked",
-    "mrcal_b200_problem_projection_uncertainty",
+    "mrcal_b200_problem_projection_uncertainty", "mrcal_b200_problem_projection_uncertainty_cameras",
+    "mrcal_b200_problem_regional_statistics", "mrcal_b200_is_within_region",
     "mrcal_b200_implied_Rt10__from_unprojections", "mrcal_b200_projection_diff",
     "mrcal_rectified_resolution", "mrcal_rectified_system2", "mrcal_rectified_system", "mrcal_rectification_maps",
     "mrcal_stereo_range_sparse", "mrcal_stereo_range_dense", "mrcal_b200_stereo_unproject",
@@ -169,6 +170,15 @@ lib.mrcal_b200_problem_drt_cross_reprojection__dbpacked.argtypes = [C.c_void_p, 
 lib.mrcal_b200_problem_projection_uncertainty.restype = C.c_bool
 lib.mrcal_b200_problem_projection_uncertainty.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_bool, C.c_void_p, C.c_int,
                                                            C.c_double, C.c_void_p, C.c_void_p]
+lib.mrcal_b200_problem_projection_uncertainty_cameras.restype = C.c_bool
+lib.mrcal_b200_problem_projection_uncertainty_cameras.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                                   C.c_bool, C.c_void_p, C.c_double, C.c_void_p,
+                                                                   C.c_void_p]
+lib.mrcal_b200_problem_regional_statistics.restype = C.c_bool
+lib.mrcal_b200_problem_regional_statistics.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                                       C.c_void_p, C.c_bool, C.c_void_p, C.c_void_p]
+lib.mrcal_b200_is_within_region.restype = C.c_bool
+lib.mrcal_b200_is_within_region.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
 lib.mrcal_b200_implied_Rt10__from_unprojections.restype = C.c_bool
 lib.mrcal_b200_implied_Rt10__from_unprojections.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
                                                              C.c_void_p, C.c_void_p, C.c_bool, C.c_void_p, C.c_double]

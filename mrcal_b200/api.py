@@ -753,6 +753,51 @@ class Problem:
             raise RuntimeError("projection_uncertainty: " + _capi.last_error())
         return Var, sigma.value
 
+    def projection_uncertainty_cameras(self, p_cams, icams_intrinsics, method="cross-reprojection-ccp", atinfinity=False,
+                                       observed_pixel_uncertainty=None):
+        """([Var], sigma): projection_uncertainty() of the points p_cams[k] (N_k,3) by camera icams_intrinsics[k], for
+        every k from one evaluation and factorization of the problem. Each Var equals what projection_uncertainty()
+        gives for that camera alone, bit for bit"""
+        if method not in _UNCERTAINTY_METHODS:
+            raise RuntimeError(f"Unknown uncertainty method: '{method}'. I know about {set(_UNCERTAINTY_METHODS)}")
+        if len(p_cams) != len(icams_intrinsics):
+            raise RuntimeError("p_cams and icams_intrinsics must have the same length")
+        ps = [np.ascontiguousarray(p, np.float64) for p in p_cams]
+        for p in ps:
+            if p.ndim != 2 or p.shape[1] != 3:
+                raise RuntimeError(f"each p_cam must have shape (N,3); got {p.shape}")
+        N = np.array([p.shape[0] for p in ps], np.int32)
+        icams = np.array(icams_intrinsics, np.int32).reshape(-1)
+        p_all = np.ascontiguousarray(np.concatenate(ps) if ps else np.zeros((0, 3)))
+        Var = np.zeros((p_all.shape[0], 2, 2))
+        sigma = C.c_double(0.)
+        s = -1.0 if observed_pixel_uncertainty is None else float(observed_pixel_uncertainty)
+        if observed_pixel_uncertainty is not None and not s > 0:
+            raise RuntimeError("observed_pixel_uncertainty must be > 0 (or None to estimate it)")
+        if not lib.mrcal_b200_problem_projection_uncertainty_cameras(self._h, _ptr(icams), _ptr(N), len(ps),
+                                                                    _UNCERTAINTY_METHODS[method], bool(atinfinity),
+                                                                    _ptr(p_all), s, _ptr(Var), C.byref(sigma)):
+            raise RuntimeError("projection_uncertainty: " + _capi.last_error())
+        return np.split(Var, np.cumsum(N)[:-1]), sigma.value
+
+    def regional_statistics(self, icams_intrinsics, q_cell_center, rcell, evaluate=True):
+        """(stats, x): the board residuals binned by imager cell for the cameras icams_intrinsics, one grid shape for
+        all: stats (Ncameras, gridn_height, gridn_width, 3) of (mean, stdev, count), from the cell centres
+        q_cell_center (Ncameras, gridn_height, gridn_width, 2) and half-sizes rcell (Ncameras, 2); x the residuals used.
+        evaluate=False uses the residuals of the last evaluation (csrc/regions.cu)"""
+        icams = np.array(icams_intrinsics, np.int32).reshape(-1)
+        q = np.ascontiguousarray(q_cell_center, np.float64)
+        r = np.ascontiguousarray(rcell, np.float64)
+        if q.ndim != 4 or q.shape[0] != icams.size or q.shape[-1] != 2 or r.shape != (icams.size, 2):
+            raise RuntimeError(f"q_cell_center must have shape (Ncameras,Nh,Nw,2) and rcell (Ncameras,2); got "
+                               f"{q.shape} and {r.shape} for {icams.size} cameras")
+        stats = np.zeros(q.shape[:-1] + (3,))
+        x = np.zeros(self.Nmeasurements)
+        if not lib.mrcal_b200_problem_regional_statistics(self._h, _ptr(icams), icams.size, q.shape[2], q.shape[1],
+                                                          _ptr(q), _ptr(r), bool(evaluate), _ptr(stats), _ptr(x)):
+            raise RuntimeError("regional_statistics: " + _capi.last_error())
+        return stats, x
+
     def callback(self, jacobian=True):
         b = np.zeros(self.Nstate)
         x = np.zeros(self.Nmeasurements)

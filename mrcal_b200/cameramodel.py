@@ -221,8 +221,19 @@ class cameramodel:
     extrinsics_rt_fromref = rt_cam_ref
     extrinsics_rt_toref = rt_ref_cam
 
-    def valid_intrinsics_region(self):
-        return None if self._valid_intrinsics_region is None else self._valid_intrinsics_region.copy()
+    def valid_intrinsics_region(self, valid_intrinsics_region=None):
+        """The valid-intrinsics region (N,2), or None if the model has none. Given a region, sets it instead (a copy),
+        closing an open contour first, and returns True: it must be (N,2) with N >= 4 once closed, or (0,2) for "valid
+        nowhere" (mrcal/cameramodel.py:1820-1865)"""
+        if valid_intrinsics_region is None:
+            return None if self._valid_intrinsics_region is None else self._valid_intrinsics_region.copy()
+        from .regions import close_contour
+        r = close_contour(np.array(valid_intrinsics_region))
+        if not (r.ndim == 2 and r.shape[1] == 2 and (r.shape[0] >= 4 or r.shape[0] == 0)):
+            raise RuntimeError("The valid-intrinsics region must be a numpy array of shape (N,2) with N >= 4 or N == 0. "
+                               f"Instead got shape {r.shape}")
+        self._valid_intrinsics_region = np.array(r, dtype=float)
+        return True
 
     def optimization_inputs(self):
         if self._optimization_inputs_string is None:

@@ -12,6 +12,7 @@
 #include "common.h"
 #include "device_math.cuh"
 #include "lens_dispatch.cuh"
+#include "polygon.cuh"
 #include "problem_impl.h"
 #include "unproject.cuh"
 
@@ -53,15 +54,6 @@ __global__ void reprojection_rays_kernel(LensArgs a, bool behind_ok, RayTransfor
         ray[3 * k + r] = T.M[3 * r] * v[0] + T.M[3 * r + 1] * v[1] + T.M[3 * r + 2] * v[2] + T.c[r];
 }
 
-// even-odd crossing number of the closed polygon P[N] around (x, y). A NaN point crosses nothing: outside
-__device__ __forceinline__ bool inside_polygon(double x, double y, const double2* P, int N)
-{
-    bool c = false;
-    for(int i = 0, j = N - 1; i < N; j = i++)
-        if((P[i].y > y) != (P[j].y > y) && x < (P[j].x - P[i].x) * (y - P[i].y) / (P[j].y - P[i].y) + P[i].x) c = !c;
-    return c;
-}
-
 // map[k] = project_from(ray[k]) as a float32 pair; (-1, -1) outside the region, if one is given (Nregion > 0)
 template <int KIND>
 __global__ void reprojection_map_kernel(LensArgs a, const double* __restrict__ ray, long Npix,
@@ -77,6 +69,41 @@ __global__ void reprojection_map_kernel(LensArgs a, const double* __restrict__ r
     project_any<KIND>(q, g, p, a);
     if(Nregion > 0 && !inside_polygon(q[0], q[1], poly, Nregion)) { q[0] = -1.; q[1] = -1.; }
     map[k] = make_float2((float)q[0], (float)q[1]);
+}
+
+////////////////////////////////////////////////////////////////////////////////
+// is_within_valid_intrinsics_region(): the strict test
+////////////////////////////////////////////////////////////////////////////////
+
+// vertices per shared-memory tile of the strict test (16 KB of double2)
+constexpr int kRegionTile = 1024;
+
+// mask[k]: q[k] lies strictly inside the region: on none of its edges, and inside by the even-odd rule. The vertices
+// go through shared memory a tile at a time, slot 0 of a tile holding the vertex before the tile's first, so that a
+// region of any size is accepted. The parity is the same whatever the order of the edges
+__global__ void __launch_bounds__(256) within_region_kernel(const double2* __restrict__ q, long N,
+                                                            const double2* __restrict__ region, int Nregion,
+                                                            bool* __restrict__ mask)
+{
+    __shared__ double2 tile[kRegionTile + 1];
+    const long k = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    const double2 p = k < N ? q[k] : make_double2(NAN, NAN);
+    bool in = false, edge = false;
+    for(int t0 = 0; t0 < Nregion; t0 += kRegionTile)
+    {
+        const int n = min(kRegionTile, Nregion - t0);
+        __syncthreads();
+        for(int r = threadIdx.x; r <= n; r += blockDim.x)
+            tile[r] = region[r > 0 ? t0 + r - 1 : (t0 > 0 ? t0 - 1 : Nregion - 1)];
+        __syncthreads();
+        for(int i = 1; i <= n; i++)
+        {
+            const double2 a = tile[i], b = tile[i - 1];
+            edge = edge || on_segment(p.x, p.y, a, b);
+            if(edge_crosses(p.x, p.y, a, b)) in = !in;
+        }
+    }
+    if(k < N) mask[k] = in && !edge;
 }
 
 ////////////////////////////////////////////////////////////////////////////////
@@ -384,6 +411,28 @@ extern "C" bool mrcal_b200_image_transformation_map(float* mapxy, int W_to, int 
     })) return false;
     MB200_CUDA_CHECK(cudaGetLastError());
     MB200_CUDA_CHECK(cudaMemcpyAsync(mapxy, d_map, Npix * sizeof(float2), cudaMemcpyDeviceToHost, S.s));
+    MB200_CUDA_CHECK(cudaStreamSynchronize(S.s));
+    return true;
+}
+
+extern "C" bool mrcal_b200_is_within_region(bool* mask, const mrcal_point2_t* q, int N, const mrcal_point2_t* region,
+                                            int Nregion)
+{
+    if(N < 0 || Nregion < 0) { set_error("is_within_region: N = %d and Nregion = %d must be >= 0", N, Nregion); return false; }
+    if(N == 0) return true;
+    if(!have_device()) return false;
+    DeviceArena mem;   // freed after the stream has drained
+    Stream S;
+    MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
+    double *d_q, *d_region;
+    bool* d_mask;
+    if(!upload(mem, &d_q, (const double*)q, 2 * (size_t)N, S.s) ||
+       !upload(mem, &d_region, (const double*)region, 2 * (size_t)Nregion, S.s) || !mem.alloc(&d_mask, (size_t)N))
+        return false;
+    within_region_kernel<<<(unsigned)((N + 255) / 256), 256, 0, S.s>>>((const double2*)d_q, N, (const double2*)d_region,
+                                                                       Nregion, d_mask);
+    MB200_CUDA_CHECK(cudaGetLastError());
+    MB200_CUDA_CHECK(cudaMemcpyAsync(mask, d_mask, (size_t)N * sizeof(bool), cudaMemcpyDeviceToHost, S.s));
     MB200_CUDA_CHECK(cudaStreamSynchronize(S.s));
     return true;
 }

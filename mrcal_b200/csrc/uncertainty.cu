@@ -23,6 +23,7 @@
 // tiles of kSolveTile right-hand sides when there are many. The 2x2 per point is reduced by one warp in a fixed order:
 // no atomics anywhere, two calls give bit-identical results.
 #include <algorithm>
+#include <vector>
 
 #include "device_math.cuh"
 #include "reduce.cuh"
@@ -307,6 +308,171 @@ bool camera_extrinsics(const mrcal_b200_problem* P, int icam, int* e_first, int*
     return true;
 }
 
+// What the reference refuses whatever the camera, for a known method (model_analysis.py:727-734, 1447-1452, 901-902)
+bool uncertainty_method_ok(const mrcal_b200_problem* P, int method)
+{
+    const Layout& L = P->L;
+    const DevProblem& dp = P->dp;
+    if(dp.Ntri > 0) { set_error("Some measurements other than boards, points and regularization are present. Don't know what to do"); return false; }
+    if(L.Nmeas_board + L.Nmeas_point == 0)
+    { set_error("observed_pixel_uncertainty cannot be computed because we don't have any board or point observations"); return false; }
+    if(L.Nmeas_reg > 0 && L.Nmeas_board + L.Nmeas_point == 0) { set_error("No non-regularization measurements. Don't know what to do"); return false; }
+    if(method == MRCAL_B200_UNCERTAINTY_MEAN_PCAM && dp.opt_frames && dp.Nobs_point > 0)
+    { set_error("We have point observations that we are optimizing; only cross-reprojection uncertainty can work here. Have method='mean-pcam'"); return false; }
+    return true;
+}
+
+// One camera's query points: what the reference refuses for it (model_analysis.py:1460-1483), and its extrinsics
+struct CameraQuery
+{
+    int icam, Npts;
+    int e_first = -1, Ne = 0;
+    size_t p0 = 0;   // its first point among all the cameras' points
+};
+bool camera_query_ok(const mrcal_b200_problem* P, int method, CameraQuery* Q)
+{
+    // (ccp does not look at the camera's extrinsics: model_analysis.py:1347-1417 returns before that)
+    if(method != MRCAL_B200_UNCERTAINTY_CCP && !camera_extrinsics(P, Q->icam, &Q->e_first, &Q->Ne)) return false;
+    if(method == MRCAL_B200_UNCERTAINTY_RRP_JFP && Q->Ne > 1) { set_error("I only handle stationary cameras for now"); return false; }
+    return true;
+}
+
+// The part every camera shares: the Jacobian at the current state, the structured factor of JtJ, and sigma
+struct UncertaintyFactor
+{
+    mrcal_b200_factorization F;   // its buffers only: it does not own the problem here
+    DeviceArena mem;
+    double* sigma = nullptr;
+    int* bad = nullptr;
+    double* K = nullptr;          // [6][Nstate] for the cross-reprojection methods
+    int c0K = 0;                  // the first column K can be nonzero in
+};
+bool uncertainty_factor(mrcal_b200_problem* P, int method, double observed_pixel_uncertainty, UncertaintyFactor* U)
+{
+    const Layout& L = P->L;
+    const DevProblem& dp = P->dp;
+    U->F.P = P;
+    if(!schur_factor_build(P, &U->F)) return false;
+    if(!U->mem.alloc(&U->sigma, 1) || !U->mem.alloc(&U->bad, 1, true)) return false;
+    U->c0K = L.Nstate;
+    if(method != MRCAL_B200_UNCERTAINTY_MEAN_PCAM)
+    {
+        if(!U->mem.alloc(&U->K, (size_t)6 * L.Nstate)) return false;
+        for(int c : {dp.i_extr0, dp.i_frame0, dp.i_point0, dp.i_warp0}) if(c >= 0 && c < U->c0K) U->c0K = c;
+    }
+    const EvalBuffers& op = P->op[P->cur];
+    sigma_kernel<<<1, 256, 0, P->stream>>>(op.x, L.m_board0, L.Nmeas_board, L.m_point0, L.Nmeas_point, L.Nstate,
+                                           observed_pixel_uncertainty, U->sigma);
+    return true;
+}
+
+// The points in a chunk of the solves: as many as a fixed memory budget holds, at most Npts
+int uncertainty_chunk(const UncertaintyFactor& U, const NormalBuffers& N, int Npts)
+{
+    const size_t per_rhs = (size_t)(U.F.Nelim > 0 ? U.F.Nelim : 1) + N.ldS + (N.n_r > 0 ? N.n_r : 1);
+    const size_t budget = (size_t)512 << 20;
+    int chunk = (int)(budget / (2 * per_rhs * sizeof(double)));
+    chunk = chunk < kSolveTile ? kSolveTile : (chunk / kSolveTile) * kSolveTile;
+    return chunk > Npts ? Npts : chunk;
+}
+
+// Var of one camera's points pts [Npts][3] (device) into out [Npts][2][2] (device): its rows, the solves and the
+// 2x2 reductions, chunk points at a time. Bf .. V hold a chunk
+bool uncertainty_camera(mrcal_b200_problem* P, const UncertaintyFactor& U, int method, bool atinfinity,
+                        const CameraQuery& Q, const double* pts, double* Bf, double* Bs, double* Bi, double* G,
+                        double* V, double* out)
+{
+    const Layout& L = P->L;
+    const DevProblem& dp = P->dp;
+    const NormalBuffers N = P->ws->N;
+    const int Nelim = U.F.Nelim, nBi = N.n_r, Nstate = L.Nstate;
+    const EvalBuffers& op = P->op[P->cur];
+    cudaStream_t s = P->stream;
+    // K of the cross-reprojection methods (the Jacobian was evaluated by the factorization)
+    if(U.K && !cross_reprojection_K(P, method == MRCAL_B200_UNCERTAINTY_CCP ? Q.icam : -1, false, U.K)) return false;
+
+    RowArgs A{};
+    A.method = method; A.atinfinity = atinfinity; A.icam = Q.icam; A.e_first = Q.e_first; A.Ne = Q.Ne;
+    A.intr_col0 = (dp.i_intr0 >= 0 && dp.Nintr_state > 0) ? dp.i_intr0 + Q.icam * dp.Nintr_state : -1;
+    A.intr_arg0 = dp.opt_core ? 0 : 4;
+    A.Nelim = Nelim;
+    A.scale = P->d_scale;
+
+    const int chunk = uncertainty_chunk(U, N, Q.Npts);
+    const bool reg = L.Nmeas_reg > 0;
+    for(int p0 = 0; p0 < Q.Npts; p0 += chunk)
+    {
+        const int np = Q.Npts - p0 < chunk ? Q.Npts - p0 : chunk, nr = 2 * np;
+        MB200_CUDA_CHECK(cudaMemsetAsync(Bf, 0, (size_t)nr * (Nelim > 0 ? Nelim : 1) * sizeof(double), s));
+        MB200_CUDA_CHECK(cudaMemsetAsync(Bs, 0, (size_t)nr * N.ldS * sizeof(double), s));
+        MB200_CUDA_CHECK(cudaMemsetAsync(Bi, 0, (size_t)nr * (nBi > 0 ? nBi : 1) * sizeof(double), s));
+        if(!launch_rows(dp, N, A, pts + 3 * (size_t)p0, np, Bf, Bs, Bi, U.K ? G : nullptr, s)) return false;
+        if(U.K && U.c0K < Nstate)
+        {
+            const long tot = (long)nr * (Nstate - U.c0K);
+            uncertainty_K_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, s>>>(N, Nelim, G, U.K, Nstate, U.c0K, nr, Bf, Bs, Bi);
+        }
+        // Z = inv(L) P dF'
+        if(!schur_solve_pieces(&U.F, Bf, Bs, Bi, nr, true, BackSolve::none, s)) return false;
+        ztz_kernel<<<(unsigned)((np * 32 + 255) / 256), 256, 0, s>>>(N, Bf, Nelim, Bs, Bi, nBi, np, V);
+        // X on the shared unknowns = inv(L_S') Z_s, inv(L_I') Z_i
+        if(reg && !schur_solve_pieces(&U.F, Bf, Bs, Bi, nr, false, BackSolve::shared, s)) return false;
+        finish_kernel<<<(unsigned)((np * 32 + 255) / 256), 256, 0, s>>>(N, Bs, Bi, P->d_rowptr, op.Jcol, op.Jval, L.m_reg0,
+                                                                         reg ? L.m_reg0 + L.Nmeas_reg : L.m_reg0, np, V, U.sigma,
+                                                                         out + 4 * (size_t)p0, U.bad);
+        MB200_CUDA_CHECK(cudaGetLastError());
+    }
+    return true;
+}
+
+// Var of the cameras Q[Ncams] from one factorization: p_cam and Var hold every camera's points, camera after camera
+bool uncertainty_cameras(mrcal_b200_problem* P, int method, bool atinfinity, std::vector<CameraQuery>& Q,
+                         const mrcal_point3_t* p_cam, double observed_pixel_uncertainty, double* Var, double* sigma_used)
+{
+    if(method < MRCAL_B200_UNCERTAINTY_MEAN_PCAM || method > MRCAL_B200_UNCERTAINTY_CCP)
+    { set_error("Unknown uncertainty method %d", method); return false; }
+    for(const CameraQuery& q : Q)
+    {
+        if(q.icam < 0 || q.icam >= P->dp.Ncam_i) { set_error("icam_intrinsics = %d is out of range", q.icam); return false; }
+        if(q.Npts < 0) { set_error("projection_uncertainty: N < 0"); return false; }
+    }
+    if(!uncertainty_method_ok(P, method)) return false;
+    size_t Ntotal = 0;
+    for(CameraQuery& q : Q)
+    {
+        if(!camera_query_ok(P, method, &q)) return false;
+        q.p0 = Ntotal;
+        Ntotal += (size_t)q.Npts;
+    }
+    cudaStream_t s = P->stream;
+    UncertaintyFactor U;
+    if(!uncertainty_factor(P, method, observed_pixel_uncertainty, &U)) return false;
+    if(Ntotal > 0)
+    {
+        const NormalBuffers N = P->ws->N;
+        int maxchunk = 0;
+        for(const CameraQuery& q : Q) maxchunk = std::max(maxchunk, uncertainty_chunk(U, N, q.Npts));
+        const int maxrhs = 2 * maxchunk, Nelim = U.F.Nelim, nBi = N.n_r;
+        DeviceArena& mem = U.mem;
+        double *Bf, *Bs, *Bi, *G, *pts, *V, *out;
+        if(!mem.alloc(&Bf, (size_t)maxrhs * (Nelim > 0 ? Nelim : 1)) || !mem.alloc(&Bs, (size_t)maxrhs * N.ldS) ||
+           !mem.alloc(&Bi, (size_t)maxrhs * (nBi > 0 ? nBi : 1)) || !mem.alloc(&G, (size_t)maxrhs * 6) ||
+           !mem.alloc(&pts, 3 * Ntotal) || !mem.alloc(&V, (size_t)3 * maxchunk) || !mem.alloc(&out, 4 * Ntotal))
+            return false;
+        MB200_CUDA_CHECK(cudaMemcpyAsync(pts, p_cam, 3 * Ntotal * sizeof(double), cudaMemcpyHostToDevice, s));
+        for(const CameraQuery& q : Q)
+            if(q.Npts > 0 && !uncertainty_camera(P, U, method, atinfinity, q, pts + 3 * q.p0, Bf, Bs, Bi, G, V, out + 4 * q.p0))
+                return false;
+        MB200_CUDA_CHECK(cudaMemcpyAsync(Var, out, 4 * Ntotal * sizeof(double), cudaMemcpyDeviceToHost, s));
+    }
+    int h_bad = 0;
+    MB200_CUDA_CHECK(cudaMemcpyAsync(&h_bad, U.bad, sizeof(int), cudaMemcpyDeviceToHost, s));
+    if(sigma_used) MB200_CUDA_CHECK(cudaMemcpyAsync(sigma_used, U.sigma, sizeof(double), cudaMemcpyDeviceToHost, s));
+    MB200_CUDA_CHECK(cudaStreamSynchronize(s));
+    if(h_bad) { set_error("projection_uncertainty: a regularization term touches an eliminated unknown"); return false; }
+    return true;
+}
+
 }  // namespace
 }  // namespace mb200
 using namespace mb200;
@@ -317,102 +483,21 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
 {
     if(mrcal_b200_device_count() <= 0) { set_error("no usable CUDA device: libmrcal_b200 has no CPU fallback"); return false; }
     if(P == nullptr) { set_error("projection_uncertainty: no problem"); return false; }
-    const Layout& L = P->L;
-    const DevProblem& dp = P->dp;
-    if(method < MRCAL_B200_UNCERTAINTY_MEAN_PCAM || method > MRCAL_B200_UNCERTAINTY_CCP)
-    { set_error("Unknown uncertainty method %d", method); return false; }
-    if(icam < 0 || icam >= dp.Ncam_i) { set_error("icam_intrinsics = %d is out of range", icam); return false; }
-    if(Npts < 0) { set_error("projection_uncertainty: N < 0"); return false; }
-    // what the reference refuses (model_analysis.py:727-734, 1447-1452, 1460-1483, 901-902)
-    if(dp.Ntri > 0) { set_error("Some measurements other than boards, points and regularization are present. Don't know what to do"); return false; }
-    if(L.Nmeas_board + L.Nmeas_point == 0)
-    { set_error("observed_pixel_uncertainty cannot be computed because we don't have any board or point observations"); return false; }
-    if(L.Nmeas_reg > 0 && L.Nmeas_board + L.Nmeas_point == 0) { set_error("No non-regularization measurements. Don't know what to do"); return false; }
-    if(method == MRCAL_B200_UNCERTAINTY_MEAN_PCAM && dp.opt_frames && dp.Nobs_point > 0)
-    { set_error("We have point observations that we are optimizing; only cross-reprojection uncertainty can work here. Have method='mean-pcam'"); return false; }
-    // (ccp does not look at the camera's extrinsics: model_analysis.py:1347-1417 returns before that)
-    int e_first = -1, Ne = 0;
-    if(method != MRCAL_B200_UNCERTAINTY_CCP && !camera_extrinsics(P, icam, &e_first, &Ne)) return false;
-    if(method == MRCAL_B200_UNCERTAINTY_RRP_JFP && Ne > 1) { set_error("I only handle stationary cameras for now"); return false; }
+    std::vector<CameraQuery> Q(1);
+    Q[0].icam = icam; Q[0].Npts = Npts;
+    return uncertainty_cameras(P, method, atinfinity, Q, p_cam, observed_pixel_uncertainty, Var, sigma_used);
+}
 
-    cudaStream_t s = P->stream;
-    // 1-2. the Jacobian at the current state, and the structured factor
-    DeviceArena mem;
-    mrcal_b200_factorization F;   // its buffers only: it does not own P here
-    F.P = P;
-    const EvalBuffers& op = P->op[P->cur];
-    const int Nstate = L.Nstate;
-    if(!schur_factor_build(P, &F)) return false;
-    const NormalBuffers N = P->ws->N;
-    const int Nelim = F.Nelim;
-    const int nBi = N.n_r;
-    // 3. K, if the method needs it (the Jacobian was evaluated above)
-    double *K = nullptr, *sigma = nullptr;
-    int* bad = nullptr;
-    if(!mem.alloc(&sigma, 1) || !mem.alloc(&bad, 1, true)) return false;
-    int c0K = Nstate;
-    if(method != MRCAL_B200_UNCERTAINTY_MEAN_PCAM)
-    {
-        if(!mem.alloc(&K, (size_t)6 * Nstate) ||
-           !cross_reprojection_K(P, method == MRCAL_B200_UNCERTAINTY_CCP ? icam : -1, false, K)) return false;
-        for(int c : {dp.i_extr0, dp.i_frame0, dp.i_point0, dp.i_warp0}) if(c >= 0 && c < c0K) c0K = c;
-    }
-    sigma_kernel<<<1, 256, 0, s>>>(op.x, L.m_board0, L.Nmeas_board, L.m_point0, L.Nmeas_point, Nstate, observed_pixel_uncertainty, sigma);
-    if(Npts == 0)
-    {
-        if(sigma_used) { MB200_CUDA_CHECK(cudaMemcpyAsync(sigma_used, sigma, sizeof(double), cudaMemcpyDeviceToHost, s)); }
-        MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-        return true;
-    }
-
-    RowArgs A{};
-    A.method = method; A.atinfinity = atinfinity; A.icam = icam; A.e_first = e_first; A.Ne = Ne;
-    A.intr_col0 = (dp.i_intr0 >= 0 && dp.Nintr_state > 0) ? dp.i_intr0 + icam * dp.Nintr_state : -1;
-    A.intr_arg0 = dp.opt_core ? 0 : 4;
-    A.Nelim = Nelim;
-    A.scale = P->d_scale;
-
-    // 4-6 in chunks of points under a fixed memory budget
-    const size_t per_rhs = (size_t)(Nelim > 0 ? Nelim : 1) + N.ldS + (nBi > 0 ? nBi : 1);
-    const size_t budget = (size_t)512 << 20;
-    int chunk = (int)(budget / (2 * per_rhs * sizeof(double)));
-    chunk = chunk < kSolveTile ? kSolveTile : (chunk / kSolveTile) * kSolveTile;
-    if(chunk > Npts) chunk = Npts;
-    const int maxrhs = 2 * chunk;
-    double *Bf, *Bs, *Bi, *G, *pts, *V, *out;
-    if(!mem.alloc(&Bf, (size_t)maxrhs * (Nelim > 0 ? Nelim : 1)) || !mem.alloc(&Bs, (size_t)maxrhs * N.ldS) ||
-       !mem.alloc(&Bi, (size_t)maxrhs * (nBi > 0 ? nBi : 1)) || !mem.alloc(&G, (size_t)maxrhs * 6) ||
-       !mem.alloc(&pts, (size_t)3 * Npts) || !mem.alloc(&V, (size_t)3 * chunk) || !mem.alloc(&out, (size_t)4 * Npts))
-        return false;
-    MB200_CUDA_CHECK(cudaMemcpyAsync(pts, p_cam, (size_t)3 * Npts * sizeof(double), cudaMemcpyHostToDevice, s));
-    const bool reg = L.Nmeas_reg > 0;
-    for(int p0 = 0; p0 < Npts; p0 += chunk)
-    {
-        const int np = Npts - p0 < chunk ? Npts - p0 : chunk, nr = 2 * np;
-        MB200_CUDA_CHECK(cudaMemsetAsync(Bf, 0, (size_t)nr * (Nelim > 0 ? Nelim : 1) * sizeof(double), s));
-        MB200_CUDA_CHECK(cudaMemsetAsync(Bs, 0, (size_t)nr * N.ldS * sizeof(double), s));
-        MB200_CUDA_CHECK(cudaMemsetAsync(Bi, 0, (size_t)nr * (nBi > 0 ? nBi : 1) * sizeof(double), s));
-        if(!launch_rows(dp, N, A, pts + 3 * (size_t)p0, np, Bf, Bs, Bi, K ? G : nullptr, s)) return false;
-        if(K && c0K < Nstate)
-        {
-            const long tot = (long)nr * (Nstate - c0K);
-            uncertainty_K_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, s>>>(N, Nelim, G, K, Nstate, c0K, nr, Bf, Bs, Bi);
-        }
-        // Z = inv(L) P dF'
-        if(!schur_solve_pieces(&F, Bf, Bs, Bi, nr, true, BackSolve::none, s)) return false;
-        ztz_kernel<<<(unsigned)((np * 32 + 255) / 256), 256, 0, s>>>(N, Bf, Nelim, Bs, Bi, nBi, np, V);
-        // X on the shared unknowns = inv(L_S') Z_s, inv(L_I') Z_i
-        if(reg && !schur_solve_pieces(&F, Bf, Bs, Bi, nr, false, BackSolve::shared, s)) return false;
-        finish_kernel<<<(unsigned)((np * 32 + 255) / 256), 256, 0, s>>>(N, Bs, Bi, P->d_rowptr, op.Jcol, op.Jval, L.m_reg0,
-                                                                         reg ? L.m_reg0 + L.Nmeas_reg : L.m_reg0, np, V, sigma,
-                                                                         out + 4 * (size_t)p0, bad);
-        MB200_CUDA_CHECK(cudaGetLastError());
-    }
-    int h_bad = 0;
-    MB200_CUDA_CHECK(cudaMemcpyAsync(Var, out, (size_t)4 * Npts * sizeof(double), cudaMemcpyDeviceToHost, s));
-    MB200_CUDA_CHECK(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, s));
-    if(sigma_used) MB200_CUDA_CHECK(cudaMemcpyAsync(sigma_used, sigma, sizeof(double), cudaMemcpyDeviceToHost, s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-    if(h_bad) { set_error("projection_uncertainty: a regularization term touches an eliminated unknown"); return false; }
-    return true;
+extern "C" bool mrcal_b200_problem_projection_uncertainty_cameras(mrcal_b200_problem_t* P, const int* icam_intrinsics,
+                                                                  const int* N, int Ncameras, int method, bool atinfinity,
+                                                                  const mrcal_point3_t* p_cam,
+                                                                  double observed_pixel_uncertainty, double* Var,
+                                                                  double* sigma_used)
+{
+    if(mrcal_b200_device_count() <= 0) { set_error("no usable CUDA device: libmrcal_b200 has no CPU fallback"); return false; }
+    if(P == nullptr) { set_error("projection_uncertainty: no problem"); return false; }
+    if(Ncameras < 0) { set_error("projection_uncertainty: Ncameras < 0"); return false; }
+    std::vector<CameraQuery> Q(Ncameras);
+    for(int c = 0; c < Ncameras; c++) { Q[c].icam = icam_intrinsics[c]; Q[c].Npts = N[c]; }
+    return uncertainty_cameras(P, method, atinfinity, Q, p_cam, observed_pixel_uncertainty, Var, sigma_used);
 }
