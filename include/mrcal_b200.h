@@ -722,6 +722,31 @@ bool mrcal_b200_transform_image_device(void* out, const void* image, int W, int 
                                        int channels, const float* mapxy, int W_out, int H_out, int interpolation,
                                        int border_mode, const double* border_value, void* stream);
 
+/* Template matching for M features in one call, as mrcal.match_feature() computes it with cv2.matchTemplate(): the
+   device part, after the host has decided which features can be matched. image0 [H0][W0] and image1 [H1][W1] (rows
+   stride0, stride1 bytes apart) are both MRCAL_B200_IMAGE_UINT8 or both MRCAL_B200_IMAGE_FLOAT. Feature i is
+   features[6i..6i+5] = (tx, ty, cx, cy, cw, ch): its template's top-left pixel in image 1 and its search cut of image
+   1, cw x ch pixels at (cx, cy), inside image 1 and at least template_w x template_h; and Hinv[9i..9i+8], the float32
+   inverse of its homography H10 (row-major). The template is image0 remapped (INTER_LINEAR, BORDER_CONSTANT 0) through
+   apply_homography(Hinv, q1) of the template's pixels q1; its match output has (ch - template_h + 1) rows of
+   (cw - template_w + 1) values of method (OpenCV's TM_* values, 0..5). out: M rows of 4 doubles (the sub-pixel
+   optimum's x and y in match-output coordinates and its value, NaN unless the status is MRCAL_B200_MATCH_OK; the
+   status), then M slots of slot_w * slot_h float32, each starting with its feature's packed match output. No output
+   may exceed its slot. templates: NULL, or M * template_h * template_w elements of the image type. False +
+   mrcal_b200_last_error() on refusal or failure */
+enum { MRCAL_B200_MATCH_OK = 0, MRCAL_B200_MATCH_EDGE_PEAK = 1, MRCAL_B200_MATCH_OUTSIDE_IMAGE1 = 2,
+       MRCAL_B200_MATCH_OUTSIDE_IMAGE0 = 3, MRCAL_B200_MATCH_SEARCH_TOO_SMALL = 4 };
+bool mrcal_b200_match_feature(double* out, void* templates, const void* image0, int W0, int H0, int stride0,
+                              const void* image1, int W1, int H1, int stride1, int type, const int* features,
+                              const float* Hinv, int M, int template_w, int template_h, int slot_w, int slot_h,
+                              int method);
+/* The same with image0 and image1 on the device, aligned to their element: the work is enqueued on stream (a
+   cudaStream_t; NULL: the default stream), and the call returns once out and templates (host memory) are written */
+bool mrcal_b200_match_feature_device(double* out, void* templates, const void* image0, int W0, int H0, int stride0,
+                                     const void* image1, int W1, int H1, int stride1, int type, const int* features,
+                                     const float* Hinv, int M, int template_w, int template_h, int slot_w, int slot_h,
+                                     int method, void* stream);
+
 // Timing hook for benchmarks: run N cost-function evaluations (residuals +
 // Jacobian) at the current state back to back, return the mean device time per
 // evaluation in milliseconds (CUDA events on the library's stream); <0 on error

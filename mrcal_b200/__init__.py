@@ -23,6 +23,9 @@ from .seeding import (  # noqa: F401
 )
 from .stereo import (  # noqa: F401
     rectified_resolution, rectified_system, rectification_maps, stereo_range, stereo_unproject,
+    apply_homography, match_feature,
+    TM_SQDIFF, TM_SQDIFF_NORMED, TM_CCORR, TM_CCORR_NORMED, TM_CCOEFF, TM_CCOEFF_NORMED,
+    MATCH_OK, MATCH_EDGE_PEAK, MATCH_OUTSIDE_IMAGE1, MATCH_OUTSIDE_IMAGE0, MATCH_SEARCH_TOO_SMALL,
 )
 from .image_transforms import (  # noqa: F401
     scale_focal__best_pinhole_fit, pinhole_model_for_reprojection, image_transformation_map, transform_image,

@@ -14,6 +14,7 @@
 #include "lens_dispatch.cuh"
 #include "polygon.cuh"
 #include "problem_impl.h"
+#include "remap.h"
 #include "unproject.cuh"
 
 namespace mb200 {
@@ -268,7 +269,10 @@ bool remap_arguments_ok(int W, int H, int stride, int Wo, int Ho, int type, int 
     return true;
 }
 
-// The one launcher of both transform entry points: device pointers; the map and the output are packed
+}  // namespace
+
+// The one launcher of both transform entry points and of match_feature()'s templates (remap.h): device pointers; the
+// map and the output are packed
 bool launch_remap(const void* src, size_t stride, int W, int H, const float* map, int Wo, int Ho, int type, int channels,
                   int interpolation, int border, const double* border_value, void* dst, cudaStream_t s)
 {
@@ -284,6 +288,8 @@ bool launch_remap(const void* src, size_t stride, int W, int H, const float* map
         return launch_remap_typed<float>(src, stride, W, H, map, Npix, channels, interpolation, border, border_value, dst, s);
     }
 }
+
+namespace {
 
 bool have_device()
 {

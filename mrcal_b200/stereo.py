@@ -6,12 +6,19 @@ refusals (mrcal/stereo.py:23-484, 784-923, 978-1308, 1453-1607):
     mrcal_b200.rectification_maps(models, models_rect)  -> float32 (2, Nel, Naz, 2)
     mrcal_b200.stereo_range(disparity, models_rect)     -> ranges
     mrcal_b200.stereo_unproject(disparity, models_rect) -> points in rectified camera-0 coordinates
+    mrcal_b200.apply_homography(H, q)                   -> q mapped through the homography H
+    mrcal_b200.match_feature(image0, image1, q0, ...)   -> (q1, diagnostics)
 
 The geometry is host code in libmrcal_b200.so (csrc/stereo.cu); the maps, the ranges and the points are computed on
-the device, one thread per element. This module only marshals arguments.
+the device, one thread per element. match_feature() decides on the host which features can be matched, and matches
+all of them on the device in one call (csrc/match.cu). This module only marshals arguments.
+
+TM_SQDIFF .. TM_CCOEFF_NORMED have OpenCV's values.
 """
 import ctypes as C
+import operator
 import re
+import sys
 
 import numpy as np
 
@@ -22,6 +29,11 @@ from .cameramodel import cameramodel
 
 # the reference's Python wrapper takes an az0_deg above this for "autodetect" (mrcal-pywrap.c:4029-4030)
 _AZ0_AUTODETECT = 1e7
+
+# cv2.TemplateMatchModes
+TM_SQDIFF, TM_SQDIFF_NORMED, TM_CCORR, TM_CCORR_NORMED, TM_CCOEFF, TM_CCOEFF_NORMED = range(6)
+# match_feature()'s per-feature status in a batched call (MRCAL_B200_MATCH_* of include/mrcal_b200.h)
+MATCH_OK, MATCH_EDGE_PEAK, MATCH_OUTSIDE_IMAGE1, MATCH_OUTSIDE_IMAGE0, MATCH_SEARCH_TOO_SMALL = range(5)
 
 
 def _rectification_model_type(name):
@@ -287,3 +299,275 @@ def stereo_unproject(disparity, models_rectified, *, ranges=None, disparity_scal
     if a["is_scalar"] and np.ndim(qrect0) == 1:
         p = p[0]
     return p
+
+
+####################################################################################################
+# feature matching
+####################################################################################################
+def apply_homography(H, q):
+    """q (..., 2) mapped through the homography H (..., 3, 3), broadcasting: ((H00 x + H01 y) + H02) / ((H20 x + H21 y)
+    + H22), and likewise for y, as the reference computes it. In float32 if both are float32, else in float64; every
+    operation is rounded on its own, so the bits are the reference's"""
+    H, q = np.asarray(H), np.asarray(q)
+    if H.ndim < 2 or H.shape[-2:] != (3, 3):
+        raise RuntimeError(f"H must have shape (...,3,3); got {H.shape}")
+    if q.ndim < 1 or q.shape[-1] != 2:
+        raise RuntimeError(f"q must have shape (...,2); got {q.shape}")
+    dtype = np.float32 if H.dtype == np.float32 and q.dtype == np.float32 else np.float64
+    H, q = H.astype(dtype, copy=False), q.astype(dtype, copy=False)
+    x, y = q[..., 0], q[..., 1]
+    with np.errstate(all="ignore"):
+        xyz = [(H[..., i, 0] * x + H[..., i, 1] * y) + H[..., i, 2] for i in range(3)]
+        return np.stack((xyz[0] / xyz[2], xyz[1] / xyz[2]), axis=-1)
+
+
+def _template_size(template_size1):
+    """(width, height), refused as the reference refuses it (stereo.py:1853-1862)"""
+    try:
+        N = len(template_size1)
+    except TypeError:
+        N = 2
+        template_size1 = (template_size1, template_size1)
+    if N != 2:
+        raise RuntimeError(f"template_size1 must be an interable of length 2 OR a scalar. Got an iterable of length {N}")
+    for i in range(2):
+        if not (isinstance(template_size1[i], int) and template_size1[i] > 0):
+            raise RuntimeError(f"Each element of template_size1 must be an integer > 0. Got {template_size1[i]}")
+    return np.array(template_size1, dtype=int)
+
+
+def _edge_refusal(shape, what, *qall):
+    """the reference's checkdims() message for the first of qall outside an image of this shape (H, W); None if all
+    are inside. NaN coordinates are inside, as the reference's comparisons have it"""
+    for q in qall:
+        if q[0] < 0:
+            return f"Too close to the left edge in {what}"
+        if q[1] < 0:
+            return f"Too close to the top edge in {what} "
+        if q[0] >= shape[1]:
+            return f"Too close to the right edge in {what} "
+        if q[1] >= shape[0]:
+            return f"Too close to the bottom edge in {what} "
+    return None
+
+
+def _images(image0, image1):
+    """(torch or None, dtype code, (H0, W0), (H1, W1)) of two images that cv2.matchTemplate() would accept: 2-D, both
+    uint8 or both float32; numpy arrays, or contiguous torch CUDA tensors on one device"""
+    if image0.ndim != 2 or image1.ndim != 2:
+        raise RuntimeError("match_feature() accepts ONLY grayscale images of shape (H,W)")
+    torch = sys.modules.get("torch")
+    is_tensor = [torch is not None and isinstance(x, torch.Tensor) for x in (image0, image1)]
+    if any(is_tensor):
+        if not all(is_tensor):
+            raise RuntimeError("match_feature(): image0 and image1 must both be numpy arrays or both be torch CUDA "
+                               "tensors")
+        if not (image0.is_cuda and image1.is_cuda) or image0.device != image1.device:
+            raise RuntimeError("match_feature(): torch images must be CUDA tensors on one device")
+        if not (image0.is_contiguous() and image1.is_contiguous()):
+            raise RuntimeError("match_feature(): torch images must be contiguous")
+        types = {torch.uint8: 0, torch.float32: 2}
+    else:
+        if not (isinstance(image0, np.ndarray) and isinstance(image1, np.ndarray)):
+            raise RuntimeError("match_feature(): image0 and image1 must be numpy arrays or torch CUDA tensors")
+        torch = None
+        types = {np.dtype(np.uint8): 0, np.dtype(np.float32): 2}
+    if image0.dtype != image1.dtype:
+        raise RuntimeError(f"match_feature(): image0 and image1 must have the same dtype, as cv2.matchTemplate() "
+                           f"requires; got {image0.dtype} and {image1.dtype}")
+    if image0.dtype not in types:
+        raise RuntimeError(f"match_feature() supports uint8 and float32 images only, as cv2.matchTemplate() does; "
+                           f"got {image0.dtype}")
+    return torch, types[image0.dtype], tuple(image0.shape), tuple(image1.shape)
+
+
+def _packed_rows(image):
+    """image, or a copy of it, with packed pixels and a positive row stride"""
+    if image.strides[1] != image.itemsize or image.strides[0] < image.shape[1] * image.itemsize:
+        image = np.ascontiguousarray(image)
+    return image
+
+
+def _match_features(image0, image1, q0, search_radius1, template_size1, q1_estimate, H10, method, single,
+                    return_templates=False):
+    """match_feature()'s work for q0 (2,) (single) or (N,2). Returns a dict of per-feature arrays: status, q1,
+    q1_estimate, q1_template_min, q1_min, at, value, qshift and matchoutput_image; the message of the refusal
+    a single call raises (None if it does not); and, with return_templates, the (M, th, tw) templates of the features
+    that were matched"""
+    ts = _template_size(template_size1)
+    if image0.ndim != 2 or image1.ndim != 2:
+        raise RuntimeError("match_feature() accepts ONLY grayscale images of shape (H,W)")
+    if (H10 is None) == (q1_estimate is None):
+        raise RuntimeError("Exactly one of (q1_estimate,H10) must be given")
+    torch, type_code, shape0, shape1 = _images(image0, image1)
+    if method is None:
+        method = TM_CCORR_NORMED
+    if method not in range(6):
+        raise RuntimeError(f"method must be one of the TM_* constants 0..5; got {method}")
+    try:
+        r = operator.index(search_radius1)
+    except TypeError:
+        raise RuntimeError(f"search_radius1 must be an integer; got {search_radius1!r}") from None
+
+    # the reference's scalars, in its dtypes (stereo.py:1876-1901), for all features at once
+    q0 = np.asarray(q0).astype(np.float32)
+    if q0.shape[-1:] != (2,) or q0.ndim != (1 if single else 2):
+        raise RuntimeError(f"q0 must have shape (2,) or (N,2); got {q0.shape}")
+    q0 = q0.reshape(-1, 2)
+    N = q0.shape[0]
+    if H10 is None:
+        q1e = np.asarray(q1_estimate)
+        if q1e.shape not in ((2,), (N, 2)):
+            raise RuntimeError(f"q1_estimate must have shape (2,) or (N,2); got {q1e.shape}")
+        q1e = np.broadcast_to(q1e, (N, 2))
+        H = np.zeros((N, 3, 3), np.float32)
+        H[:, 0, 0] = H[:, 1, 1] = H[:, 2, 2] = 1.
+        H[:, :2, 2] = q1e - q0
+        q1e = q1e.astype(np.float32)
+    else:
+        H = np.asarray(H10).astype(np.float32)
+        if H.shape not in ((3, 3), (N, 3, 3)):
+            raise RuntimeError(f"H10 must have shape (3,3) or (N,3,3); got {H.shape}")
+        H = np.ascontiguousarray(np.broadcast_to(H, (N, 3, 3)))
+        q1e = apply_homography(H, q0)
+    tmin_f = np.round(q1e - (ts - 1.) / 2.)
+
+    status = np.full(N, MATCH_OK, np.int32)
+    H1, W1 = shape1
+    # a template whose corner is not a finite pixel of image 1 is outside it, as the reference's integer cast makes it
+    finite = np.all(np.isfinite(tmin_f) & (np.abs(tmin_f) < 2. ** 40), axis=1)
+    tmin = np.where(finite[:, None], tmin_f, 0.).astype(int)
+    tmax = tmin + ts - 1
+    out1 = ~finite | np.any((tmin < 0) | (tmax < 0), axis=1) | \
+        (tmin[:, 0] >= W1) | (tmin[:, 1] >= H1) | (tmax[:, 0] >= W1) | (tmax[:, 1] >= H1)
+    status[out1] = MATCH_OUTSIDE_IMAGE1
+    refusal = None
+    if single and out1[0]:
+        # the corner as the reference's astype(int) makes it: NaN, +-inf and anything beyond int64 become INT64_MIN
+        t = [int(v) if np.isfinite(v) and abs(v) < 2. ** 63 else -2 ** 63 for v in tmin_f[0]]
+        refusal = _edge_refusal(shape1, "image1", t, [v + int(n) - 1 for v, n in zip(t, ts)])
+
+    # the templates' maps: np.linalg.inv() in float32, the call the reference makes. A singular H10 raises in a single
+    # call, as in the reference; in a batch, its feature has no template in image 0
+    if single:
+        Hinv = np.linalg.inv(H[0])[None] if refusal is None else np.eye(3, dtype=np.float32)[None]
+    else:
+        try:
+            Hinv = np.linalg.inv(H)
+        except np.linalg.LinAlgError:
+            Hinv = np.empty_like(H)
+            for i in range(N):
+                try:
+                    Hinv[i] = np.linalg.inv(H[i])
+                except np.linalg.LinAlgError:
+                    Hinv[i] = np.nan
+                    if status[i] == MATCH_OK:
+                        status[i] = MATCH_OUTSIDE_IMAGE0
+    # the map's corners [0,0], [-1,0], [0,-1], [-1,-1], checked on image 0 (stereo.py:1927-1933)
+    corners = np.stack((tmin, np.stack((tmin[:, 0], tmax[:, 1]), 1), np.stack((tmax[:, 0], tmin[:, 1]), 1), tmax),
+                       axis=1).astype(np.float32)
+    q0c = apply_homography(Hinv[:, None], corners)
+    H0, W0 = shape0
+    with np.errstate(invalid="ignore"):
+        out0 = np.any((q0c[..., 0] < 0) | (q0c[..., 1] < 0) | (q0c[..., 0] >= W0) | (q0c[..., 1] >= H0), axis=1)
+    status[(status == MATCH_OK) & out0] = MATCH_OUTSIDE_IMAGE0
+    if single and refusal is None and out0[0]:
+        refusal = _edge_refusal(shape0, "image0", *q0c[0])
+
+    # the search cut, clipped to image 1 (stereo.py:1939-1950)
+    qmin = np.maximum(tmin - r, 0)
+    qmax = np.minimum(tmin + r + ts - 1, (W1 - 1, H1 - 1))
+    cut = qmax - qmin + 1
+    small = np.any(cut < ts, axis=1)
+    status[(status == MATCH_OK) & small] = MATCH_SEARCH_TOO_SMALL
+    if single and refusal is None and small[0]:
+        refusal = f"match_feature(): the search region {cut[0][0]}x{cut[0][1]} of image1 is smaller than the " \
+                  f"template {ts[0]}x{ts[1]}, which cv2.matchTemplate() refuses"
+
+    run = np.flatnonzero(status == MATCH_OK)
+    M = run.size
+    slot_w, slot_h = (max(1, min(2 * r + 1, n - t + 1)) for n, t in ((W1, ts[0]), (H1, ts[1])))
+    features = np.ascontiguousarray(np.concatenate((tmin[run], qmin[run], cut[run]), axis=1), np.int32)
+    Hinv_run = np.ascontiguousarray(Hinv[run], np.float32).reshape(M, 9)
+    # out: M rows of (x, y, value, status), then the M slots of float32 match output, in one buffer and one download
+    buf = np.empty(4 * M + (M * slot_w * slot_h + 1) // 2, np.float64)
+    dtype = np.uint8 if type_code == 0 else np.float32
+    templates = np.empty((M, ts[1], ts[0]), dtype) if return_templates else None
+    args = (features.ctypes.data, Hinv_run.ctypes.data, M, int(ts[0]), int(ts[1]), slot_w, slot_h, int(method))
+    if M > 0:
+        if torch is None:
+            image0, image1 = _packed_rows(image0), _packed_rows(image1)
+            _require_gpu()
+            ok = lib.mrcal_b200_match_feature(buf.ctypes.data, _ptr(templates), image0.ctypes.data, W0, H0,
+                                              image0.strides[0], image1.ctypes.data, W1, H1, image1.strides[0],
+                                              type_code, *args)
+        else:
+            es = image0.element_size()
+            with torch.cuda.device(image0.device):
+                stream = torch.cuda.current_stream(image0.device).cuda_stream
+                ok = lib.mrcal_b200_match_feature_device(buf.ctypes.data, _ptr(templates), image0.data_ptr(), W0, H0,
+                                                         W0 * es, image1.data_ptr(), W1, H1, W1 * es, type_code,
+                                                         *args, stream)
+        if not ok:
+            _fail("mrcal_b200_match_feature()")
+    res = buf[:4 * M].reshape(M, 4)
+    slots = buf[4 * M:].view(np.float32)[:M * slot_w * slot_h].reshape(M, slot_w * slot_h)
+
+    status[run] = res[:, 3].astype(np.int32)
+    at = np.full((N, 2), np.nan)
+    value = np.full(N, np.nan)
+    at[run], value[run] = res[:, :2], res[:, 2]
+    qshift = np.full((N, 2), np.nan)
+    qshift[run] = qmin[run] + q1e[run] - tmin[run]
+    ok = status == MATCH_OK
+    at[~ok], value[~ok], qshift[~ok] = np.nan, np.nan, np.nan
+    q1 = at + qshift
+    matchoutput = [None] * N
+    for k, i in enumerate(run):
+        ow, oh = cut[i] - ts + 1
+        matchoutput[i] = slots[k, :ow * oh].reshape(oh, ow)
+    result = dict(status=status, q1=q1, at=at, value=value, qshift=qshift, matchoutput_image=matchoutput)
+    return result, refusal, templates
+
+
+def match_feature(image0, image1, q0, *, search_radius1, template_size1, q1_estimate=None, H10=None, method=None,
+                  visualize=False, extratitle=None, return_plot_args=False, **kwargs):
+    """The pixel of image1 that matches the pixel q0 of image0, as mrcal.match_feature() finds it: the template is
+    image0 remapped through the homography H10 (or the translation to q1_estimate) around q1_estimate =
+    apply_homography(H10, q0), template_size1 (width, height) pixels of image1; it is matched with method (OpenCV's
+    TM_*; TM_CCORR_NORMED by default) over a window of image1 search_radius1 pixels around it in each direction, clipped
+    to the image; the discrete optimum is refined by a quadratic fit to its 3x3 neighbourhood.
+
+    q0 (2,): returns (q1, diagnostics) with the reference's keys; q1 is None if the optimum is on the edge of the match
+    output. It raises where the reference or cv2.matchTemplate() would: a template too close to an edge of either image,
+    bad arguments, mixed or unsupported dtypes, a search region smaller than the template.
+
+    q0 (N,2): every feature in one call; H10 (3,3) or (N,3,3), q1_estimate (2,) or (N,2). Returns q1 (N,2), NaN where a
+    feature failed, and diagnostics of stacked arrays (matchoutput_optimum_subpixel_at, matchoutput_optimum_subpixel,
+    qshift_image1_matchoutput, NaN where a feature failed), a per-feature status (MATCH_OK, MATCH_EDGE_PEAK,
+    MATCH_OUTSIDE_IMAGE1, MATCH_OUTSIDE_IMAGE0, MATCH_SEARCH_TOO_SMALL) and matchoutput_image, a list of each feature's
+    match output (None where there is none). No feature's failure raises, and row i is bit for bit the single call's.
+
+    Images: 2-D, both uint8 or both float32; numpy arrays (rows may be strided) or contiguous torch CUDA tensors on one
+    device, in which case the work is enqueued on torch.cuda.current_stream() with nothing uploaded. The results are
+    numpy arrays either way. visualize=True is refused: it needs gnuplotlib, which this package does not use."""
+    if visualize:
+        raise RuntimeError("match_feature(visualize=True) is not supported: it plots with gnuplotlib, which this "
+                           "package does not use. The diagnostics hold what the plot shows")
+    single = np.ndim(q0) == 1
+    r, refusal, _ = _match_features(image0, image1, q0, search_radius1, template_size1, q1_estimate, H10, method,
+                                    single)
+    if not single:
+        diagnostics = dict(matchoutput_image=r["matchoutput_image"], matchoutput_optimum_subpixel_at=r["at"],
+                           matchoutput_optimum_subpixel=r["value"], qshift_image1_matchoutput=r["qshift"],
+                           status=r["status"])
+        return r["q1"], diagnostics
+    if refusal is not None:
+        raise RuntimeError(refusal)
+    diagnostics = dict(matchoutput_image=r["matchoutput_image"][0])
+    if r["status"][0] != MATCH_OK:
+        return None, diagnostics
+    diagnostics["matchoutput_optimum_subpixel_at"] = r["at"][0]
+    diagnostics["matchoutput_optimum_subpixel"] = r["value"][0]
+    diagnostics["qshift_image1_matchoutput"] = r["qshift"][0]
+    return r["q1"][0], diagnostics
