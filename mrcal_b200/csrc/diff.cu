@@ -22,9 +22,9 @@
 #include <cuda_runtime.h>
 
 #include "common.h"
+#include "device_call.h"
 #include "device_math.cuh"
 #include "lens_dispatch.cuh"
-#include "problem_impl.h"
 #include "reduce.cuh"
 
 namespace mb200 {
@@ -352,21 +352,6 @@ __global__ void diff_stdev_kernel(const double* __restrict__ norm2, int K, long 
     difflen[j] = sqrt(s / K);
 }
 
-bool have_device()
-{
-    if(mrcal_b200_device_count() > 0) return true;
-    set_error("no usable CUDA device: libmrcal_b200 has no CPU fallback");
-    return false;
-}
-
-template <typename T>
-bool upload(DeviceArena& mem, T** d, const T* h, size_t n, cudaStream_t s)
-{
-    if(!mem.alloc(d, n)) return false;
-    MB200_CUDA_CHECK(cudaMemcpyAsync(*d, h, n * sizeof(T), cudaMemcpyHostToDevice, s));
-    return true;
-}
-
 void launch_fit(const FitArgs& A, int Nfits, bool atinfinity, cudaStream_t s)
 {
     if(atinfinity) implied_fit_kernel<3><<<Nfits, kFitThreads, 0, s>>>(A);
@@ -380,12 +365,6 @@ bool fit_status(const std::vector<int>& status)
     return true;
 }
 
-struct Stream
-{
-    cudaStream_t s = nullptr;
-    ~Stream() { if(s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
-};
-
 }  // namespace
 }  // namespace mb200
 
@@ -396,30 +375,25 @@ extern "C" bool mrcal_b200_implied_Rt10__from_unprojections(double* Rt10, const 
                                                             const double* weights, bool atinfinity,
                                                             const double* focus_center, double focus_radius)
 {
-    if(!have_device()) return false;
+    DeviceCall D;
+    if(!D.start()) return false;
     if(N < 0 || M < 1) { set_error("implied_Rt10__from_unprojections: need N >= 0 and M >= 1"); return false; }
-    DeviceArena mem;   // freed after the stream has drained
-    Stream S;
-    MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
     FitArgs A{};
     double *d_q0, *d_p0, *d_v1, *d_w = nullptr, *d_Rt;
     int* d_status;
     const size_t MN = (size_t)M * N;
-    if(!upload(mem, &d_q0, (const double*)q0, 2 * (size_t)N, S.s) || !upload(mem, &d_p0, (const double*)p0, 3 * MN, S.s) ||
-       !upload(mem, &d_v1, (const double*)v1, 3 * (size_t)N, S.s) || (weights && !upload(mem, &d_w, weights, MN, S.s)) ||
-       !mem.alloc(&d_Rt, 12) || !mem.alloc(&d_status, 1))
+    if(!D.upload(&d_q0, (const double*)q0, 2 * (size_t)N) || !D.upload(&d_p0, (const double*)p0, 3 * MN) ||
+       !D.upload(&d_v1, (const double*)v1, 3 * (size_t)N) || (weights && !D.upload(&d_w, weights, MN)) ||
+       !D.alloc(&d_Rt, 12) || !D.alloc(&d_status, 1))
         return false;
     A.q0 = d_q0; A.p0 = d_p0; A.v1 = d_v1; A.w = d_w;
     A.N = N; A.M = M;
     A.cx = focus_center[0]; A.cy = focus_center[1]; A.r2 = focus_radius * focus_radius;
     A.Rt10 = d_Rt; A.status = d_status;
-    launch_fit(A, 1, atinfinity, S.s);
+    launch_fit(A, 1, atinfinity, D.stream);
     MB200_CUDA_CHECK(cudaGetLastError());
     std::vector<int> status(1);
-    MB200_CUDA_CHECK(cudaMemcpyAsync(Rt10, d_Rt, 12 * sizeof(double), cudaMemcpyDeviceToHost, S.s));
-    MB200_CUDA_CHECK(cudaMemcpyAsync(status.data(), d_status, sizeof(int), cudaMemcpyDeviceToHost, S.s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(S.s));
-    return fit_status(status);
+    return D.download(Rt10, d_Rt, 12) && D.download(status.data(), d_status, 1) && D.finish() && fit_status(status);
 }
 
 extern "C" bool mrcal_b200_projection_diff(double* Rt10, double* difflen, double* diff,
@@ -429,49 +403,41 @@ extern "C" bool mrcal_b200_projection_diff(double* Rt10, double* difflen, double
                                            const double* uncertainties, const double* focus_center, double focus_radius,
                                            bool fit_Rt10)
 {
-    if(!have_device()) return false;
+    DeviceCall D;
+    if(!D.start()) return false;
     if(Nmodels < 2) { set_error("At least 2 models are required to compute the diff"); return false; }
     if(N < 0 || Nd < 1 || (distance == nullptr && Nd != 1))
     {
         set_error("projection_diff: need N >= 0, and Nd >= 1 (Nd == 1 at infinity)");
         return false;
     }
-    std::vector<int> kinds(Nmodels), Nintr(Nmodels);
-    std::vector<LensArgs> lens(Nmodels);
+    std::vector<HostLens> lens(Nmodels);
     size_t Nintr_all = 0;
     for(int k = 0; k < Nmodels; k++)
     {
-        kinds[k] = lens_kind_of(&lensmodels[k]);
-        if(kinds[k] < 0) { set_error("this lens model has no CUDA implementation"); return false; }
-        if(!lens_args_setup(&lens[k], kinds[k], &lensmodels[k])) return false;
-        Nintr[k] = mrcal_lensmodel_num_params(&lensmodels[k]);
-        Nintr_all += Nintr[k];
+        if(!lens_setup(&lens[k], &lensmodels[k])) return false;
+        Nintr_all += lens[k].Nintr;
     }
     const int Npairs = Nmodels - 1;
     const long NdN = (long)Nd * N;
-    DeviceArena mem;   // freed after the stream has drained
-    Stream S;
-    MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
     double *d_q0, *d_v, *d_dist = nullptr, *d_intr, *d_U = nullptr, *d_w = nullptr, *d_Rt, *d_diff = nullptr, *d_len,
            *d_n2 = nullptr;
     int* d_status = nullptr;
-    if(!upload(mem, &d_q0, (const double*)q0, 2 * (size_t)N, S.s) ||
-       !upload(mem, &d_v, (const double*)v, 3 * (size_t)Nmodels * N, S.s) ||
-       (distance && !upload(mem, &d_dist, distance, (size_t)Nd, S.s)) ||
-       !upload(mem, &d_intr, intrinsics, Nintr_all, S.s) || !mem.alloc(&d_Rt, 12 * (size_t)Npairs) ||
-       !mem.alloc(&d_len, (size_t)NdN))
+    if(!D.upload(&d_q0, (const double*)q0, 2 * (size_t)N) || !D.upload(&d_v, (const double*)v, 3 * (size_t)Nmodels * N) ||
+       (distance && !D.upload(&d_dist, distance, (size_t)Nd)) || !D.upload(&d_intr, intrinsics, Nintr_all) ||
+       !D.alloc(&d_Rt, 12 * (size_t)Npairs) || !D.alloc(&d_len, (size_t)NdN))
         return false;
-    if(Nmodels == 2) { if(!mem.alloc(&d_diff, 2 * (size_t)NdN)) return false; }
-    else if(!mem.alloc(&d_n2, (size_t)Npairs * NdN)) return false;
+    if(Nmodels == 2) { if(!D.alloc(&d_diff, 2 * (size_t)NdN)) return false; }
+    else if(!D.alloc(&d_n2, (size_t)Npairs * NdN)) return false;
     std::vector<int> status;
     if(fit_Rt10)
     {
-        if(!mem.alloc(&d_status, (size_t)Npairs)) return false;
+        if(!D.alloc(&d_status, (size_t)Npairs)) return false;
         if(uncertainties)
         {
-            if(!upload(mem, &d_U, uncertainties, (size_t)Nmodels * NdN, S.s) || !mem.alloc(&d_w, (size_t)Npairs * NdN))
+            if(!D.upload(&d_U, uncertainties, (size_t)Nmodels * NdN) || !D.alloc(&d_w, (size_t)Npairs * NdN))
                 return false;
-            if(NdN > 0) diff_weights_kernel<<<(unsigned)((NdN + 255) / 256), 256, 0, S.s>>>(d_U, Nmodels, NdN, d_w);
+            if(NdN > 0) diff_weights_kernel<<<(unsigned)((NdN + 255) / 256), 256, 0, D.stream>>>(d_U, Nmodels, NdN, d_w);
         }
         FitArgs A{};
         A.q0 = d_q0; A.p0 = d_v; A.dist = d_dist; A.v1 = d_v + 3 * (size_t)N; A.w = d_w;
@@ -479,38 +445,34 @@ extern "C" bool mrcal_b200_projection_diff(double* Rt10, double* difflen, double
         A.N = N; A.M = Nd;
         A.cx = focus_center[0]; A.cy = focus_center[1]; A.r2 = focus_radius * focus_radius;
         A.Rt10 = d_Rt; A.status = d_status;
-        launch_fit(A, Npairs, distance == nullptr, S.s);
+        launch_fit(A, Npairs, distance == nullptr, D.stream);
         status.resize(Npairs);
     }
-    else MB200_CUDA_CHECK(cudaMemcpyAsync(d_Rt, Rt10, 12 * (size_t)Npairs * sizeof(double), cudaMemcpyHostToDevice, S.s));
+    else MB200_CUDA_CHECK(cudaMemcpyAsync(d_Rt, Rt10, 12 * (size_t)Npairs * sizeof(double), cudaMemcpyHostToDevice, D.stream));
     if(NdN > 0)
     {
         const unsigned blocks = (unsigned)((NdN + 127) / 128);
-        const double* intr = d_intr + Nintr[0];
+        const double* intr = d_intr + lens[0].Nintr;
         for(int k = 1; k < Nmodels; k++)
         {
-            LensArgs a = lens[k];
+            LensArgs a = lens[k].a;
             a.intr = intr;
-            intr += Nintr[k];
+            intr += lens[k].Nintr;
             const double* Rt = d_Rt + 12 * (k - 1);
             double* n2 = d_n2 ? d_n2 + (k - 1) * NdN : nullptr;
-            if(!dispatch_lens_kind(kinds[k], [&](auto kk)
+            if(!dispatch_lens_kind(lens[k].kind, [&](auto kk)
                {
-                   reproject_diff_kernel<decltype(kk)::value><<<blocks, 128, 0, S.s>>>(a, Rt, d_q0, d_v, d_dist, N, Nd,
-                                                                                     d_diff, d_len, n2);
+                   reproject_diff_kernel<decltype(kk)::value><<<blocks, 128, 0, D.stream>>>(a, Rt, d_q0, d_v, d_dist, N,
+                                                                                          Nd, d_diff, d_len, n2);
                }))
                 return false;
         }
-        if(d_n2) diff_stdev_kernel<<<(unsigned)((NdN + 255) / 256), 256, 0, S.s>>>(d_n2, Npairs, NdN, d_len);
+        if(d_n2) diff_stdev_kernel<<<(unsigned)((NdN + 255) / 256), 256, 0, D.stream>>>(d_n2, Npairs, NdN, d_len);
     }
     MB200_CUDA_CHECK(cudaGetLastError());
-    if(fit_Rt10)
-    {
-        MB200_CUDA_CHECK(cudaMemcpyAsync(Rt10, d_Rt, 12 * (size_t)Npairs * sizeof(double), cudaMemcpyDeviceToHost, S.s));
-        MB200_CUDA_CHECK(cudaMemcpyAsync(status.data(), d_status, Npairs * sizeof(int), cudaMemcpyDeviceToHost, S.s));
-    }
-    MB200_CUDA_CHECK(cudaMemcpyAsync(difflen, d_len, NdN * sizeof(double), cudaMemcpyDeviceToHost, S.s));
-    if(diff && d_diff) MB200_CUDA_CHECK(cudaMemcpyAsync(diff, d_diff, 2 * NdN * sizeof(double), cudaMemcpyDeviceToHost, S.s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(S.s));
-    return fit_status(status);
+    if(fit_Rt10 && !(D.download(Rt10, d_Rt, 12 * (size_t)Npairs) && D.download(status.data(), d_status, (size_t)Npairs)))
+        return false;
+    if(!D.download(difflen, d_len, (size_t)NdN) || (diff && d_diff && !D.download(diff, d_diff, 2 * (size_t)NdN)))
+        return false;
+    return D.finish() && fit_status(status);
 }

@@ -9,6 +9,7 @@
 // shared memory; each thread evaluates its corner's projection and gradients
 // in registers and writes its two fixed-width Jacobian rows. Row positions are
 // analytic (fixed nnz per row class), so there is no serial fill pointer.
+#include "lens_dispatch.cuh"
 #include "observation.cuh"
 #include "ptx.cuh"
 #include "triangulated.cuh"
@@ -780,22 +781,10 @@ bool launch_evaluate(const DevProblem& dp, const EvalBuffers& out, bool with_jac
         MB200_CUDA_CHECK(cudaMemsetAsync(out.norm2, 0, sizeof(double), stream));
         if(!launch_unpack_state(dp, out.p, stream, nlaunch)) return false;
     }
-    switch(dp.lens_kind)
-    {
-    case LENS_PINHOLE:       if(!launch_kind<LENS_PINHOLE>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_STEREOGRAPHIC: if(!launch_kind<LENS_STEREOGRAPHIC>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_LONLAT:        if(!launch_kind<LENS_LONLAT>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_LATLON:        if(!launch_kind<LENS_LATLON>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_OPENCV4:       if(!launch_kind<LENS_OPENCV4>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_OPENCV5:       if(!launch_kind<LENS_OPENCV5>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_OPENCV8:       if(!launch_kind<LENS_OPENCV8>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_OPENCV12:      if(!launch_kind<LENS_OPENCV12>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_SPLINED3:      if(!launch_kind<LENS_SPLINED3>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_SPLINED2:      if(!launch_kind<LENS_SPLINED2>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_CAHVOR:        if(!launch_kind<LENS_CAHVOR>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    case LENS_CAHVORE:       if(!launch_kind<LENS_CAHVORE>(dp, out, with_jacobian, stream, nlaunch, boards)) return false; break;
-    default: set_error("lens model kind %d has no CUDA implementation", dp.lens_kind); return false;
-    }
+    bool ok = false;
+    if(!dispatch_lens_kind(dp.lens_kind, [&](auto k)
+       { ok = launch_kind<decltype(k)::value>(dp, out, with_jacobian, stream, nlaunch, boards); }) || !ok)
+        return false;
     if(dp.Ntri > 0)
     {
         const int threads = 128, blocks = (dp.Ntri + threads - 1) / threads;

@@ -10,10 +10,10 @@
 #include <cstdint>
 
 #include "common.h"
+#include "device_call.h"
 #include "device_math.cuh"
 #include "lens_dispatch.cuh"
 #include "polygon.cuh"
-#include "problem_impl.h"
 #include "remap.h"
 #include "unproject.cuh"
 
@@ -291,27 +291,6 @@ bool launch_remap(const void* src, size_t stride, int W, int H, const float* map
 
 namespace {
 
-bool have_device()
-{
-    if(mrcal_b200_device_count() > 0) return true;
-    set_error("no usable CUDA device: libmrcal_b200 has no CPU fallback");
-    return false;
-}
-
-struct Stream
-{
-    cudaStream_t s = nullptr;
-    ~Stream() { if(s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
-};
-
-template <typename T>
-bool upload(DeviceArena& mem, T** d, const T* h, size_t n, cudaStream_t s)
-{
-    if(!mem.alloc(d, n)) return false;
-    if(n) MB200_CUDA_CHECK(cudaMemcpyAsync(*d, h, n * sizeof(T), cudaMemcpyHostToDevice, s));
-    return true;
-}
-
 // the inverse of the 3x3 A (row-major) by its adjugate; false if A is singular
 bool invert3(double out[9], const double A[9])
 {
@@ -350,18 +329,9 @@ extern "C" bool mrcal_b200_image_transformation_map(float* mapxy, int W_to, int 
         set_error("The valid-intrinsics region must have between 1 and %d vertices; got %d", kMaxRegion, Nregion);
         return false;
     }
-    const int kind_from = lens_kind_of(lensmodel_from), kind_to = lens_kind_of(lensmodel_to);
-    if(kind_from < 0 || kind_to < 0) { set_error("this lens model has no CUDA implementation"); return false; }
-    LensArgs a_from, a_to;
-    if(!lens_args_setup(&a_from, kind_from, lensmodel_from) || !lens_args_setup(&a_to, kind_to, lensmodel_to)) return false;
-    const int Nintr_from = mrcal_lensmodel_num_params(lensmodel_from), Nintr_to = mrcal_lensmodel_num_params(lensmodel_to);
-    if(kind_to == LENS_CAHVORE)
-        for(int i = Nintr_to - 3; i < Nintr_to; i++)
-            if(intrinsics_to[i] != 0.)
-            {
-                set_error("unproject() currently only works with a central projection. So I cannot unproject(CAHVORE,E!=0)");
-                return false;
-            }
+    HostLens from, to;
+    if(!lens_setup(&from, lensmodel_from) || !lens_setup(&to, lensmodel_to) || !central_projection(to, intrinsics_to))
+        return false;
 
     RayTransform T{};
     T.M[0] = T.M[4] = T.M[8] = 1.;
@@ -389,36 +359,32 @@ extern "C" bool mrcal_b200_image_transformation_map(float* mapxy, int W_to, int 
             }
         }
     }
-    if(!have_device()) return false;
+    DeviceCall D;
+    if(!D.start()) return false;
 
     const long Npix = (long)W_to * H_to;
-    DeviceArena mem;   // freed after the stream has drained
-    Stream S;
-    MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
     double *d_intr_from, *d_intr_to, *d_ray, *d_region = nullptr;
     float2* d_map;
-    if(!upload(mem, &d_intr_from, intrinsics_from, (size_t)Nintr_from, S.s)) return false;
-    if(!upload(mem, &d_intr_to, intrinsics_to, (size_t)Nintr_to, S.s)) return false;
-    if(region && !upload(mem, &d_region, (const double*)region, 2 * (size_t)Nregion, S.s)) return false;
-    if(!mem.alloc(&d_ray, 3 * (size_t)Npix) || !mem.alloc(&d_map, (size_t)Npix)) return false;
-    a_from.intr = d_intr_from;
-    a_to.intr = d_intr_to;
+    if(!D.upload(&d_intr_from, intrinsics_from, (size_t)from.Nintr) || !D.upload(&d_intr_to, intrinsics_to, (size_t)to.Nintr) ||
+       (region && !D.upload(&d_region, (const double*)region, 2 * (size_t)Nregion)) ||
+       !D.alloc(&d_ray, 3 * (size_t)Npix) || !D.alloc(&d_map, (size_t)Npix))
+        return false;
+    from.a.intr = d_intr_from;
+    to.a.intr = d_intr_to;
     const bool behind_ok = mrcal_lensmodel_metadata(lensmodel_to).can_project_behind_camera;
     const unsigned blocks = (unsigned)((Npix + 127) / 128);
-    if(!dispatch_lens_kind(kind_to, [&](auto k)
+    if(!dispatch_lens_kind(to.kind, [&](auto k)
     {
-        reprojection_rays_kernel<decltype(k)::value><<<blocks, 128, 0, S.s>>>(a_to, behind_ok, T, W_to, Npix, d_ray);
+        reprojection_rays_kernel<decltype(k)::value><<<blocks, 128, 0, D.stream>>>(to.a, behind_ok, T, W_to, Npix, d_ray);
     })) return false;
     const int nreg = region ? Nregion : 0;
-    if(!dispatch_lens_kind(kind_from, [&](auto k)
+    if(!dispatch_lens_kind(from.kind, [&](auto k)
     {
-        reprojection_map_kernel<decltype(k)::value><<<blocks, 128, nreg * sizeof(double2), S.s>>>(
-            a_from, d_ray, Npix, (const double2*)d_region, nreg, d_map);
+        reprojection_map_kernel<decltype(k)::value><<<blocks, 128, nreg * sizeof(double2), D.stream>>>(
+            from.a, d_ray, Npix, (const double2*)d_region, nreg, d_map);
     })) return false;
     MB200_CUDA_CHECK(cudaGetLastError());
-    MB200_CUDA_CHECK(cudaMemcpyAsync(mapxy, d_map, Npix * sizeof(float2), cudaMemcpyDeviceToHost, S.s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(S.s));
-    return true;
+    return D.download((float2*)mapxy, d_map, (size_t)Npix) && D.finish();
 }
 
 extern "C" bool mrcal_b200_is_within_region(bool* mask, const mrcal_point2_t* q, int N, const mrcal_point2_t* region,
@@ -426,21 +392,16 @@ extern "C" bool mrcal_b200_is_within_region(bool* mask, const mrcal_point2_t* q,
 {
     if(N < 0 || Nregion < 0) { set_error("is_within_region: N = %d and Nregion = %d must be >= 0", N, Nregion); return false; }
     if(N == 0) return true;
-    if(!have_device()) return false;
-    DeviceArena mem;   // freed after the stream has drained
-    Stream S;
-    MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
+    DeviceCall D;
     double *d_q, *d_region;
     bool* d_mask;
-    if(!upload(mem, &d_q, (const double*)q, 2 * (size_t)N, S.s) ||
-       !upload(mem, &d_region, (const double*)region, 2 * (size_t)Nregion, S.s) || !mem.alloc(&d_mask, (size_t)N))
+    if(!D.start() || !D.upload(&d_q, (const double*)q, 2 * (size_t)N) ||
+       !D.upload(&d_region, (const double*)region, 2 * (size_t)Nregion) || !D.alloc(&d_mask, (size_t)N))
         return false;
-    within_region_kernel<<<(unsigned)((N + 255) / 256), 256, 0, S.s>>>((const double2*)d_q, N, (const double2*)d_region,
-                                                                       Nregion, d_mask);
+    within_region_kernel<<<(unsigned)((N + 255) / 256), 256, 0, D.stream>>>((const double2*)d_q, N, (const double2*)d_region,
+                                                                            Nregion, d_mask);
     MB200_CUDA_CHECK(cudaGetLastError());
-    MB200_CUDA_CHECK(cudaMemcpyAsync(mask, d_mask, (size_t)N * sizeof(bool), cudaMemcpyDeviceToHost, S.s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(S.s));
-    return true;
+    return D.download(mask, d_mask, (size_t)N) && D.finish();
 }
 
 extern "C" bool mrcal_b200_transform_image(void* out, const void* image, int W, int H, int image_stride, int type,
@@ -448,28 +409,23 @@ extern "C" bool mrcal_b200_transform_image(void* out, const void* image, int W, 
                                            int border_mode, const double* border_value)
 {
     if(!remap_arguments_ok(W, H, image_stride, W_out, H_out, type, channels, interpolation, border_mode)) return false;
-    if(!have_device()) return false;
+    DeviceCall D;
+    if(!D.start()) return false;
     const size_t row = (size_t)W * channels * element_size(type);
     const long Npix = (long)W_out * H_out;
     if(Npix == 0) return true;
     const size_t out_bytes = Npix * channels * element_size(type);
-    DeviceArena mem;   // freed after the stream has drained
-    Stream S;
-    MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
     uint8_t *d_src, *d_dst;
     float* d_map;
-    if(!mem.alloc(&d_src, row * H) || !mem.alloc(&d_dst, out_bytes)) return false;
-    MB200_CUDA_CHECK(cudaMemcpy2DAsync(d_src, row, image, image_stride, row, H, cudaMemcpyHostToDevice, S.s));
-    if(!upload(mem, &d_map, mapxy, 2 * (size_t)Npix, S.s)) return false;
     // a transparent border leaves pixels as they were: start from the caller's output
-    if(border_mode == MRCAL_B200_BORDER_TRANSPARENT)
-        MB200_CUDA_CHECK(cudaMemcpyAsync(d_dst, out, out_bytes, cudaMemcpyHostToDevice, S.s));
-    if(!launch_remap(d_src, row, W, H, d_map, W_out, H_out, type, channels, interpolation, border_mode, border_value, d_dst,
-                     S.s))
+    const bool transparent = border_mode == MRCAL_B200_BORDER_TRANSPARENT;
+    if(!D.upload(&d_src, image, (size_t)image_stride, row, (size_t)H) ||
+       !(transparent ? D.upload(&d_dst, (const uint8_t*)out, out_bytes) : D.alloc(&d_dst, out_bytes)) ||
+       !D.upload(&d_map, mapxy, 2 * (size_t)Npix))
         return false;
-    MB200_CUDA_CHECK(cudaMemcpyAsync(out, d_dst, out_bytes, cudaMemcpyDeviceToHost, S.s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(S.s));
-    return true;
+    return launch_remap(d_src, row, W, H, d_map, W_out, H_out, type, channels, interpolation, border_mode, border_value,
+                        d_dst, D.stream) &&
+           D.download((uint8_t*)out, d_dst, out_bytes) && D.finish();
 }
 
 extern "C" bool mrcal_b200_transform_image_device(void* out, const void* image, int W, int H, int image_stride,

@@ -1,5 +1,6 @@
-// Lens-model dispatch shared by the point-wise kernels (project.cu, diff.cu): the per-call lens arguments, one
-// projection call for every kind, and the runtime kind -> template instantiation switch.
+// Lens-model dispatch: the per-call lens arguments and their host setup, one projection call for every kind, and the
+// runtime kind -> template instantiation switch, for the point-wise kernels (project.cu, diff.cu, image_transforms.cu,
+// stereo.cu) and the problem's own (eval.cu, uncertainty.cu).
 #pragma once
 #include <type_traits>
 
@@ -27,17 +28,35 @@ __device__ __forceinline__ void project_any(double q[2], double dq_dp[2][3], con
         project_parametric<KIND>(q, dq_dp, nullptr, p, a.intr, a.cfg);
 }
 
-// Everything of LensArgs but intr, for a lens model whose kind has been checked (lens_kind_of() >= 0)
-inline bool lens_args_setup(LensArgs* a, int kind, const mrcal_lensmodel_t* lensmodel)
+// A lens model as the point-wise kernels take it. a.intr is left for the caller to point at the uploaded intrinsics
+struct HostLens { int kind; LensArgs a; int Nintr; };
+
+// false + set_error() for a lens model without a kernel or with an invalid spline grid
+inline bool lens_setup(HostLens* L, const mrcal_lensmodel_t* lensmodel)
 {
-    *a = LensArgs{};
-    if(kind == LENS_SPLINED3 || kind == LENS_SPLINED2)
+    *L = HostLens{lens_kind_of(lensmodel), LensArgs{}, mrcal_lensmodel_num_params(lensmodel)};
+    if(L->kind < 0) { set_error("this lens model has no CUDA implementation"); return false; }
+    if(L->kind == LENS_SPLINED3 || L->kind == LENS_SPLINED2)
     {
-        a->Nx = lensmodel->LENSMODEL_SPLINED_STEREOGRAPHIC__config.Nx;
-        a->Ny = lensmodel->LENSMODEL_SPLINED_STEREOGRAPHIC__config.Ny;
-        if(!spline_segments_per_u(&a->segments_per_u, lensmodel)) return false;
+        L->a.Nx = lensmodel->LENSMODEL_SPLINED_STEREOGRAPHIC__config.Nx;
+        L->a.Ny = lensmodel->LENSMODEL_SPLINED_STEREOGRAPHIC__config.Ny;
+        if(!spline_segments_per_u(&L->a.segments_per_u, lensmodel)) return false;
     }
-    if(kind == LENS_CAHVORE) a->cfg = lensmodel->LENSMODEL_CAHVORE__config.linearity;
+    if(L->kind == LENS_CAHVORE) L->a.cfg = lensmodel->LENSMODEL_CAHVORE__config.linearity;
+    return true;
+}
+
+// unproject() needs a central projection: false + set_error() for CAHVORE with E != 0, the reference's rule
+// (mrcal.c:3203-3214)
+inline bool central_projection(const HostLens& L, const double* intrinsics)
+{
+    if(L.kind == LENS_CAHVORE)
+        for(int i = L.Nintr - 3; i < L.Nintr; i++)
+            if(intrinsics[i] != 0.)
+            {
+                set_error("unproject() currently only works with a central projection. So I cannot unproject(CAHVORE,E!=0)");
+                return false;
+            }
     return true;
 }
 

@@ -21,8 +21,8 @@
 #include <cstdint>
 
 #include "common.h"
+#include "device_call.h"
 #include "problem.h"
-#include "problem_impl.h"
 #include "remap.h"
 
 namespace mb200 {
@@ -371,20 +371,6 @@ __global__ void match_optimum_kernel(const MatchFeature* __restrict__ feat, int 
 // the launches
 ////////////////////////////////////////////////////////////////////////////////
 
-bool have_device()
-{
-    if(mrcal_b200_device_count() > 0) return true;
-    set_error("no usable CUDA device: libmrcal_b200 has no CPU fallback");
-    return false;
-}
-
-struct Stream
-{
-    cudaStream_t s = nullptr;
-    bool own = false;
-    ~Stream() { if(s) cudaStreamSynchronize(s); if(own && s) cudaStreamDestroy(s); }
-};
-
 size_t element_size(int type) { return type == MRCAL_B200_IMAGE_UINT8 ? 1 : 4; }
 
 bool arguments_ok(int W0, int H0, int stride0, int W1, int H1, int stride1, int type, const int* features, int M,
@@ -422,7 +408,7 @@ bool arguments_ok(int W0, int H0, int stride0, int W1, int H1, int stride1, int 
 template <typename T>
 bool match_run(const T* img0, size_t stride0, int W0, int H0, const T* img1, size_t stride1, int W1, int H1, int type,
                const int* features, const float* Hinv, int M, int tw, int th, int slot_w, int slot_h, int method,
-               double* out, void* templates, DeviceArena& mem, cudaStream_t s)
+               double* out, void* templates, DeviceCall& D)
 {
     const long slot = (long)slot_w * slot_h;
     const int n = tw * th;
@@ -435,12 +421,12 @@ bool match_run(const T* img0, size_t stride0, int W0, int H0, const T* img1, siz
     T* d_templ;
     TemplateSums* d_tsums;
     uint8_t* d_out;
-    if(!mem.alloc(&d_feat, (size_t)M) || !mem.alloc(&d_Hinv, 9 * (size_t)M) || !mem.alloc(&d_map, 2 * (size_t)M * n) ||
-       !mem.alloc(&d_templ, (size_t)M * n) || !mem.alloc(&d_tsums, (size_t)M) || !mem.alloc(&d_out, out_bytes))
-        return false;
     static_assert(sizeof(MatchFeature) == 6 * sizeof(int), "MatchFeature is the host's 6 ints");
-    MB200_CUDA_CHECK(cudaMemcpyAsync(d_feat, features, (size_t)M * sizeof(MatchFeature), cudaMemcpyHostToDevice, s));
-    MB200_CUDA_CHECK(cudaMemcpyAsync(d_Hinv, Hinv, 9 * (size_t)M * sizeof(float), cudaMemcpyHostToDevice, s));
+    if(!D.upload(&d_feat, (const MatchFeature*)features, (size_t)M) || !D.upload(&d_Hinv, Hinv, 9 * (size_t)M) ||
+       !D.alloc(&d_map, 2 * (size_t)M * n) || !D.alloc(&d_templ, (size_t)M * n) || !D.alloc(&d_tsums, (size_t)M) ||
+       !D.alloc(&d_out, out_bytes))
+        return false;
+    const cudaStream_t s = D.stream;
     MatchResult* d_res = (MatchResult*)d_out;
     float* d_match = (float*)(d_out + res_bytes);
 
@@ -470,23 +456,20 @@ bool match_run(const T* img0, size_t stride0, int W0, int H0, const T* img1, siz
     match_optimum_kernel<<<(M + 3) / 4, 128, 0, s>>>(d_feat, M, tw, th, method, slot, d_match, d_res);
     MB200_CUDA_CHECK(cudaGetLastError());
 
-    MB200_CUDA_CHECK(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, s));
-    if(templates)
-        MB200_CUDA_CHECK(cudaMemcpyAsync(templates, d_templ, (size_t)M * n * sizeof(T), cudaMemcpyDeviceToHost, s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(s));
-    return true;
+    return D.download((uint8_t*)out, d_out, out_bytes) && (!templates || D.download((T*)templates, d_templ, (size_t)M * n)) &&
+           D.finish();
 }
 
 bool match_dispatch(const void* img0, int stride0, int W0, int H0, const void* img1, int stride1, int W1, int H1,
                     int type, const int* features, const float* Hinv, int M, int tw, int th, int slot_w, int slot_h,
-                    int method, double* out, void* templates, DeviceArena& mem, cudaStream_t s)
+                    int method, double* out, void* templates, DeviceCall& D)
 {
     if(type == MRCAL_B200_IMAGE_UINT8)
         return match_run<uint8_t>((const uint8_t*)img0, (size_t)stride0, W0, H0, (const uint8_t*)img1,
                                   (size_t)stride1, W1, H1, type, features, Hinv, M, tw, th, slot_w, slot_h, method,
-                                  out, templates, mem, s);
+                                  out, templates, D);
     return match_run<float>((const float*)img0, (size_t)stride0 / 4, W0, H0, (const float*)img1, (size_t)stride1 / 4,
-                            W1, H1, type, features, Hinv, M, tw, th, slot_w, slot_h, method, out, templates, mem, s);
+                            W1, H1, type, features, Hinv, M, tw, th, slot_w, slot_h, method, out, templates, D);
 }
 
 }  // namespace
@@ -502,18 +485,14 @@ extern "C" bool mrcal_b200_match_feature(double* out, void* templates, const voi
     if(!arguments_ok(W0, H0, stride0, W1, H1, stride1, type, features, M, template_w, template_h, slot_w, slot_h, method))
         return false;
     if(M == 0) return true;
-    if(!have_device()) return false;
     const size_t es = element_size(type), row0 = (size_t)W0 * es, row1 = (size_t)W1 * es;
-    DeviceArena mem;   // freed after the stream has drained
-    Stream S;
-    MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
-    S.own = true;
+    DeviceCall D;
     uint8_t *d0, *d1;
-    if(!mem.alloc(&d0, row0 * H0) || !mem.alloc(&d1, row1 * H1)) return false;
-    MB200_CUDA_CHECK(cudaMemcpy2DAsync(d0, row0, image0, stride0, row0, H0, cudaMemcpyHostToDevice, S.s));
-    MB200_CUDA_CHECK(cudaMemcpy2DAsync(d1, row1, image1, stride1, row1, H1, cudaMemcpyHostToDevice, S.s));
+    if(!D.start() || !D.upload(&d0, image0, (size_t)stride0, row0, (size_t)H0) ||
+       !D.upload(&d1, image1, (size_t)stride1, row1, (size_t)H1))
+        return false;
     return match_dispatch(d0, (int)row0, W0, H0, d1, (int)row1, W1, H1, type, features, Hinv, M, template_w,
-                          template_h, slot_w, slot_h, method, out, templates, mem, S.s);
+                          template_h, slot_w, slot_h, method, out, templates, D);
 }
 
 extern "C" bool mrcal_b200_match_feature_device(double* out, void* templates, const void* image0, int W0, int H0,
@@ -527,9 +506,8 @@ extern "C" bool mrcal_b200_match_feature_device(double* out, void* templates, co
     if((uintptr_t)image0 % es || (uintptr_t)image1 % es)
     { set_error("match_feature(): the images must be aligned to their element size (%zu bytes)", es); return false; }
     if(M == 0) return true;
-    DeviceArena mem;   // freed after the stream has drained
-    Stream S;
-    S.s = (cudaStream_t)stream;
-    return match_dispatch(image0, stride0, W0, H0, image1, stride1, W1, H1, type, features, Hinv, M, template_w,
-                          template_h, slot_w, slot_h, method, out, templates, mem, S.s);
+    DeviceCall D;
+    return D.start((cudaStream_t)stream) &&
+           match_dispatch(image0, stride0, W0, H0, image1, stride1, W1, H1, type, features, Hinv, M, template_w,
+                          template_h, slot_w, slot_h, method, out, templates, D);
 }

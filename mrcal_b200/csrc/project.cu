@@ -5,9 +5,9 @@
 #include <cuda_runtime.h>
 
 #include "common.h"
+#include "device_call.h"
 #include "device_math.cuh"
 #include "lens_dispatch.cuh"
-#include "problem.h"
 #include "unproject.cuh"
 
 namespace mb200 {
@@ -68,63 +68,33 @@ __global__ void unproject_kernel(LensArgs a, const double* __restrict__ q, int N
     v[3 * i] = out[0]; v[3 * i + 1] = out[1]; v[3 * i + 2] = out[2];
 }
 
-struct Scratch
-{
-    double *d_intr = nullptr, *d_in = nullptr, *d_out = nullptr, *d_grad = nullptr, *d_gi = nullptr;
-    ~Scratch() { cudaFree(d_intr); cudaFree(d_in); cudaFree(d_out); cudaFree(d_grad); cudaFree(d_gi); }
-};
-
 bool run(bool unproject, double* out, double* dq_dp, double* dq_di, const double* in, int N, const mrcal_lensmodel_t* lensmodel, const double* intrinsics)
 {
-    int ndev = 0;
-    if(cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0)
-    {
-        cudaGetLastError();
-        set_error("no usable CUDA device: libmrcal_b200 has no CPU fallback");
-        return false;
-    }
-    const int kind = lens_kind_of(lensmodel);
-    if(kind < 0) { set_error("this lens model has no CUDA implementation"); return false; }
-    const int Nintr = mrcal_lensmodel_num_params(lensmodel);
+    DeviceCall D;
+    HostLens L;
+    if(!D.start() || !lens_setup(&L, lensmodel)) return false;
     if(N <= 0) return true;
-    LensArgs a;
-    if(!lens_args_setup(&a, kind, lensmodel)) return false;
-    if(kind == LENS_CAHVORE && unproject)
-        for(int i = Nintr - 3; i < Nintr; i++)
-            if(intrinsics[i] != 0.)
-            {
-                // the reference's rule (mrcal.c:3203-3214)
-                set_error("unproject() currently only works with a central projection. So I cannot unproject(CAHVORE,E!=0)");
-                return false;
-            }
-    Scratch S;
+    if(unproject && !central_projection(L, intrinsics)) return false;
+    const int Nintr = L.Nintr;
     const size_t nin = (size_t)N * (unproject ? 2 : 3), nout = (size_t)N * (unproject ? 3 : 2);
-    MB200_CUDA_CHECK(cudaMalloc(&S.d_intr, Nintr * sizeof(double)));
-    MB200_CUDA_CHECK(cudaMalloc(&S.d_in, nin * sizeof(double)));
-    MB200_CUDA_CHECK(cudaMalloc(&S.d_out, nout * sizeof(double)));
-    if(dq_dp) MB200_CUDA_CHECK(cudaMalloc(&S.d_grad, (size_t)N * 6 * sizeof(double)));
-    if(dq_di)
-    {
-        MB200_CUDA_CHECK(cudaMalloc(&S.d_gi, (size_t)N * 2 * Nintr * sizeof(double)));
-        MB200_CUDA_CHECK(cudaMemset(S.d_gi, 0, (size_t)N * 2 * Nintr * sizeof(double)));
-    }
-    MB200_CUDA_CHECK(cudaMemcpy(S.d_intr, intrinsics, Nintr * sizeof(double), cudaMemcpyHostToDevice));
-    MB200_CUDA_CHECK(cudaMemcpy(S.d_in, in, nin * sizeof(double), cudaMemcpyHostToDevice));
-    a.intr = S.d_intr;
+    double *d_intr, *d_in, *d_out, *d_grad = nullptr, *d_gi = nullptr;
+    if(!D.upload(&d_intr, intrinsics, (size_t)Nintr) || !D.upload(&d_in, in, nin) || !D.alloc(&d_out, nout) ||
+       (dq_dp && !D.alloc(&d_grad, (size_t)N * 6)) || (dq_di && !D.alloc(&d_gi, (size_t)N * 2 * Nintr)))
+        return false;
+    if(dq_di) MB200_CUDA_CHECK(cudaMemsetAsync(d_gi, 0, (size_t)N * 2 * Nintr * sizeof(double), D.stream));
+    L.a.intr = d_intr;
     const mrcal_lensmodel_metadata_t meta = mrcal_lensmodel_metadata(lensmodel);
     const int threads = 128, blocks = (N + threads - 1) / threads;
-    const bool ok = dispatch_lens_kind(kind, [&](auto k)
+    const bool ok = dispatch_lens_kind(L.kind, [&](auto k)
     {
         constexpr int K = decltype(k)::value;
-        if(unproject) unproject_kernel<K><<<blocks, threads>>>(a, S.d_in, N, S.d_out, meta.can_project_behind_camera);
-        else          project_kernel<K><<<blocks, threads>>>(a, S.d_in, N, S.d_out, S.d_grad, S.d_gi, Nintr);
+        if(unproject) unproject_kernel<K><<<blocks, threads, 0, D.stream>>>(L.a, d_in, N, d_out, meta.can_project_behind_camera);
+        else          project_kernel<K><<<blocks, threads, 0, D.stream>>>(L.a, d_in, N, d_out, d_grad, d_gi, Nintr);
     });
     if(!ok) return false;
     MB200_CUDA_CHECK(cudaGetLastError());
-    MB200_CUDA_CHECK(cudaMemcpy(out, S.d_out, nout * sizeof(double), cudaMemcpyDeviceToHost));
-    if(dq_dp) MB200_CUDA_CHECK(cudaMemcpy(dq_dp, S.d_grad, (size_t)N * 6 * sizeof(double), cudaMemcpyDeviceToHost));
-    if(dq_di) MB200_CUDA_CHECK(cudaMemcpy(dq_di, S.d_gi, (size_t)N * 2 * Nintr * sizeof(double), cudaMemcpyDeviceToHost));
-    return true;
+    return D.download(out, d_out, nout) && (!dq_dp || D.download(dq_dp, d_grad, (size_t)N * 6)) &&
+           (!dq_di || D.download(dq_di, d_gi, (size_t)N * 2 * Nintr)) && D.finish();
 }
 
 }  // namespace

@@ -15,6 +15,7 @@
 // is well under a millisecond, next to the factorization the region also needs.
 #include <vector>
 
+#include "device_call.h"
 #include "reduce.cuh"
 #include "solver_internal.h"
 
@@ -92,7 +93,7 @@ extern "C" bool mrcal_b200_problem_regional_statistics(mrcal_b200_problem_t* P, 
                                                        int gridn_width, int gridn_height, const double* q_cell_center,
                                                        const double* rcell, bool evaluate, double* stats, double* x)
 {
-    if(mrcal_b200_device_count() <= 0) { set_error("no usable CUDA device: libmrcal_b200 has no CPU fallback"); return false; }
+    if(!have_device()) return false;
     if(P == nullptr) { set_error("regional_statistics: no problem"); return false; }
     if(P->sharded) { set_error("regional_statistics: not available for sharded problems"); return false; }
     if(Ncameras < 0 || gridn_width < 2 || gridn_height < 2)

@@ -9,9 +9,9 @@
 #include <cfloat>
 
 #include "common.h"
+#include "device_call.h"
 #include "device_math.cuh"
 #include "lens_dispatch.cuh"
-#include "problem_impl.h"
 
 namespace mb200 {
 namespace {
@@ -409,13 +409,6 @@ bool compute_pinhole_cxy(double* cxy, double fxy, double tanazel0, double fov_de
     return true;
 }
 
-bool have_device()
-{
-    if(mrcal_b200_device_count() > 0) return true;
-    set_error("no usable CUDA device: libmrcal_b200 has no CPU fallback");
-    return false;
-}
-
 bool valid_rectification_model(mrcal_lensmodel_type_t t)
 {
     if(t == MRCAL_LENSMODEL_LATLON || t == MRCAL_LENSMODEL_PINHOLE) return true;
@@ -426,20 +419,6 @@ bool valid_rectification_model(mrcal_lensmodel_type_t t)
     else set_error("Invalid rectification_model_type for rectification: %s; I know about MRCAL_LENSMODEL_LATLON and "
                    "MRCAL_LENSMODEL_PINHOLE", name);
     return false;
-}
-
-struct Stream
-{
-    cudaStream_t s = nullptr;
-    ~Stream() { if(s) { cudaStreamSynchronize(s); cudaStreamDestroy(s); } }
-};
-
-template <typename T>
-bool upload(DeviceArena& mem, T** d, const T* h, size_t n, cudaStream_t s)
-{
-    if(!mem.alloc(d, n)) return false;
-    if(n) MB200_CUDA_CHECK(cudaMemcpyAsync(*d, h, n * sizeof(T), cudaMemcpyHostToDevice, s));
-    return true;
 }
 
 template <class F>
@@ -455,45 +434,31 @@ bool run_range(const RangeInput& host_in, const uint16_t* d16_host, int d16_stri
                double* range, int range_stride, double* p, mrcal_lensmodel_type_t rect, const double* fxycxy,
                double baseline)
 {
-    if(!have_device()) return false;
+    DeviceCall D;
+    if(!D.start()) return false;
     if(N <= 0) return true;
-    DeviceArena mem;   // freed after the stream has drained
-    Stream S;
-    MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
     RangeInput in = host_in;
     const long H = W > 0 ? N / W : 0;
-    if(d16_host)
-    {
-        uint16_t* d;
-        if(!mem.alloc(&d, (size_t)N)) return false;
-        MB200_CUDA_CHECK(cudaMemcpy2DAsync(d, W * sizeof(uint16_t), d16_host, d16_stride, W * sizeof(uint16_t), H,
-                                           cudaMemcpyHostToDevice, S.s));
-        in.d16 = d;
-    }
+    uint16_t* d_d16 = nullptr;
     double *d_d = nullptr, *d_ranges = nullptr, *d_q = nullptr, *d_range = nullptr, *d_p = nullptr;
-    if(host_in.d && !upload(mem, &d_d, host_in.d, (size_t)N, S.s)) return false;
-    if(host_in.ranges && !upload(mem, &d_ranges, host_in.ranges, (size_t)N, S.s)) return false;
-    if(host_in.q && !upload(mem, &d_q, host_in.q, 2 * (size_t)N, S.s)) return false;
-    in.d = d_d; in.ranges = d_ranges; in.q = d_q;
-    if(range && !mem.alloc(&d_range, (size_t)N)) return false;
-    if(p && !mem.alloc(&d_p, 3 * (size_t)N)) return false;
+    if((d16_host && !D.upload(&d_d16, d16_host, (size_t)d16_stride, (size_t)W, (size_t)H)) ||
+       (host_in.d && !D.upload(&d_d, host_in.d, (size_t)N)) ||
+       (host_in.ranges && !D.upload(&d_ranges, host_in.ranges, (size_t)N)) ||
+       (host_in.q && !D.upload(&d_q, host_in.q, 2 * (size_t)N)) || (range && !D.alloc(&d_range, (size_t)N)) ||
+       (p && !D.alloc(&d_p, 3 * (size_t)N)))
+        return false;
+    in.d16 = d_d16; in.d = d_d; in.ranges = d_ranges; in.q = d_q;
     const Fxycxy f{fxycxy[0], fxycxy[1], fxycxy[2], fxycxy[3]};
     const unsigned blocks = (unsigned)((N + 255) / 256);
     dispatch_rect(rect, [&](auto r)
     {
-        stereo_range_kernel<decltype(r)::value><<<blocks, 256, 0, S.s>>>(in, f, baseline, N, d_range, d_p);
+        stereo_range_kernel<decltype(r)::value><<<blocks, 256, 0, D.stream>>>(in, f, baseline, N, d_range, d_p);
     });
     MB200_CUDA_CHECK(cudaGetLastError());
-    if(range)
-    {
-        if(range_stride > 0)
-            MB200_CUDA_CHECK(cudaMemcpy2DAsync(range, range_stride, d_range, W * sizeof(double), W * sizeof(double), H,
-                                               cudaMemcpyDeviceToHost, S.s));
-        else MB200_CUDA_CHECK(cudaMemcpyAsync(range, d_range, N * sizeof(double), cudaMemcpyDeviceToHost, S.s));
-    }
-    if(p) MB200_CUDA_CHECK(cudaMemcpyAsync(p, d_p, 3 * N * sizeof(double), cudaMemcpyDeviceToHost, S.s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(S.s));
-    return true;
+    if(range && !(range_stride > 0 ? D.download(range, (size_t)range_stride, d_range, (size_t)W, (size_t)H)
+                                   : D.download(range, d_range, (size_t)N)))
+        return false;
+    return (!p || D.download(p, d_p, 3 * (size_t)N)) && D.finish();
 }
 
 }  // namespace
@@ -787,18 +752,12 @@ extern "C" bool mrcal_rectification_maps(float* rectification_maps,
         set_error("mrcal_rectification_maps() supports MRCAL_LENSMODEL_LATLON and MRCAL_LENSMODEL_PINHOLE only");
         return false;
     }
-    if(!have_device()) return false;
-    const mrcal_lensmodel_t* lms[2] = {lensmodel0, lensmodel1};
+    DeviceCall D;
+    if(!D.start()) return false;
     const double* intr[2] = {intrinsics0, intrinsics1};
     const double* r_cam_ref[2] = {r_cam0_ref, r_cam1_ref};
-    int kinds[2];
-    LensArgs a[2];
-    for(int c = 0; c < 2; c++)
-    {
-        kinds[c] = lens_kind_of(lms[c]);
-        if(kinds[c] < 0) { set_error("this lens model has no CUDA implementation"); return false; }
-        if(!lens_args_setup(&a[c], kinds[c], lms[c])) return false;
-    }
+    HostLens L[2];
+    if(!lens_setup(&L[0], lensmodel0) || !lens_setup(&L[1], lensmodel1)) return false;
     const int Naz = (int)imagersize_rectified[0], Nel = (int)imagersize_rectified[1];
     const long Npix = (long)Naz * Nel;
     if(Npix <= 0) return true;
@@ -819,33 +778,29 @@ extern "C" bool mrcal_rectification_maps(float* rectification_maps,
             }
     }
     const Fxycxy f{fxycxy_rectified[0], fxycxy_rectified[1], fxycxy_rectified[2], fxycxy_rectified[3]};
-    DeviceArena mem;   // freed after the stream has drained
-    Stream S;
-    MB200_CUDA_CHECK(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
     float2* d_map;
-    if(!mem.alloc(&d_map, 2 * (size_t)Npix)) return false;
+    if(!D.alloc(&d_map, 2 * (size_t)Npix)) return false;
     const unsigned blocks = (unsigned)((Npix + 127) / 128);
     for(int c = 0; c < 2; c++)
     {
         double* d_intr;
-        if(!upload(mem, &d_intr, intr[c], (size_t)mrcal_lensmodel_num_params(lms[c]), S.s)) return false;
-        a[c].intr = d_intr;
+        if(!D.upload(&d_intr, intr[c], (size_t)L[c].Nintr)) return false;
+        L[c].a.intr = d_intr;
         float2* out = d_map + c * Npix;
         bool ok = false;
         dispatch_rect(rectification_model_type, [&](auto r)
         {
             constexpr int RECT = decltype(r)::value;
-            ok = dispatch_lens_kind(kinds[c], [&](auto k)
+            ok = dispatch_lens_kind(L[c].kind, [&](auto k)
             {
-                rectification_maps_kernel<decltype(k)::value, RECT><<<blocks, 128, 0, S.s>>>(a[c], R[c], f, Naz, Npix, out);
+                rectification_maps_kernel<decltype(k)::value, RECT><<<blocks, 128, 0, D.stream>>>(
+                    L[c].a, R[c], f, Naz, Npix, out);
             });
         });
         if(!ok) return false;
     }
     MB200_CUDA_CHECK(cudaGetLastError());
-    MB200_CUDA_CHECK(cudaMemcpyAsync(rectification_maps, d_map, 2 * Npix * sizeof(float2), cudaMemcpyDeviceToHost, S.s));
-    MB200_CUDA_CHECK(cudaStreamSynchronize(S.s));
-    return true;
+    return D.download((float2*)rectification_maps, d_map, 2 * (size_t)Npix) && D.finish();
 }
 
 extern "C" bool mrcal_stereo_range_sparse(double* range, const double* disparity, const mrcal_point2_t* qrect0, const int N,

@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "device_math.cuh"
+#include "lens_dispatch.cuh"
 #include "reduce.cuh"
 #include "solver_internal.h"
 
@@ -273,15 +274,9 @@ bool launch_rows(const DevProblem& dp, const NormalBuffers& N, const RowArgs& A,
                  double* Bf, double* Bs, double* Bi, double* G, cudaStream_t s)
 {
     const unsigned blocks = (unsigned)((Npts + 127) / 128);
-#define MB200_LENS_CASE(K) case K: uncertainty_rows_kernel<K><<<blocks, 128, 0, s>>>(dp, N, A, pcam, Npts, Bf, Bs, Bi, G); break;
-    switch(dp.lens_kind)
-    {
-        MB200_LENS_CASE(LENS_PINHOLE) MB200_LENS_CASE(LENS_STEREOGRAPHIC) MB200_LENS_CASE(LENS_LONLAT) MB200_LENS_CASE(LENS_LATLON)
-        MB200_LENS_CASE(LENS_OPENCV4) MB200_LENS_CASE(LENS_OPENCV5) MB200_LENS_CASE(LENS_OPENCV8) MB200_LENS_CASE(LENS_OPENCV12)
-        MB200_LENS_CASE(LENS_SPLINED3) MB200_LENS_CASE(LENS_SPLINED2) MB200_LENS_CASE(LENS_CAHVOR) MB200_LENS_CASE(LENS_CAHVORE)
-    default: set_error("lens model kind %d has no CUDA implementation", dp.lens_kind); return false;
-    }
-#undef MB200_LENS_CASE
+    if(!dispatch_lens_kind(dp.lens_kind, [&](auto k)
+       { uncertainty_rows_kernel<decltype(k)::value><<<blocks, 128, 0, s>>>(dp, N, A, pcam, Npts, Bf, Bs, Bi, G); }))
+        return false;
     MB200_CUDA_CHECK(cudaGetLastError());
     return true;
 }

@@ -26,6 +26,7 @@ from . import _capi
 from ._capi import lib
 from .api import _compose_Rt, _lensmodel, _ptr, _require_gpu, lensmodel_metadata_and_config
 from .cameramodel import cameramodel
+from .image_transforms import _fail
 
 # the reference's Python wrapper takes an az0_deg above this for "autodetect" (mrcal-pywrap.c:4029-4030)
 _AZ0_AUTODETECT = 1e7
@@ -38,10 +39,6 @@ MATCH_OK, MATCH_EDGE_PEAK, MATCH_OUTSIDE_IMAGE1, MATCH_OUTSIDE_IMAGE0, MATCH_SEA
 
 def _rectification_model_type(name):
     return _lensmodel(name).type
-
-
-def _fail(what):
-    raise RuntimeError(f"{what} failed: {_capi.last_error()}")
 
 
 def rectified_resolution(model0, *, az_fov_deg, el_fov_deg, az0_deg, el0_deg, R_cam0_rect0,
