@@ -7,4 +7,4 @@ for c in (2,3):
     P = mrcal_b200.Problem(**kw)
     print('config',c,'callback ms with J', P.time_callback(20,True), 'no J', P.time_callback(20,False), 'nnz', P.N_j_nonzero)
 PY
-nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm --format=csv
+python -c 'import sys; sys.path.insert(0, "scripts"); import measure; print(measure.card())'

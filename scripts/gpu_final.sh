@@ -10,4 +10,3 @@ for k in ('value','ms_per_step','iterations_per_step','phase_ms_per_iteration','
 PY
 tail -3 gpurun_out/final_bench.err
 timeout 120 python scripts/spine_stamps.py 1270 > gpurun_out/spine_stamps.txt; tail -3 gpurun_out/spine_stamps.txt
-bash scripts/profile_r02.sh e 2>&1 | tail -42

@@ -16,9 +16,10 @@ between two waits, i.e. one trust-region step in a solver that waits once per st
   enqueue    host time from the previous wait's return to the last launch call of the interval
 
 Also the number of times the launch geometry that follows the size of the reduced system changes, and the typical
-step operation by operation (median idle time before each operation and its duration). Prints one JSON line; the
-Chrome trace is written to --out (default: a temporary directory). Tracing slows the host: the unprofiled
-ms_per_iteration is the number to quote, the profiled gaps are upper bounds.
+step operation by operation (median idle time before each operation and its duration). Prints one JSON line with the
+card's name, power limit and SM clocks, read in the same run; the Chrome trace is written to --out (default: a
+temporary directory). Tracing slows the host: the unprofiled ms_per_iteration is the number to quote, the profiled gaps
+are upper bounds.
 """
 import argparse
 import json
@@ -159,6 +160,7 @@ def main():
     import torch
     import mrcal_b200
     import bench
+    import measure
 
     kw = bench.problem_inputs(args.config)
     P = mrcal_b200.Problem(**kw)
@@ -173,6 +175,7 @@ def main():
     os.makedirs(out, exist_ok=True)
     P.reset()
     torch.cuda.synchronize()
+    # not measure.kernel_ms(): the cut at the host's waits needs the whole trace, host calls included
     acts = [torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]
     with torch.profiler.profile(activities=acts) as prof:
         info = P.optimize(max_iterations=args.max_iterations)
@@ -182,22 +185,14 @@ def main():
     with open(path) as f:
         trace = json.load(f)
     rows, changes = analyse(trace)
-    props = torch.cuda.get_device_properties(0)
-    power = None
-    try:
-        import subprocess
-        power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                               capture_output=True, text=True, timeout=20).stdout.strip()
-    except Exception:
-        pass
     ms_it = [p["ms_total"] / p["Niterations"] for p in plain]
-    print(json.dumps(dict(
-        config=args.config, device=props.name, power_limit=power,
+    measure.emit(dict(
+        config=args.config, device=torch.cuda.get_device_name(),
         unprofiled=dict(ms_per_iteration=ms_it, Niterations=plain[-1]["Niterations"], Nsyncs=plain[-1]["Nsyncs"],
                         Nevaluations=plain[-1]["Nevaluations"], Nfactorizations=plain[-1]["Nfactorizations"]),
         profiled=dict(intervals=len(rows), Niterations=info["Niterations"], Nsyncs=info["Nsyncs"],
                       nc_geometry_changes=changes, per_step=summarise(rows), typical_step=op_table(rows)),
-        trace=path)))
+        trace=path))
     return 0
 
 

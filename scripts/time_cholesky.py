@@ -2,26 +2,15 @@
 """Warm device timings of the dense Cholesky: the factorization (net of the refill with an SPD matrix that every call
 needs; the persistent kernel up to n = 8192, the multi-kernel chain above) and the persistent backward substitution of
 one right-hand side. One line per size, then one JSON line
-with the card's name and power limit, read in the same run. usage: time_cholesky.py n [n...]"""
+with the card's name, power limit and SM clocks, read in the same run. usage: time_cholesky.py n [n...]"""
 import ctypes as C
-import json
-import subprocess
 import sys
 sys.path.insert(0, ".")
 from mrcal_b200 import _capi
+import measure
 f = _capi.lib.mrcal_b200_debug_time_cholesky
 f.argtypes = [C.c_int, C.c_int, C.c_int]
 f.restype = C.c_double
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, limit = [s.strip() for s in out.split(",")]
-        return name, limit
-    except Exception:
-        return "unknown", "unknown"
 
 
 res = {}
@@ -31,5 +20,4 @@ for n in [int(a) for a in sys.argv[1:]] or [1268, 4820]:
     gf = n ** 3 / 3 / 1e9
     print(f"n={n}: factorization {factor:.3f} ms ({gf / factor:.1f} TFLOP/s, GFLOP={gf:.2f}); backward substitution {backward:.4f} ms")
     res[n] = {"factor_ms": round(factor, 4), "backward_ms": round(backward, 5)}
-name, limit = card()
-print(json.dumps({"cholesky": res, "card": name, "power_limit": limit}))
+measure.emit({"cholesky": res})

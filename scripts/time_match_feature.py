@@ -4,33 +4,30 @@ pair, 10 000 features, a 31 x 31 template, search radius 20, TM_CCORR_NORMED.
 
 The device call (numpy images: upload, kernels, one download) is warmed up, then timed as the median of 5 calls; each
 call returns numpy arrays, so it ends in a device synchronisation. The same with the images already on the device as
-torch tensors. The per-feature loops -- the numpy restatement (tests/match_np.py) and, where cv2 imports, the
-reference's own sequence of cv2.remap(), cv2.matchTemplate() and np.linalg.lstsq() -- are timed on a sample of features
-and extrapolated to all of them. Prints one JSON line, with the card, its power limit and its clocks.
+torch tensors, and the device time of each of its kernels and copies from torch.profiler. The per-feature loops -- the
+numpy restatement (tests/match_np.py) and, where cv2 imports, the reference's own sequence of cv2.remap(),
+cv2.matchTemplate() and np.linalg.lstsq() -- are timed on a sample of features and extrapolated to all of them. Prints
+one JSON line with the card's name, power limit and SM clocks as separate fields (card, power_limit, sm_clock,
+max_sm_clock), which replace the one unparsed `gpu` string this line used to carry.
 
     python scripts/time_match_feature.py [--features 10000] [--sample 100]"""
 import argparse
-import json
 import os
-import re
-import subprocess
 import sys
 import time
 
 import numpy as np
+import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import mrcal_b200  # noqa: E402
 import match_np  # noqa: E402
+import measure  # noqa: E402
 
-
-def gpu_info():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
-                               "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        return "unknown"
+# what one call with device images runs, in launch order; each is timed from torch.profiler
+KERNELS = ("Memcpy HtoD", "template_maps_kernel", "remap_kernel", "template_sums_kernel", "match_kernel",
+           "match_optimum_kernel", "Memcpy DtoH")
 
 
 def cv2_loop(cv2, image0, image1, q0, H10, r, ts):
@@ -68,30 +65,15 @@ def main():
     H10[:, :2, 2] = (-5., -3.)
     kw = dict(search_radius1=r, template_size1=ts, H10=H10)
 
-    def median_ms(f, n=5):
-        f()
-        t = []
-        for _ in range(n):
-            t0 = time.perf_counter()
-            f()
-            t.append(time.perf_counter() - t0)
-        return 1e3 * float(np.median(t))
-
-    out = dict(gpu=gpu_info(), features=a.features, image=f"{W}x{H} uint8", template=ts, search_radius=r,
-               method="TM_CCORR_NORMED")
+    out = dict(features=a.features, image=f"{W}x{H} uint8", template=ts, search_radius=r, method="TM_CCORR_NORMED")
     q1, d = mrcal_b200.match_feature(image0, image1, q0, **kw)
     out["matched"] = int(np.sum(d["status"] == mrcal_b200.MATCH_OK))
-    out["device_numpy_ms"] = median_ms(lambda: mrcal_b200.match_feature(image0, image1, q0, **kw))
-    try:
-        import torch
-        t0, t1 = torch.from_numpy(image0).cuda(), torch.from_numpy(image1).cuda()
-        out["device_torch_ms"] = median_ms(lambda: mrcal_b200.match_feature(t0, t1, q0, **kw))
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            mrcal_b200.match_feature(t0, t1, q0, **kw)
-        out["kernels_us"] = {(re.search(r"\w+_kernel|Memcpy \w+", e.key) or re.search(".*", e.key))[0]:
-                             round(e.device_time_total, 1) for e in prof.key_averages() if e.device_time_total > 0}
-    except ImportError:
-        pass
+    out["device_numpy_ms"] = measure.median_ms(lambda: mrcal_b200.match_feature(image0, image1, q0, **kw), 5)
+    t0, t1 = torch.from_numpy(image0).cuda(), torch.from_numpy(image1).cuda()
+    device_call = lambda: mrcal_b200.match_feature(t0, t1, q0, **kw)
+    out["device_torch_ms"] = measure.median_ms(device_call, 5)
+    out["kernels_us"] = {k: round(1e3 * measure.kernel_ms(device_call, k), 1) for k in KERNELS}
+    # the host loops take seconds per hundred features: one pass over a sample, extrapolated to all the features
     s = rng.choice(a.features, a.sample, replace=False)
     t = time.perf_counter()
     for i in s:
@@ -104,7 +86,7 @@ def main():
         out["cv2_loop_ms_extrapolated"] = 1e3 * (time.perf_counter() - t) / a.sample * a.features
     except ImportError:
         out["cv2_loop_ms_extrapolated"] = None
-    print(json.dumps(out))
+    measure.emit(out)
 
 
 if __name__ == "__main__":

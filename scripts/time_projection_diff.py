@@ -4,12 +4,9 @@ implied transformation and the reprojection. Cases: the test models cam0 OPENCV8
 BASELINE config 3 at infinity, weighted by their uncertainties, on the 60-wide grid. Each fit is also timed on the
 route the reference takes, the scipy fit of tests/diff_np.py, followed by mrcal_b200.project() and the difference in
 numpy. Times are medians in ms; every timed call ends with a device synchronisation. Prints one JSON line with the
-card's name and power limit, read in the same run."""
-import json
+card's name, power limit and SM clocks, read in the same run."""
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 
@@ -19,26 +16,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import mrcal_b200  # noqa: E402
 from mrcal_b200 import synthetic  # noqa: E402
 import diff_np  # noqa: E402
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, limit = [s.strip() for s in out.split(",")]
-        return name, limit
-    except Exception:
-        return "unknown", "unknown"
-
-
-def timed(f, reps):
-    f()   # warm-up
-    t = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        f()
-        t.append(time.perf_counter() - t0)
-    return 1e3 * float(np.median(t))
+import measure  # noqa: E402
 
 
 def reproject(Rt, q0, v, distance, lms, intr):
@@ -65,30 +43,33 @@ def case(models, gridn, distance, use_uncertainties, reps):
     atinfinity = distance is None
     d = 1. if atinfinity else distance
     unp = lambda: mrcal_b200.sample_imager_unproject(gridn, None, W, H, lms, intr, normalize=True)
-    res["ms_unproject"] = timed(unp, reps)
+    res["ms_unproject"] = measure.median_ms(unp, reps)
     v, q0 = unp()
     w = None
     if use_uncertainties:
         unc = lambda: [mrcal_b200.projection_uncertainty(v[k] * d, models[k], atinfinity=atinfinity,
                                                          what="worstdirection-stdev") for k in range(2)]
-        res["ms_uncertainties"] = timed(unc, reps)
+        res["ms_uncertainties"] = measure.median_ms(unc, reps)
         u = unc()
         w = (1. / (u[0] * u[1])) ** 2
         center, radius = ((W - 1) / 2., (H - 1) / 2.), max(W, H) * 100.
     else:
         center, radius = ((W - 1) / 2., (H - 1) / 2.), min(W, H) / 6.
     kw = dict(weights=w, atinfinity=atinfinity, focus_center=center, focus_radius=radius)
-    res["ms_fit"] = timed(lambda: mrcal_b200.implied_Rt10__from_unprojections(q0, v[0] * d, v[1], **kw), reps)
+    res["ms_fit"] = measure.median_ms(
+        lambda: mrcal_b200.implied_Rt10__from_unprojections(q0, v[0] * d, v[1], **kw), reps)
     Rt = mrcal_b200.implied_Rt10__from_unprojections(q0, v[0] * d, v[1], **kw)
-    res["ms_reproject"] = timed(lambda: reproject(Rt, q0, v, None if atinfinity else distance, lms, intr), reps)
+    res["ms_reproject"] = measure.median_ms(
+        lambda: reproject(Rt, q0, v, None if atinfinity else distance, lms, intr), reps)
     dist = None if atinfinity else distance
-    res["ms_total"] = timed(lambda: mrcal_b200.projection_diff(models, gridn_width=gridn, distance=dist,
-                                                               use_uncertainties=use_uncertainties), reps)
+    res["ms_total"] = measure.median_ms(lambda: mrcal_b200.projection_diff(models, gridn_width=gridn, distance=dist,
+                                                                           use_uncertainties=use_uncertainties), reps)
 
     def composed():
         Rt_ref = diff_np.fit(q0, v[0] * d, v[1], **kw)
         return mrcal_b200.project(v[0] * d @ Rt_ref[:3].T + Rt_ref[3], lms[1], intr[1]) - q0
-    res["ms_composed_fit_and_reproject"] = timed(composed, 1)
+    # the scipy fit takes up to a second: one call after the warm-up
+    res["ms_composed_fit_and_reproject"] = measure.median_ms(composed, 1)
     Rt_ref = diff_np.fit(q0, v[0] * d, v[1], **kw)
     res["cost_device_over_scipy"] = (diff_np.robust_cost(Rt, q0, v[0] * d, v[1], **kw) /
                                      diff_np.robust_cost(Rt_ref, q0, v[0] * d, v[1], **kw))
@@ -106,9 +87,7 @@ def main():
     mrcal_b200.optimize(**kw)
     cams = [mrcal_b200.cameramodel(optimization_inputs=kw, icam_intrinsics=i) for i in (0, 1)]
     out["config3_cam0_vs_cam1_infinity_uncertainties_grid60"] = case(cams, 60, None, True, 3)
-    name, limit = card()
-    out.update(card=name, power_limit=limit)
-    print(json.dumps(out))
+    measure.emit(out)
 
 
 if __name__ == "__main__":

@@ -4,59 +4,23 @@ optimizer_callback() returns at BASELINE configs 3 and 5, and the dense CHOLMOD_
 
 For each factor, sys in (A, L, Lt) and nrhs: the median wall time of a call (every call ends in a device
 synchronisation; it includes the copies of the right-hand sides both ways), after a warm-up call, and the device time
-of the call's kernels from torch.profiler in a separate call. One JSON line per point, then one with the card's name
-and power limit, read in the same run. --out also writes the lines to a file."""
+of the call's kernels from torch.profiler in a separate call. One JSON line per point, each with the card's name, power
+limit and SM clocks, read as that point is written. --out also writes the lines to a file."""
 import argparse
-import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import scipy.sparse
-import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import mrcal_b200  # noqa: E402
 from mrcal_b200 import synthetic  # noqa: E402
+import measure  # noqa: E402
 
 NRHS = (1, 2, 8, 32, 64, 128, 256, 512, 3960)
 SYSTEMS = ("A", "L", "Lt")
 FACTORS = ("config3", "config5", "dense1100", "dense8300")
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, limit = [s.strip() for s in out.split(",")]
-        return name, limit
-    except Exception:
-        return "unknown", "unknown"
-
-
-def timed(f):
-    """median ms of a call after a warm-up; fewer repetitions for slow calls"""
-    t0 = time.perf_counter()
-    f()
-    first = time.perf_counter() - t0
-    reps = 7 if first < 0.05 else (3 if first < 1. else 1)
-    t = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        f()
-        t.append(time.perf_counter() - t0)
-    return 1e3 * float(np.median(t))
-
-
-def kernel_ms(f):
-    """device time of the kernels of one call of f, from torch.profiler"""
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        f()
-        torch.cuda.synchronize()
-    us = sum(e.device_time_total for e in prof.events() if not e.name.startswith(("Memcpy", "Memset")))
-    return us / 1e3
 
 
 def make_factor(name):
@@ -76,13 +40,8 @@ def main():
     ap.add_argument("--nrhs", default=",".join(map(str, NRHS)))
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
-    lines = []
-
-    def emit(d):
-        print(json.dumps(d), flush=True)
-        lines.append(json.dumps(d))
-
-    torch.zeros(1, device="cuda")   # the profiler's CUDA context
+    if args.out:
+        open(args.out, "w").close()   # emit() appends each point's line
     nrhs_all = [int(v) for v in args.nrhs.split(",")]
     for fname in args.factors.split(","):
         F, n = make_factor(fname)
@@ -93,14 +52,13 @@ def main():
 
                 def call():
                     return F.solve_xt_JtJ_bt(bt, sys=sys_)
-                emit(dict(factor=fname, n=n, sys=sys_, nrhs=nrhs, ms_call=round(timed(call), 4),
-                          ms_kernels=round(kernel_ms(call), 4)))
+                # the warm-up call is timed too, to take fewer repetitions of slow calls
+                first = measure.median_ms(call, 1, warmup=0)
+                ms_call = measure.median_ms(call, 7 if first < 50 else (3 if first < 1000 else 1), warmup=0)
+                # every kernel of the library is named *_kernel; the copies of the right-hand sides are left out
+                measure.emit(dict(factor=fname, n=n, sys=sys_, nrhs=nrhs, ms_call=round(ms_call, 4),
+                                  ms_kernels=round(measure.kernel_ms(call, "_kernel"), 4)), args.out)
         del F
-    name, limit = card()
-    emit(dict(card=name, power_limit=limit))
-    if args.out:
-        with open(args.out, "w") as f:
-            f.write("\n".join(lines) + "\n")
 
 
 if __name__ == "__main__":

@@ -2,50 +2,18 @@
 at full resolution (pixels_per_deg = -1), and the dense stereo_range() / stereo_unproject() on a whole rectified image.
 For each, the call (arguments, upload, kernels, copy back into numpy) and the device time of its kernels alone
 (torch.profiler). Where oracle/_ref was built, the reference's single-threaded C for the same maps and ranges.
-Times are medians in ms. Prints one JSON line with the card's name and power limit, read in the same run."""
-import json
+Times are medians in ms. Prints one JSON line with the card's name, power limit and SM clocks, read in the same run."""
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
-import torch
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
 import mrcal_b200  # noqa: E402
 from mrcal_b200.seeding import rt_from_Rt  # noqa: E402
 from oracle import stereo_ref as ref  # noqa: E402
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, limit = [s.strip() for s in out.split(",")]
-        return name, limit
-    except Exception:
-        return "unknown", "unknown"
-
-
-def timed(f, reps):
-    f()   # warm-up
-    t = []
-    for _ in range(reps):
-        t0 = time.perf_counter()
-        f()
-        t.append(time.perf_counter() - t0)
-    return 1e3 * float(np.median(t))
-
-
-def kernel_ms(f, name):
-    """device time of the kernels whose name contains `name` in one call of f, from torch.profiler"""
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        f()
-        torch.cuda.synchronize()
-    us = sum(e.device_time_total for e in prof.events() if name in e.name)
-    return us / 1e3
+import measure  # noqa: E402
 
 
 def pair(names, rt01=(0.1, 0.2, 0.05, 3.0, 0.2, 1.0)):
@@ -64,34 +32,32 @@ def case(models, reps):
     W, H = (int(x) for x in rect[0].imagersize())
     res["rectified_imager"] = [W, H]
     maps = lambda: mrcal_b200.rectification_maps(models, rect)
-    res["ms_maps_call"] = timed(maps, reps)
-    res["ms_maps_kernels"] = kernel_ms(maps, "rectification_maps_kernel")
+    res["ms_maps_call"] = measure.median_ms(maps, reps)
+    res["ms_maps_kernels"] = measure.kernel_ms(maps, "rectification_maps_kernel")
     d = np.random.default_rng(0).integers(0, 2000, size=(H, W)).astype(np.uint16)
     rng = lambda: mrcal_b200.stereo_range(d, rect, disparity_scale=16)
     unp = lambda: mrcal_b200.stereo_unproject(d, rect, disparity_scale=16)
-    res["ms_range_call"] = timed(rng, reps)
-    res["ms_range_kernel"] = kernel_ms(rng, "stereo_range_kernel")
-    res["ms_unproject_call"] = timed(unp, reps)
-    res["ms_unproject_kernel"] = kernel_ms(unp, "stereo_range_kernel")
+    res["ms_range_call"] = measure.median_ms(rng, reps)
+    res["ms_range_kernel"] = measure.kernel_ms(rng, "stereo_range_kernel")
+    res["ms_unproject_call"] = measure.median_ms(unp, reps)
+    res["ms_unproject_kernel"] = measure.kernel_ms(unp, "stereo_range_kernel")
     if ref.available():
         f, size, r = rect[0].intrinsics()[1], rect[0].imagersize(), rect[0].rt_cam_ref()[:3]
         args = (*models[0].intrinsics(), models[0].rt_cam_ref()[:3], *models[1].intrinsics(), models[1].rt_cam_ref()[:3],
                 "LENSMODEL_LATLON", f, size, r)
-        res["ms_maps_reference_c"] = timed(lambda: ref.rectification_maps(*args), 1)
+        # the reference's maps take about a second on one thread: one call after the warm-up
+        res["ms_maps_reference_c"] = measure.median_ms(lambda: ref.rectification_maps(*args), 1)
         baseline = float(np.linalg.norm(rect[0].rt_cam_ref()[3:] - rect[1].rt_cam_ref()[3:]))
-        res["ms_range_reference_c"] = timed(lambda: ref.stereo_range_dense(d, 16, 0, 65535, "LENSMODEL_LATLON", f,
-                                                                           baseline), 3)
+        res["ms_range_reference_c"] = measure.median_ms(
+            lambda: ref.stereo_range_dense(d, 16, 0, 65535, "LENSMODEL_LATLON", f, baseline), 3)
     return res
 
 
 def main():
-    torch.cuda.init()
     out = {}
     out["splined_pair"] = case(pair(("cam0.splined.cameramodel", "cam1.splined.cameramodel")), 5)
     out["opencv8_pair"] = case(pair(("cam0.opencv8.cameramodel", "cam0.opencv8.cameramodel")), 5)
-    name, limit = card()
-    out.update(card=name, power_limit=limit)
-    print(json.dumps(out))
+    measure.emit(out)
 
 
 if __name__ == "__main__":
