@@ -323,6 +323,26 @@ bool mrcal_project(mrcal_point2_t* q, mrcal_point3_t* dq_dp, double* dq_dintrins
 // into the rays of mrcal_observation_point_triangulated_t (mrcal-pywrap.c:1383-1401)
 bool mrcal_unproject(mrcal_point3_t* out, const mrcal_point2_t* q, int N,
                      const mrcal_lensmodel_t* lensmodel, const double* intrinsics);
+/* The unprojection of N pixels with its gradients, as mrcal.unproject(normalize=, get_gradients=) returns it
+   (mrcal/projections.py:112-397). dv_dq (N,3,2) and dv_dintrinsics (N,3,Nintrinsics; dense) may be NULL. With neither,
+   v is mrcal_unproject()'s, or with normalize its unit vector (the zero vector where the unprojection failed). With
+   either: the closed-form models (pinhole, stereographic, lonlat, latlon) give their closed-form ray and derivatives;
+   the others give v = unproject_stereographic(project_stereographic(mrcal_unproject())) -- the same direction, a
+   different magnitude where mrcal_unproject() flipped a point to the front -- with dv/dq = dv/du (dq/du)^-1 in its
+   stereographic coordinates u, and dv/dintrinsics = -dv/dq dq/dintrinsics. normalize: unit rays and the gradients of
+   the unit rays. A failed unprojection or a singular dq/du gives NaN. Refuses CAHVORE with E != 0. False +
+   mrcal_b200_last_error() on refusal or failure */
+bool mrcal_b200_unproject_with_gradients(mrcal_point3_t* v, double* dv_dq, double* dv_dintrinsics,
+                                         const mrcal_point2_t* q, int N, const mrcal_lensmodel_t* lensmodel,
+                                         const double* intrinsics, bool normalize);
+/* The angular resolution of a camera in degrees per pixel at N pixels, as mrcal.model_resolution__deg_pixel()
+   computes it (mrcal/model_analysis.py:2152-2246): from the eigenvalues of M'M, M = dq/dv [u0 u1] at the unit ray v
+   of each pixel, [u0 u1] an orthonormal basis of the plane perpendicular to v, the smaller one clamped at 1e-6. mode:
+   one of MB200_RESOLUTION_*. One fused kernel. Refuses CAHVORE with E != 0. False + mrcal_b200_last_error() on refusal
+   or failure */
+enum { MB200_RESOLUTION_MEAN = 0, MB200_RESOLUTION_MIN = 1, MB200_RESOLUTION_MAX = 2, MB200_RESOLUTION_ECCENTRICITY = 3 };
+bool mrcal_b200_model_resolution__deg_pixel(double* resolution, const mrcal_point2_t* q, int N,
+                                            const mrcal_lensmodel_t* lensmodel, const double* intrinsics, int mode);
 
 // Stereo (replaces stereo.h:15-173, stereo.c:19-972, 1242-1417). Host buffers in and out, as in the reference.
 // The geometry is host code; the maps and the ranges are computed on the device, one thread per element.
@@ -662,6 +682,15 @@ bool mrcal_b200_projection_diff(double* Rt10, double* difflen, double* diff,
                                 const mrcal_lensmodel_t* lensmodels, const double* intrinsics,
                                 const double* uncertainties, const double* focus_center, double focus_radius,
                                 bool fit_Rt10);
+
+/* The reprojection of pixels q [N] from camera 0 to camera 1 of Npairs (1 or 2) camera pairs, as mrcal.stereo_pair_diff()
+   computes it (mrcal/model_analysis.py:1931-2103): q1_p = project_p1(R_p (distance unproject_p0(q, normalized)) + t_p)
+   with Rt10 [Npairs][4][3] (R, then t). lensmodels [Npairs][2] and their intrinsics, concatenated in that order. out
+   [N][2] is q1_0 for one pair and q1_1 - q1_0 for two; outlen [N] (may be NULL) is |out|. Refuses a camera 0 that is
+   CAHVORE with E != 0. False + mrcal_b200_last_error() on refusal or failure */
+bool mrcal_b200_stereo_pair_reproject(double* out, double* outlen, const mrcal_point2_t* q, int N, int Npairs,
+                                      const mrcal_lensmodel_t* lensmodels, const double* intrinsics, const double* Rt10,
+                                      double distance);
 
 // The point cloud of disparities in rectified camera-0 coordinates, as mrcal.stereo_unproject() computes it
 // (mrcal/stereo.py:1453-1607) in one pass on the device: p[k] = range[k] * normalize(unproject_rect(qrect0[k])),

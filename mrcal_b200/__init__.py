@@ -16,6 +16,9 @@ from .api import (  # noqa: F401
     num_measurements, num_measurements_boards, num_measurements_points,
     num_measurements_points_triangulated, num_measurements_regularization,
     corresponding_icam_extrinsics, pack_state, unpack_state, project, unproject,
+    project_pinhole, unproject_pinhole, project_stereographic, unproject_stereographic,
+    project_lonlat, unproject_lonlat, project_latlon, unproject_latlon,
+    model_resolution__deg_pixel, stereo_pair_diff,
     _Jt_x, _A_Jt_J_At, _A_Jt_J_At__2,
 )
 from .seeding import (  # noqa: F401

@@ -92,6 +92,7 @@ SELECTION_BITS = ("do_optimize_intrinsics_core",
 # every symbol include/mrcal_b200.h declares; tests check the .so exports each
 EXPORTED_SYMBOLS = (
     "_mrcal_precompute_lensmodel_data", "mrcal_project", "mrcal_unproject", "mrcal_b200_problem_create_triangulated",
+    "mrcal_b200_unproject_with_gradients", "mrcal_b200_model_resolution__deg_pixel", "mrcal_b200_stereo_pair_reproject",
     "mrcal_lensmodel_from_name", "mrcal_lensmodel_type_from_name", "mrcal_lensmodel_name",
     "mrcal_lensmodel_name_unconfigured", "mrcal_lensmodel_metadata", "mrcal_lensmodel_num_params",
     "mrcal_supported_lensmodel_names", "mrcal_knots_for_splined_models",
@@ -187,6 +188,12 @@ lib.mrcal_b200_projection_diff.restype = C.c_bool
 lib.mrcal_b200_projection_diff.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
                                            C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                            C.c_double, C.c_bool]
+lib.mrcal_b200_unproject_with_gradients.restype = C.c_bool
+lib.mrcal_b200_unproject_with_gradients.argtypes = [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_void_p, C.c_bool]
+lib.mrcal_b200_model_resolution__deg_pixel.restype = C.c_bool
+lib.mrcal_b200_model_resolution__deg_pixel.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+lib.mrcal_b200_stereo_pair_reproject.restype = C.c_bool
+lib.mrcal_b200_stereo_pair_reproject.argtypes = [C.c_void_p] * 3 + [C.c_int] * 2 + [C.c_void_p] * 3 + [C.c_double]
 for _n in ["mrcal_rectified_resolution", "mrcal_rectified_system2", "mrcal_rectified_system", "mrcal_rectification_maps",
            "mrcal_stereo_range_sparse", "mrcal_stereo_range_dense", "mrcal_b200_stereo_unproject"]:
     getattr(lib, _n).restype = C.c_bool

@@ -543,6 +543,101 @@ def projection_diff(models, *, implied_Rt10=None, gridn_width=60, gridn_height=N
     return difflen, diff, q0, (Rt10[0] if Nmodels == 2 else Rt10)
 
 
+_RESOLUTION_MODES = {"mean": 0, "min": 1, "max": 2, "eccentricity": 3}   # MB200_RESOLUTION_* in mrcal_b200.h
+
+
+def model_resolution__deg_pixel(q, model, *, mode="mean"):
+    """The angular resolution of the camera of `model` at pixels q (...,2), in degrees per pixel, as
+    mrcal.model_resolution__deg_pixel() computes it (mrcal/model_analysis.py:2152-2246): from the sensitivity of the
+    projection to motions perpendicular to each unit ray. mode 'min' and 'max' report the finest and the coarsest
+    direction, 'mean' their average and 'eccentricity' max/min. One fused kernel on the device (csrc/project.cu)"""
+    if mode not in _RESOLUTION_MODES:
+        raise RuntimeError("Mode must be one of ('min','max','mean','eccentricity')")
+    _require_gpu()
+    q = np.ascontiguousarray(q, dtype=np.float64)
+    if q.shape[-1:] != (2,):
+        raise RuntimeError(f"q must have shape (...,2); got {q.shape}")
+    lensmodel, intrinsics = model.intrinsics()
+    lm = _lensmodel(lensmodel)
+    intr = np.ascontiguousarray(intrinsics, dtype=np.float64)
+    flat = q.reshape(-1, 2)
+    out = np.zeros(flat.shape[0])
+    if not lib.mrcal_b200_model_resolution__deg_pixel(_ptr(out), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr),
+                                                      _RESOLUTION_MODES[mode]):
+        raise RuntimeError("model_resolution__deg_pixel() failed: " + _capi.last_error())
+    return out.reshape(q.shape[:-1])
+
+
+def _invert_Rt(Rt):
+    return np.vstack((Rt[:3].T, -Rt[:3].T @ Rt[3]))
+
+
+def _stereo_pair_reproject(q, models, Rts, distance):
+    """out, |out|: the pixels q (...,2) of camera 0 of each (camera 0, camera 1) pair in models, reprojected into its
+    camera 1 through Rt (4,3) from camera 0 to camera 1: q1 for one pair, q1[1] - q1[0] for two"""
+    q = np.ascontiguousarray(q, dtype=np.float64)
+    if q.shape[-1:] != (2,):
+        raise RuntimeError(f"q must have shape (...,2); got {q.shape}")
+    flat = q.reshape(-1, 2)
+    lms = (_capi.Lensmodel * len(models))(*[_lensmodel(lm) for lm, _ in models])
+    intr = np.ascontiguousarray(np.concatenate([i for _, i in models]), np.float64)
+    Rt = np.ascontiguousarray(Rts, np.float64)
+    out = np.zeros(flat.shape)
+    outlen = np.zeros(flat.shape[0])
+    if not lib.mrcal_b200_stereo_pair_reproject(_ptr(out), _ptr(outlen), _ptr(flat), flat.shape[0], len(models) // 2,
+                                                lms, _ptr(intr), _ptr(Rt), float(distance)):
+        raise RuntimeError("stereo_pair_diff() failed: " + _capi.last_error())
+    return out.reshape(q.shape), outlen.reshape(q.shape[:-1])
+
+
+def stereo_pair_diff(model_pairs, *, gridn_width=60, gridn_height=None, distance=None):
+    """The difference between two calibrations of a camera pair, intrinsics and extrinsics together, as
+    mrcal.stereo_pair_diff() computes it (mrcal/model_analysis.py:1931-2103): a grid q0 over the imager of camera 0 is
+    unprojected by each pair's camera 0 to the distance (infinity if None: distance 1 and no translation), mapped to
+    camera 1 by that pair's Rt10 = Rt_cam_ref(m1) Rt_ref_cam(m0) and projected by its camera 1. Returns (difflen, diff,
+    q0, reproject_pairp_from_cami): diff (Nh, Nw, 2) = q1[pair 1] - q1[pair 0], difflen its length, q0 the grid (Nh, Nw,
+    2), and reproject_pairp_from_cami(q, p, i) mapping pixels q of camera i of pair p to the other camera of that pair.
+    A noncentral CAHVORE model is centralized (E = 0) in a copy where that is exact (|E|^2 < 1e-12) or at infinity. The
+    unprojections and reprojections run on the device (csrc/diff.cu)"""
+    if len(model_pairs) != 2:
+        raise RuntimeError("Exactly 2 model_pairs are expected")
+    Rt10_pairs = np.array([_compose_Rt(m1.Rt_cam_ref(), m0.Rt_ref_cam()) for m0, m1 in model_pairs])
+    atinfinity = distance is None
+    if atinfinity:
+        distance = 1.
+        Rt10_pairs[:, 3, :] = 0
+    intrinsics = [[m.intrinsics() for m in pair] for pair in model_pairs]
+    for pair in intrinsics:
+        for i, (lm, intr) in enumerate(pair):
+            if not lensmodel_metadata_and_config(lm)["noncentral"]:
+                continue
+            if not re.match("LENSMODEL_CAHVORE_", lm):
+                raise RuntimeError("I have a noncentral model that I cannot centralize. unproject() isn't implemented "
+                                   "yet in this case")
+            if np.sum(intr[-3:] ** 2) < 1e-12 or atinfinity:
+                intr = np.array(intr, np.float64)
+                intr[-3:] = 0
+                pair[i] = (lm, intr)
+                continue
+            raise RuntimeError("I have a noncentral model. I can centralize it, but that's only valid at infinity")
+    imagersizes0 = np.array([pair[0].imagersize() for pair in model_pairs])
+    if np.any(imagersizes0[1] - imagersizes0[0]):
+        raise RuntimeError("The first camera in each given pair MUST have identical imager dimensions")
+    imagersizes1 = np.array([pair[1].imagersize() for pair in model_pairs])
+    if np.any(imagersizes1[1] - imagersizes1[0]):
+        raise RuntimeError("The second camera in each given pair must have identical imager dimensions. I technically "
+                           "don't NEED this, but it's extremely likely to be an unintentional mistake by the caller")
+    Rt10_Rt01_pairs = (Rt10_pairs, np.array([_invert_Rt(Rt) for Rt in Rt10_pairs]))
+    d = float(distance)
+
+    def reproject_pairp_from_cami(q, p, i):
+        return _stereo_pair_reproject(q, (intrinsics[p][i], intrinsics[p][1 - i]), Rt10_Rt01_pairs[i][p][None], d)[0]
+
+    q0 = sample_imager(gridn_width, gridn_height, *imagersizes0[0])
+    diff, difflen = _stereo_pair_reproject(q0, intrinsics[0] + intrinsics[1], Rt10_pairs, d)
+    return difflen, diff, q0, reproject_pairp_from_cami
+
+
 def optimizer_callback(no_jacobian=False, no_factorization=False, **kwargs):
     """One evaluation of the cost function at the given seed.
 
@@ -1238,9 +1333,13 @@ def project(v, lensmodel, intrinsics_data, get_gradients=False):
     return q, g.reshape(v.shape[:-1] + (2, 3)), gi.reshape(v.shape[:-1] + (2, intr.shape[0]))
 
 
-def unproject(q, lensmodel, intrinsics_data):
-    """Observation rays (not normalised) of pixels q (...,2): the reference's mrcal.unproject() without
-    gradients (mrcal.h:193-224)."""
+def unproject(q, lensmodel, intrinsics_data, *, normalize=False, get_gradients=False):
+    """Observation rays of pixels q (...,2), as the reference's mrcal.unproject() returns them
+    (mrcal/projections.py:112-397). Returns v (...,3); with get_gradients, (v, dv_dq (...,3,2), dv_dintrinsics
+    (...,3,Nintrinsics), dense). The rays are not normalised unless normalize; then the gradients are those of the unit
+    rays. As in the reference, the magnitude of an unnormalised ray may change with get_gradients: the gradients are
+    those of the ray returned with them. A pixel that cannot be unprojected gives NaN (the zero vector with normalize
+    and no gradients)."""
     _require_gpu()
     q = np.ascontiguousarray(q, dtype=np.float64)
     if q.shape[-1] != 2:
@@ -1249,6 +1348,82 @@ def unproject(q, lensmodel, intrinsics_data):
     intr = np.ascontiguousarray(intrinsics_data, dtype=np.float64)
     flat = q.reshape(-1, 2)
     v = np.zeros((flat.shape[0], 3))
-    if not lib.mrcal_unproject(_ptr(v), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr)):
-        raise RuntimeError("mrcal_unproject() failed: " + _capi.last_error())
-    return v.reshape(q.shape[:-1] + (3,))
+    if not normalize and not get_gradients:
+        if not lib.mrcal_unproject(_ptr(v), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr)):
+            raise RuntimeError("mrcal_unproject() failed: " + _capi.last_error())
+        return v.reshape(q.shape[:-1] + (3,))
+    Nintr = lib.mrcal_lensmodel_num_params(C.byref(lm))
+    if intr.shape != (Nintr,):
+        raise RuntimeError(f"unproject(): intrinsics_data must have shape ({Nintr},)")
+    g = np.zeros((flat.shape[0], 3, 2)) if get_gradients else None
+    gi = np.zeros((flat.shape[0], 3, Nintr)) if get_gradients else None
+    if not lib.mrcal_b200_unproject_with_gradients(_ptr(v), _ptr(g), _ptr(gi), _ptr(flat), flat.shape[0], C.byref(lm),
+                                                   _ptr(intr), bool(normalize)):
+        raise RuntimeError("unproject() failed: " + _capi.last_error())
+    v = v.reshape(q.shape[:-1] + (3,))
+    if not get_gradients:
+        return v
+    return v, g.reshape(q.shape[:-1] + (3, 2)), gi.reshape(q.shape[:-1] + (3, Nintr))
+
+
+_FXYCXY_IDENTITY = np.array((1.0, 1.0, 0.0, 0.0))
+
+
+def _project_closed_form(lensmodel, points, fxycxy, get_gradients):
+    if not get_gradients:
+        return project(points, lensmodel, fxycxy)
+    q, dq_dp, _ = project(points, lensmodel, fxycxy, get_gradients=True)
+    return q, dq_dp
+
+
+def _unproject_closed_form(lensmodel, points, fxycxy, get_gradients):
+    if not get_gradients:
+        return unproject(points, lensmodel, fxycxy)
+    v, dv_dq, _ = unproject(points, lensmodel, fxycxy, get_gradients=True)
+    return v, dv_dq
+
+
+def project_pinhole(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+    """q = (f x/z + c) of points (...,3), as mrcal.project_pinhole(); with get_gradients, (q, dq_dp (...,2,3))"""
+    return _project_closed_form("LENSMODEL_PINHOLE", points, fxycxy, get_gradients)
+
+
+def unproject_pinhole(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+    """v = ((q - c)/f, 1) of pixels (...,2), as mrcal.unproject_pinhole(); with get_gradients, (v, dv_dq (...,3,2))"""
+    return _unproject_closed_form("LENSMODEL_PINHOLE", points, fxycxy, get_gradients)
+
+
+def project_stereographic(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+    """The stereographic projection of points (...,3), as mrcal.project_stereographic(); with get_gradients,
+    (q, dq_dp (...,2,3))"""
+    return _project_closed_form("LENSMODEL_STEREOGRAPHIC", points, fxycxy, get_gradients)
+
+
+def unproject_stereographic(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+    """The stereographic unprojection of pixels (...,2), as mrcal.unproject_stereographic(); with get_gradients,
+    (v, dv_dq (...,3,2))"""
+    return _unproject_closed_form("LENSMODEL_STEREOGRAPHIC", points, fxycxy, get_gradients)
+
+
+def project_lonlat(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+    """The equirectangular (longitude, latitude) projection of points (...,3), as mrcal.project_lonlat(); with
+    get_gradients, (q, dq_dp (...,2,3))"""
+    return _project_closed_form("LENSMODEL_LONLAT", points, fxycxy, get_gradients)
+
+
+def unproject_lonlat(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+    """Unit rays of equirectangular (longitude, latitude) pixels (...,2), as mrcal.unproject_lonlat(); with
+    get_gradients, (v, dv_dq (...,3,2))"""
+    return _unproject_closed_form("LENSMODEL_LONLAT", points, fxycxy, get_gradients)
+
+
+def project_latlon(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+    """The transverse equirectangular (latitude, longitude) projection of points (...,3), as mrcal.project_latlon();
+    with get_gradients, (q, dq_dp (...,2,3))"""
+    return _project_closed_form("LENSMODEL_LATLON", points, fxycxy, get_gradients)
+
+
+def unproject_latlon(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+    """Unit rays of transverse equirectangular (latitude, longitude) pixels (...,2), as mrcal.unproject_latlon(); with
+    get_gradients, (v, dv_dq (...,3,2))"""
+    return _unproject_closed_form("LENSMODEL_LATLON", points, fxycxy, get_gradients)

@@ -1,5 +1,6 @@
 // projection_diff(): the comparison of camera models, as mrcal.projection_diff() and
-// mrcal.implied_Rt10__from_unprojections() compute it (mrcal/model_analysis.py:27-395, 1520-1928).
+// mrcal.implied_Rt10__from_unprojections() compute it (mrcal/model_analysis.py:27-395, 1520-1928), and the
+// reprojection between the cameras of a stereo pair that mrcal.stereo_pair_diff() diffs (:1931-2103).
 //
 // The fit of the transformation the two sets of intrinsics imply is one CTA per pair of models, all pairs in one launch.
 // It minimizes the reference's objective, sum over kept points of huber((w th2)^2) with th2 = 2 (1 - cos(angle between
@@ -26,6 +27,7 @@
 #include "device_math.cuh"
 #include "lens_dispatch.cuh"
 #include "reduce.cuh"
+#include "unproject.cuh"
 
 namespace mb200 {
 namespace {
@@ -475,4 +477,55 @@ extern "C" bool mrcal_b200_projection_diff(double* Rt10, double* difflen, double
     if(!D.download(difflen, d_len, (size_t)NdN) || (diff && d_diff && !D.download(diff, d_diff, 2 * (size_t)NdN)))
         return false;
     return D.finish() && fit_status(status);
+}
+
+// Each pair: the normalized unprojection in its camera 0, then reproject_diff_kernel() into its camera 1, diffed against
+// zeros for pair 0 (out = q1_0) and against q1_0 for pair 1 (out = q1_1 - q1_0). One lens kind per launch
+extern "C" bool mrcal_b200_stereo_pair_reproject(double* out, double* outlen, const mrcal_point2_t* q, int N, int Npairs,
+                                                 const mrcal_lensmodel_t* lensmodels, const double* intrinsics,
+                                                 const double* Rt10, double distance)
+{
+    DeviceCall D;
+    if(!D.start()) return false;
+    if(N < 0 || Npairs < 1 || Npairs > 2) { set_error("stereo_pair_reproject: need N >= 0 and 1 or 2 pairs"); return false; }
+    HostLens lens[4];
+    size_t off[5] = {0};
+    for(int k = 0; k < 2 * Npairs; k++)
+    {
+        if(!lens_setup(&lens[k], &lensmodels[k])) return false;
+        off[k + 1] = off[k] + lens[k].Nintr;
+    }
+    for(int p = 0; p < Npairs; p++)
+        if(!central_projection(lens[2 * p], intrinsics + off[2 * p])) return false;
+    if(N == 0) return true;
+    double *d_q, *d_intr, *d_Rt, *d_dist, *d_v, *d_zero, *d_q1, *d_out, *d_len;
+    if(!D.upload(&d_q, (const double*)q, 2 * (size_t)N) || !D.upload(&d_intr, intrinsics, off[2 * Npairs]) ||
+       !D.upload(&d_Rt, Rt10, 12 * (size_t)Npairs) || !D.upload(&d_dist, &distance, 1) || !D.alloc(&d_v, 3 * (size_t)N) ||
+       !D.alloc(&d_zero, 2 * (size_t)N) || !D.alloc(&d_q1, 2 * (size_t)N) || !D.alloc(&d_out, 2 * (size_t)N) ||
+       !D.alloc(&d_len, (size_t)N))
+        return false;
+    MB200_CUDA_CHECK(cudaMemsetAsync(d_zero, 0, 2 * (size_t)N * sizeof(double), D.stream));
+    const unsigned blocks = (unsigned)((N + 127) / 128);
+    for(int p = 0; p < Npairs; p++)
+    {
+        LensArgs a0 = lens[2 * p].a, a1 = lens[2 * p + 1].a;
+        a0.intr = d_intr + off[2 * p];
+        a1.intr = d_intr + off[2 * p + 1];
+        const bool behind_ok = mrcal_lensmodel_metadata(&lensmodels[2 * p]).can_project_behind_camera;
+        const double* ref = p == 0 ? d_zero : d_q1;
+        double* dst = p == Npairs - 1 ? d_out : d_q1;
+        if(!dispatch_lens_kind(lens[2 * p].kind, [&](auto k)
+           {
+               unproject_kernel<decltype(k)::value><<<blocks, 128, 0, D.stream>>>(a0, d_q, N, d_v, nullptr, nullptr, 0,
+                                                                                  behind_ok, true);
+           }) ||
+           !dispatch_lens_kind(lens[2 * p + 1].kind, [&](auto k)
+           {
+               reproject_diff_kernel<decltype(k)::value><<<blocks, 128, 0, D.stream>>>(a1, d_Rt + 12 * p, ref, d_v, d_dist,
+                                                                                       N, 1, dst, d_len, nullptr);
+           }))
+            return false;
+    }
+    MB200_CUDA_CHECK(cudaGetLastError());
+    return D.download(out, d_out, 2 * (size_t)N) && (!outlen || D.download(outlen, d_len, (size_t)N)) && D.finish();
 }

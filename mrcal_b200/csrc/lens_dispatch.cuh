@@ -28,6 +28,49 @@ __device__ __forceinline__ void project_any(double q[2], double dq_dp[2][3], con
         project_parametric<KIND>(q, dq_dp, nullptr, p, a.intr, a.cfg);
 }
 
+// A projection with its gradient in the intrinsics, kept in the compact form the model computes it in. scatter() hands
+// every nonzero entry of dq/dintrinsics to emit(row, column, value), in the dense layout of mrcal.c:2936-2992: the core
+// (dq/df on its own axis only, from q; dq/dc = I), then the distortions -- dense for the parametric models, the RUN x RUN
+// touched control points of the matching surface for the splined ones
+template <int KIND>
+struct IntrinsicsGradient
+{
+    static constexpr int ND = LensTraits<KIND>::NDIST, RUN = LensTraits<KIND>::RUN;
+    double q[2];
+    double ddist[2][ND > 0 ? ND : 1];
+    double wx[4], wy[4], upd[2];
+    int ivar0;
+
+    __device__ __forceinline__ void project(double dq_dp[2][3], const double* p, const LensArgs& a)
+    {
+        if constexpr(LensTraits<KIND>::SPLINED)
+            project_splined<RUN>(q, dq_dp, wx, wy, &ivar0, upd, p, a.intr, a.Nx, a.Ny, a.segments_per_u);
+        else
+            project_parametric<KIND>(q, dq_dp, ddist, p, a.intr, a.cfg);
+    }
+
+    template <class F>
+    __device__ __forceinline__ void scatter(const LensArgs& a, F&& emit) const
+    {
+        if constexpr(LensTraits<KIND>::SPLINED)
+        {
+            emit(0, 0, upd[0]); emit(1, 1, upd[1]);
+            for(int k = 0; k < 2; k++)
+                for(int iy = 0; iy < RUN; iy++)
+                    for(int ix = 0; ix < RUN; ix++)
+                        emit(k, ivar0 + 2 * a.Nx * iy + 2 * ix + k, wx[ix] * wy[iy] * a.intr[k]);
+        }
+        else
+        {
+            emit(0, 0, (q[0] - a.intr[2]) / a.intr[0]);          // mrcal.c:1427-1431
+            emit(1, 1, (q[1] - a.intr[3]) / a.intr[1]);
+            for(int k = 0; k < 2; k++)
+                for(int d = 0; d < ND; d++) emit(k, 4 + d, ddist[k][d]);
+        }
+        emit(0, 2, 1.); emit(1, 3, 1.);
+    }
+};
+
 // A lens model as the point-wise kernels take it. a.intr is left for the caller to point at the uploaded intrinsics
 struct HostLens { int kind; LensArgs a; int Nintr; };
 

@@ -1,5 +1,7 @@
-// The per-point unprojection of every lens kind, shared by mrcal_unproject() (project.cu) and the reprojection maps
-// (image_transforms.cu).
+// The per-point unprojection of every lens kind: unproject_any(), used by the reprojection maps (image_transforms.cu)
+// and model_resolution__deg_pixel() (project.cu); its gradients, unproject_gradient(); the normalizations; and
+// unproject_kernel, which runs mrcal_unproject() and mrcal_b200_unproject_with_gradients() (project.cu) and the
+// unprojections of mrcal_b200_stereo_pair_reproject() (diff.cu).
 //
 // Unprojection of the models without a closed form follows the reference's scheme (mrcal.c:3106-3270): search the 2D
 // stereographic coordinates u of the ray so that project(unproject_stereographic(u)) = q, seeded from the pinhole
@@ -76,6 +78,147 @@ __device__ __forceinline__ void unproject_any(double out[3], double qx, double q
         out[0] = u[0]; out[1] = u[1]; out[2] = 1. - 0.25 * (u[0] * u[0] + u[1] * u[1]);
         if(!(n2 / 2. <= 1e-4)) { out[0] = nan(""); out[1] = nan(""); }
         else if(!behind_ok && out[2] < 0.) { out[0] = -out[0]; out[1] = -out[1]; out[2] = -out[2]; }
+    }
+}
+
+// The ray of pixel (qx, qy) and dv/dq, as the reference's unproject(get_gradients=True) returns them
+// (mrcal/projections.py:250-397), and G: the projection at v with its intrinsics gradient, for dv/dintrinsics =
+// -dv/dq dq/dintrinsics.
+// - The closed-form kinds: their ray and its closed-form derivative (mrcal.c:1475-1880). G holds only the core, from
+//   the given q, as the reference's dv/dintrinsics uses it.
+// - The others, the reference's "q -> vs -> u -> v": the ray vs of unproject_any() is taken to its stereographic
+//   coordinates u and back, v = unproject_stereographic(u), and dv/dq = dv/du (dq/du)^-1 with dq/du = dq/dv dv/du (2x2).
+//   A ray that unproject_any() flipped to the front comes back with another magnitude, as in the reference. A singular
+//   dq/du gives NaN dv/dq
+template <int KIND>
+__device__ __forceinline__ void unproject_gradient(double v[3], double dv_dq[3][2], IntrinsicsGradient<KIND>& G,
+                                                   double qx, double qy, const LensArgs& a, bool behind_ok)
+{
+    unproject_any<KIND>(v, qx, qy, a, behind_ok);
+    const double fxr = 1. / a.intr[0], fyr = 1. / a.intr[1];
+    if constexpr(KIND == LENS_PINHOLE || KIND == LENS_STEREOGRAPHIC || KIND == LENS_LONLAT || KIND == LENS_LATLON)
+    {
+        G.q[0] = qx; G.q[1] = qy;
+        const double x = (qx - a.intr[2]) * fxr, y = (qy - a.intr[3]) * fyr;
+        if constexpr(KIND == LENS_PINHOLE || KIND == LENS_STEREOGRAPHIC)
+        {
+            dv_dq[0][0] = fxr; dv_dq[0][1] = 0.;
+            dv_dq[1][0] = 0.;  dv_dq[1][1] = fyr;
+            dv_dq[2][0] = KIND == LENS_PINHOLE ? 0. : -x / 2. * fxr;
+            dv_dq[2][1] = KIND == LENS_PINHOLE ? 0. : -y / 2. * fyr;
+        }
+        else if constexpr(KIND == LENS_LONLAT)
+        {
+            double slon, clon, slat, clat;
+            sincos(x, &slon, &clon);
+            sincos(y, &slat, &clat);
+            dv_dq[0][0] = fxr * clat * clon;  dv_dq[0][1] = -fyr * slat * slon;
+            dv_dq[1][0] = 0.;                 dv_dq[1][1] = fyr * clat;
+            dv_dq[2][0] = -fxr * clat * slon; dv_dq[2][1] = -fyr * slat * clon;
+        }
+        else
+        {
+            double slat, clat, slon, clon;
+            sincos(x, &slat, &clat);
+            sincos(y, &slon, &clon);
+            dv_dq[0][0] = fxr * clat;         dv_dq[0][1] = 0.;
+            dv_dq[1][0] = -fxr * slat * slon; dv_dq[1][1] = fyr * clat * clon;
+            dv_dq[2][0] = -fxr * slat * clon; dv_dq[2][1] = -fyr * clat * slon;
+        }
+    }
+    else
+    {
+        // u = project_stereographic(vs), v = unproject_stereographic(u) (mrcal.c:1511-1600, f = 1, c = 0)
+        const double mag = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+        const double scale = 2. / (mag + v[2]);
+        const double u[2] = {v[0] * scale, v[1] * scale};
+        v[0] = u[0]; v[1] = u[1]; v[2] = 1. - 0.25 * (u[0] * u[0] + u[1] * u[1]);
+        const double dv_du[3][2] = {{1., 0.}, {0., 1.}, {-u[0] / 2., -u[1] / 2.}};
+        double dq_dv[2][3];
+        G.project(dq_dv, v, a);
+        double J[2][2];
+        for(int r = 0; r < 2; r++)
+            for(int c = 0; c < 2; c++) J[r][c] = dq_dv[r][0] * dv_du[0][c] + dq_dv[r][1] * dv_du[1][c] + dq_dv[r][2] * dv_du[2][c];
+        const double det = J[0][0] * J[1][1] - J[0][1] * J[1][0];
+        const double id = det != 0. ? 1. / det : nan("");
+        const double Ji[2][2] = {{J[1][1] * id, -J[0][1] * id}, {-J[1][0] * id, J[0][0] * id}};
+        for(int r = 0; r < 3; r++)
+            for(int c = 0; c < 2; c++) dv_dq[r][c] = dv_du[r][0] * Ji[0][c] + dv_du[r][1] * Ji[1][c];
+    }
+}
+
+// LONLAT and LATLON rays are unit vectors already: normalize leaves them as they are (mrcal/projections.py:259-276)
+template <int KIND>
+constexpr bool unit_rays = KIND == LENS_LONLAT || KIND == LENS_LATLON;
+
+// v/|v|, or the zero vector for a ray that is not finite, as the reference's unproject(normalize=True) without
+// gradients (mrcal/projections.py:334-344); unit rays unchanged
+template <int KIND>
+__device__ __forceinline__ void normalize_or_zero(double v[3])
+{
+    if constexpr(unit_rays<KIND>) return;
+    if(isfinite(v[0]) && isfinite(v[1]) && isfinite(v[2]))
+    {
+        const double m = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+        v[0] /= m; v[1] /= m; v[2] /= m;
+    }
+    else v[0] = v[1] = v[2] = 0.;
+}
+
+// v -> v/|v| and each column d of dv/dq -> (I - v v'/|v|^2) d / |v|, mrcal/projections.py:220-247. The same projector
+// taken through dv/dintrinsics = -dv/dq dq/dintrinsics normalizes that too
+__device__ __forceinline__ void normalize_with_gradient(double v[3], double dv_dq[3][2])
+{
+    const double r = 1. / sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+    for(int k = 0; k < 3; k++) v[k] *= r;
+    for(int c = 0; c < 2; c++)
+    {
+        const double d[3] = {dv_dq[0][c] * r, dv_dq[1][c] * r, dv_dq[2][c] * r};
+        const double vd = v[0] * d[0] + v[1] * d[1] + v[2] * d[2];
+        for(int k = 0; k < 3; k++) dv_dq[k][c] = d[k] - v[k] * vd;
+    }
+}
+
+// One thread per pixel: v [N][3], and if dv_dq [N][3][2] or dv_di [N][3][Nintr] is given, the gradients of
+// unproject_gradient() (dv_di zeroed by the caller: only its nonzero columns are written). normalize: unit rays, and
+// the gradients of the unit rays. A ray or dv/dq that is not finite gives NaN gradients
+template <int KIND>
+__global__ void unproject_kernel(LensArgs a, const double* __restrict__ q, int N, double* __restrict__ v,
+                                 double* __restrict__ dv_dq, double* __restrict__ dv_di, int Nintr, bool behind_ok,
+                                 bool normalize)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if(i >= N) return;
+    double out[3];
+    if(dv_dq == nullptr && dv_di == nullptr)
+    {
+        unproject_any<KIND>(out, q[2 * i], q[2 * i + 1], a, behind_ok);
+        if(normalize) normalize_or_zero<KIND>(out);
+        v[3 * i] = out[0]; v[3 * i + 1] = out[1]; v[3 * i + 2] = out[2];
+        return;
+    }
+    double D[3][2];
+    IntrinsicsGradient<KIND> G;
+    unproject_gradient<KIND>(out, D, G, q[2 * i], q[2 * i + 1], a, behind_ok);
+    if(normalize && !unit_rays<KIND>) normalize_with_gradient(out, D);
+    bool ok = isfinite(out[0]) && isfinite(out[1]) && isfinite(out[2]);
+    for(int r = 0; r < 3; r++)
+        for(int c = 0; c < 2; c++) ok = ok && isfinite(D[r][c]);
+    if(!ok)
+        for(int r = 0; r < 3; r++) D[r][0] = D[r][1] = nan("");
+    v[3 * i] = out[0]; v[3 * i + 1] = out[1]; v[3 * i + 2] = out[2];
+    if(dv_dq)
+        for(int r = 0; r < 3; r++) { dv_dq[6 * i + 2 * r] = D[r][0]; dv_dq[6 * i + 2 * r + 1] = D[r][1]; }
+    if(dv_di)
+    {
+        double* o = dv_di + (size_t)i * 3 * Nintr;
+        if(!ok)
+            for(int j = 0; j < 3 * Nintr; j++) o[j] = nan("");
+        else
+            G.scatter(a, [&](int k, int col, double val)
+            {
+                for(int r = 0; r < 3; r++) o[r * Nintr + col] -= D[r][k] * val;
+            });
     }
 }
 
