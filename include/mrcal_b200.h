@@ -776,6 +776,57 @@ bool mrcal_b200_match_feature_device(double* out, void* templates, const void* i
                                      const float* Hinv, int M, int template_w, int template_h, int slot_w, int slot_h,
                                      int method, void* stream);
 
+/* The pose utilities of mrcal.poseutils, element-wise over a broadcast shape: one operation `op`
+   (MRCAL_B200_POSE_*) applied to every element of the ndim-dimensional shape `shape`. Each operation takes one or two
+   inputs and gives a value and, with MRCAL_B200_POSE_GET_GRADIENTS, one or two gradients, in the reference's layouts
+   (mrcal/poseutils.py):
+
+     op                    inputs       value  gradients
+     R_FROM_r              r            R      dR/dr (3,3,3)
+     r_FROM_R              R            r      dr/dR (3,3,3)
+     Rt_FROM_rt            rt           Rt     dR/dr (3,3,3)
+     rt_FROM_Rt            Rt           rt     dr/dR (3,3,3)
+     INVERT_R, INVERT_Rt   R, Rt        R, Rt
+     INVERT_rt             rt           rt     drt_out/drt_in (6,6)
+     COMPOSE_Rt            Rt0, Rt1     Rt                                         inverted0, inverted1
+     COMPOSE_r             r0, r1       r      dr/dr0 (3,3), dr/dr1 (3,3)          inverted0, inverted1
+     COMPOSE_rt            rt0, rt1     rt     drt/drt0 (6,6), drt/drt1 (6,6)      inverted0, inverted1
+     COMPOSE_r_TINYr0      r1           dr/dr0 (3,3) at r0 = 0
+     COMPOSE_r_TINYr1      r0           dr/dr1 (3,3) at r1 = 0
+     COMPOSE_rt_TINYrt0    rt1          drt/drt0 (6,6) at rt0 = 0
+     COMPOSE_rt_TINYrt1    rt0          drt/drt1 (6,6) at rt1 = 0
+     ROTATE_POINT_r        r, x         x      dx/dr (3,3), dx/dx_in (3,3)         inverted (as inverted0)
+     ROTATE_POINT_R        R, x         x      dx/dR (3,3,3), dx/dx_in (3,3)       inverted
+     TRANSFORM_POINT_rt    rt, x        x      dx/drt (3,6), dx/dx_in (3,3)        inverted
+     TRANSFORM_POINT_Rt    Rt, x        x      dx/dRt (3,4,3), dx/dx_in (3,3)      inverted
+     SKEW_SYMMETRIC        a            (3,3)
+     R_FROM_QUAT           q (w,x,y,z)  R
+     QUAT_FROM_R           R            q
+     QT_FROM_Rt, Rt_FROM_qt             qt (7,) <-> Rt
+     R_ALIGNED_TO_VECTOR   v            R
+
+   Gradients are taken with respect to the inputs as passed, inverted or not. Input k's element at broadcast index
+   (i_0 .. i_ndim-1) starts at in_k + sum_d i_d strides_k[d] (in doubles; 0 where input k is repeated along d, so no
+   input needs to be expanded) and is packed. Outputs are packed: output k of element e starts at out_k + e * (its
+   size). NULL for an input or output the operation does not have. ndim <= 8. A NaN input gives NaN outputs. False +
+   mrcal_b200_last_error() on refusal or failure */
+enum { MRCAL_B200_POSE_R_FROM_r = 0, MRCAL_B200_POSE_r_FROM_R, MRCAL_B200_POSE_Rt_FROM_rt, MRCAL_B200_POSE_rt_FROM_Rt,
+       MRCAL_B200_POSE_INVERT_R, MRCAL_B200_POSE_INVERT_Rt, MRCAL_B200_POSE_INVERT_rt, MRCAL_B200_POSE_COMPOSE_Rt,
+       MRCAL_B200_POSE_COMPOSE_r, MRCAL_B200_POSE_COMPOSE_rt, MRCAL_B200_POSE_COMPOSE_r_TINYr0,
+       MRCAL_B200_POSE_COMPOSE_r_TINYr1, MRCAL_B200_POSE_COMPOSE_rt_TINYrt0, MRCAL_B200_POSE_COMPOSE_rt_TINYrt1,
+       MRCAL_B200_POSE_ROTATE_POINT_r, MRCAL_B200_POSE_ROTATE_POINT_R, MRCAL_B200_POSE_TRANSFORM_POINT_rt,
+       MRCAL_B200_POSE_TRANSFORM_POINT_Rt, MRCAL_B200_POSE_SKEW_SYMMETRIC, MRCAL_B200_POSE_R_FROM_QUAT,
+       MRCAL_B200_POSE_QUAT_FROM_R, MRCAL_B200_POSE_QT_FROM_Rt, MRCAL_B200_POSE_Rt_FROM_qt,
+       MRCAL_B200_POSE_R_ALIGNED_TO_VECTOR, MRCAL_B200_POSE_NUM_OPS };
+enum { MRCAL_B200_POSE_GET_GRADIENTS = 1, MRCAL_B200_POSE_INVERTED0 = 2, MRCAL_B200_POSE_INVERTED1 = 4 };
+bool mrcal_b200_poseutils(int op, int flags, int ndim, const int64_t* shape, const double* in0, const int64_t* strides0,
+                          const double* in1, const int64_t* strides1, double* out0, double* out1, double* out2);
+/* The same with every buffer on the device: the kernel is enqueued on stream (a cudaStream_t; NULL: the default
+   stream) and the call returns without waiting for it. shape and the strides stay on the host */
+bool mrcal_b200_poseutils_device(int op, int flags, int ndim, const int64_t* shape, const double* in0,
+                                 const int64_t* strides0, const double* in1, const int64_t* strides1, double* out0,
+                                 double* out1, double* out2, void* stream);
+
 // Timing hook for benchmarks: run N cost-function evaluations (residuals +
 // Jacobian) at the current state back to back, return the mean device time per
 // evaluation in milliseconds (CUDA events on the library's stream); <0 on error

@@ -34,6 +34,13 @@ from .image_transforms import (  # noqa: F401
     scale_focal__best_pinhole_fit, pinhole_model_for_reprojection, image_transformation_map, transform_image,
     INTER_NEAREST, INTER_LINEAR, BORDER_CONSTANT, BORDER_TRANSPARENT,
 )
+from .poseutils import (  # noqa: F401
+    R_from_r, r_from_R, Rt_from_rt, rt_from_Rt, invert_R, invert_Rt, invert_rt, compose_Rt, compose_r, compose_rt,
+    compose_r_tinyr0_gradientr0, compose_r_tinyr1_gradientr1, compose_rt_tinyrt0_gradientrt0,
+    compose_rt_tinyrt1_gradientrt1, rotate_point_r, rotate_point_R, transform_point_rt, transform_point_Rt,
+    skew_symmetric, R_from_quat, quat_from_R, qt_from_Rt, Rt_from_qt, R_aligned_to_vector,
+    identity_R, identity_r, identity_Rt, identity_rt,
+)
 from .cameramodel import cameramodel, CameramodelParseException  # noqa: F401
 from .regions import (  # noqa: F401
     measurements_board, measurements_point, residuals_board, residuals_chessboard, residuals_point,

@@ -128,6 +128,7 @@ EXPORTED_SYMBOLS = (
     "mrcal_stereo_range_sparse", "mrcal_stereo_range_dense", "mrcal_b200_stereo_unproject",
     "mrcal_b200_image_transformation_map", "mrcal_b200_transform_image", "mrcal_b200_transform_image_device",
     "mrcal_b200_match_feature", "mrcal_b200_match_feature_device",
+    "mrcal_b200_poseutils", "mrcal_b200_poseutils_device",
     "mrcal_b200_nccl_get_unique_id", "mrcal_b200_nccl_comm_init", "mrcal_b200_nccl_comm_destroy",
     "mrcal_b200_problem_set_sharding",
     "mrcal_b200_factorization_create", "mrcal_b200_factorization_destroy",
@@ -217,6 +218,10 @@ for _n in ["mrcal_b200_match_feature", "mrcal_b200_match_feature_device"]:
 lib.mrcal_b200_match_feature.argtypes = [C.c_void_p] * 3 + [C.c_int] * 3 + [C.c_void_p] + [C.c_int] * 4 + \
                                         [C.c_void_p] * 2 + [C.c_int] * 6
 lib.mrcal_b200_match_feature_device.argtypes = lib.mrcal_b200_match_feature.argtypes + [C.c_void_p]
+for _n in ["mrcal_b200_poseutils", "mrcal_b200_poseutils_device"]:
+    getattr(lib, _n).restype = C.c_bool
+lib.mrcal_b200_poseutils.argtypes = [C.c_int] * 3 + [C.c_void_p] * 8
+lib.mrcal_b200_poseutils_device.argtypes = lib.mrcal_b200_poseutils.argtypes + [C.c_void_p]
 lib.mrcal_b200_factorization_create_from_last_callback.restype = C.c_void_p
 lib.mrcal_b200_csr_create.restype = C.c_void_p
 lib.mrcal_b200_csr_destroy.restype = None

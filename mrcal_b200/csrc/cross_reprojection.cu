@@ -23,6 +23,7 @@
 //   4. 6x6 Cholesky of JJ, K = -inv(JJ) C, per column.
 // Accepts what the reference accepts and refuses what it refuses (uncertainty.c:944-989).
 #include "device_math.cuh"
+#include "pose.cuh"
 #include "problem_impl.h"
 #include "reduce.cuh"
 
@@ -55,23 +56,6 @@ __device__ void apply_Mt_pose(double* out, const double* X, int n, const double 
         out[4 * n + j] = xt[1];
         out[5 * n + j] = xt[2];
     }
-}
-
-// dr01/dr0 at r0 = 0 (poseutils.c:1003-1062): -r r' (B/tanB - 1)/(4 B^2) + (B/tanB) I - skew(r)/2, B = |r|/2
-__device__ void compose_r_tinyr0_gradient(double Dr[9], const double r[3])
-{
-    const double n2 = r[0] * r[0] + r[1] * r[1] + r[2] * r[2];
-    if(n2 < 2e-8 * 2e-8)
-    {
-        for(int i = 0; i < 9; i++) Dr[i] = (i % 4 == 0) ? 1. : 0.;
-        return;
-    }
-    const double B = sqrt(n2) / 2., BtB = B / tan(B);
-    for(int i = 0; i < 3; i++)
-        for(int j = 0; j < 3; j++) Dr[3 * i + j] = -r[i] * r[j] * (BtB - 1.) / (4. * B * B) + (i == j ? BtB : 0.);
-    Dr[1] += r[2] / 2.; Dr[2] -= r[1] / 2.;
-    Dr[3] -= r[2] / 2.; Dr[5] += r[0] / 2.;
-    Dr[6] += r[1] / 2.; Dr[7] -= r[0] / 2.;
 }
 
 // One warp per observation. icam < 0: rrp. Otherwise ccp for camera icam: the other cameras' observations contribute nothing

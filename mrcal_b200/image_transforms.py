@@ -183,17 +183,16 @@ def _image_layout(shape, what):
                        f"{tuple(shape)}")
 
 
-def _torch_if_tensors(*xs):
-    """torch, if the given arrays are torch tensors; None if they are not. Mixing the two is refused. torch is only
-    imported by a caller who already has tensors"""
+def _torch_if_tensors(*xs, what="transform_image(): image, mapxy and out"):
+    """torch, if the given arrays are torch tensors; None if they are not. Mixing the two is refused: `what` names the
+    caller and its arrays in the message. torch is only imported by a caller who already has tensors"""
     torch = sys.modules.get("torch")
     given = [x for x in xs if x is not None]
     is_tensor = [torch is not None and isinstance(x, torch.Tensor) for x in given]
     if not any(is_tensor):
         return None
     if not all(is_tensor):
-        raise RuntimeError("transform_image(): image, mapxy and out must all be numpy arrays or all be torch CUDA "
-                           "tensors; they may not be mixed")
+        raise RuntimeError(f"{what} must all be numpy arrays or all be torch CUDA tensors; they may not be mixed")
     return torch
 
 
