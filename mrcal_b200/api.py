@@ -23,6 +23,7 @@ import scipy.sparse
 
 from . import _capi
 from ._capi import lib
+from ._poses_host import compose_Rt, invert_Rt
 
 _KNOWN_KWARGS = {
     "intrinsics", "lensmodel", "imagersizes",
@@ -439,10 +440,6 @@ def implied_Rt10__from_unprojections(q0, p0, v1, *, weights=None, atinfinity=Tru
     return Rt
 
 
-def _compose_Rt(A, B):
-    return np.vstack((A[:3] @ B[:3], A[:3] @ B[3] + A[3]))
-
-
 def _identity_Rt():
     return np.vstack((np.eye(3), np.zeros(3)))
 
@@ -511,7 +508,7 @@ def projection_diff(models, *, implied_Rt10=None, gridn_width=60, gridn_height=N
     elif intrinsics_only:
         Rt10 = np.array([_identity_Rt()] * (Nmodels - 1))
     elif focus_radius == 0:
-        Rt10 = np.array([_compose_Rt(models[k].Rt_cam_ref(), models[0].Rt_ref_cam()) for k in range(1, Nmodels)])
+        Rt10 = np.array([compose_Rt(models[k].Rt_cam_ref(), models[0].Rt_ref_cam()) for k in range(1, Nmodels)])
     else:
         Rt10 = np.zeros((Nmodels - 1, 4, 3))
         fit = True
@@ -568,10 +565,6 @@ def model_resolution__deg_pixel(q, model, *, mode="mean"):
     return out.reshape(q.shape[:-1])
 
 
-def _invert_Rt(Rt):
-    return np.vstack((Rt[:3].T, -Rt[:3].T @ Rt[3]))
-
-
 def _stereo_pair_reproject(q, models, Rts, distance):
     """out, |out|: the pixels q (...,2) of camera 0 of each (camera 0, camera 1) pair in models, reprojected into its
     camera 1 through Rt (4,3) from camera 0 to camera 1: q1 for one pair, q1[1] - q1[0] for two"""
@@ -601,7 +594,7 @@ def stereo_pair_diff(model_pairs, *, gridn_width=60, gridn_height=None, distance
     unprojections and reprojections run on the device (csrc/diff.cu)"""
     if len(model_pairs) != 2:
         raise RuntimeError("Exactly 2 model_pairs are expected")
-    Rt10_pairs = np.array([_compose_Rt(m1.Rt_cam_ref(), m0.Rt_ref_cam()) for m0, m1 in model_pairs])
+    Rt10_pairs = np.array([compose_Rt(m1.Rt_cam_ref(), m0.Rt_ref_cam()) for m0, m1 in model_pairs])
     atinfinity = distance is None
     if atinfinity:
         distance = 1.
@@ -627,7 +620,7 @@ def stereo_pair_diff(model_pairs, *, gridn_width=60, gridn_height=None, distance
     if np.any(imagersizes1[1] - imagersizes1[0]):
         raise RuntimeError("The second camera in each given pair must have identical imager dimensions. I technically "
                            "don't NEED this, but it's extremely likely to be an unintentional mistake by the caller")
-    Rt10_Rt01_pairs = (Rt10_pairs, np.array([_invert_Rt(Rt) for Rt in Rt10_pairs]))
+    Rt10_Rt01_pairs = (Rt10_pairs, invert_Rt(Rt10_pairs))
     d = float(distance)
 
     def reproject_pairp_from_cami(q, p, i):

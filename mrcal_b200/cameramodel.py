@@ -21,25 +21,14 @@ import io
 
 import numpy as np
 
+from ._poses_host import R_from_r as _R_from_r  # noqa: F401  (the private name callers import from this module)
+from ._poses_host import Rt_from_rt, invert_rt
+
 _LEGACY_INPUT_NAMES = (("frames_rt_toref", "rt_ref_frame"), ("extrinsics_rt_fromref", "rt_cam_ref"))
 
 
 class CameramodelParseException(Exception):
     """A `.cameramodel` could not be parsed (the reference's name for it: mrcal/cameramodel.py:150)."""
-
-
-def _R_from_r(r):
-    th = float(np.linalg.norm(r))
-    K = np.array(((0., -r[2], r[1]), (r[2], 0., -r[0]), (-r[1], r[0], 0.)))
-    if th < 1e-10:
-        return np.eye(3) + K
-    return np.eye(3) + np.sin(th) / th * K + (1. - np.cos(th)) / (th * th) * (K @ K)
-
-
-def invert_rt(rt):
-    """(r,t) of the inverse transform: x = R y + t  <=>  y = R' x - R' t."""
-    rt = np.asarray(rt, float)
-    return np.concatenate((-rt[:3], -(_R_from_r(rt[:3]).T @ rt[3:])))
 
 
 def serialize_optimization_inputs(optimization_inputs):
@@ -212,11 +201,10 @@ class cameramodel:
 
     def Rt_cam_ref(self):
         """The pose as a (4,3) Rt transformation: R on top, t in the last row"""
-        return np.vstack((_R_from_r(self._rt_cam_ref[:3]), self._rt_cam_ref[3:]))
+        return Rt_from_rt(self._rt_cam_ref)
 
     def Rt_ref_cam(self):
-        rt = self.rt_ref_cam()
-        return np.vstack((_R_from_r(rt[:3]), rt[3:]))
+        return Rt_from_rt(self.rt_ref_cam())
 
     extrinsics_rt_fromref = rt_cam_ref
     extrinsics_rt_toref = rt_ref_cam

@@ -17,7 +17,7 @@ namespace mb200 {
 // Same quantity as mrcal_R_from_r_full (poseutils-opencv.c:42-155); the
 // near-zero branch there (:64-84) is replaced by series that are accurate to
 // roundoff for all |r| < 0.1
-__device__ __forceinline__ void rodrigues(double* __restrict__ R, double* __restrict__ dR, const double* __restrict__ r)
+__host__ __device__ __forceinline__ void rodrigues(double* __restrict__ R, double* __restrict__ dR, const double* __restrict__ r)
 {
     const double rx = r[0], ry = r[1], rz = r[2];
     const double t2 = rx * rx + ry * ry + rz * rz;

@@ -2,104 +2,15 @@
 // inversion, rotation and transformation of points, and the quaternion conversions. Every function works on one pose in
 // registers, fp64, and follows the branches of the reference (poseutils.c, poseutils-opencv.c,
 // poseutils-uses-autodiff.cc, mrcal/_poseutils_scipy.py; cited per function). Layouts are the reference's: R is
-// row-major (3,3); Rt is (4,3), R then t; rt is (6,), r then t; a quaternion is (w,x,y,z).
+// row-major (3,3); Rt is (4,3), R then t; rt is (6,), r then t; a quaternion is (w,x,y,z). The ones marked __host__
+// serve the host code too (stereo.cu).
 #pragma once
 #include <cuda_runtime.h>
 
 #include "device_math.cuh"
+#include "dual.cuh"
 
 namespace mb200 {
-
-// A value and its gradient with respect to N inputs: the forward-mode arithmetic of the reference's val_withgrad_t
-// (_autodiff.hh), so that a function restated with it takes the reference's branches and gives its gradients
-template <int N> struct Dual
-{
-    double x;
-    double j[N > 0 ? N : 1];
-    __device__ Dual(double v = 0.) : x(v)
-    {
-#pragma unroll
-        for(int i = 0; i < N; i++) j[i] = 0.;
-    }
-    // input number k of the N
-    __device__ static Dual var(double v, int k)
-    {
-        Dual d(v);
-#pragma unroll
-        for(int i = 0; i < N; i++) d.j[i] = i == k ? 1. : 0.;
-        return d;
-    }
-};
-
-template <int N> __device__ __forceinline__ Dual<N> operator+(const Dual<N>& a, const Dual<N>& b)
-{
-    Dual<N> y(a.x + b.x);
-#pragma unroll
-    for(int i = 0; i < N; i++) y.j[i] = a.j[i] + b.j[i];
-    return y;
-}
-template <int N> __device__ __forceinline__ Dual<N> operator-(const Dual<N>& a, const Dual<N>& b)
-{
-    Dual<N> y(a.x - b.x);
-#pragma unroll
-    for(int i = 0; i < N; i++) y.j[i] = a.j[i] - b.j[i];
-    return y;
-}
-template <int N> __device__ __forceinline__ Dual<N> operator*(const Dual<N>& a, const Dual<N>& b)
-{
-    Dual<N> y(a.x * b.x);
-#pragma unroll
-    for(int i = 0; i < N; i++) y.j[i] = a.j[i] * b.x + a.x * b.j[i];
-    return y;
-}
-template <int N> __device__ __forceinline__ Dual<N> operator*(const Dual<N>& a, double b)
-{
-    Dual<N> y(a.x * b);
-#pragma unroll
-    for(int i = 0; i < N; i++) y.j[i] = a.j[i] * b;
-    return y;
-}
-template <int N> __device__ __forceinline__ Dual<N> operator/(const Dual<N>& a, const Dual<N>& b)
-{
-    Dual<N> y(a.x / b.x);
-#pragma unroll
-    for(int i = 0; i < N; i++) y.j[i] = (a.j[i] * b.x - a.x * b.j[i]) / (b.x * b.x);
-    return y;
-}
-template <int N> __device__ __forceinline__ Dual<N> operator/(const Dual<N>& a, double b) { return a * (1. / b); }
-template <int N> __device__ __forceinline__ Dual<N> dsqrt(const Dual<N>& a)
-{
-    Dual<N> y(sqrt(a.x));
-#pragma unroll
-    for(int i = 0; i < N; i++) y.j[i] = a.j[i] / (2. * y.x);
-    return y;
-}
-template <int N> __device__ __forceinline__ void dsincos(const Dual<N>& a, Dual<N>& s, Dual<N>& c)
-{
-    double sv, cv;
-    sincos(a.x, &sv, &cv);
-    s = Dual<N>(sv);
-    c = Dual<N>(cv);
-#pragma unroll
-    for(int i = 0; i < N; i++) { s.j[i] = cv * a.j[i]; c.j[i] = -sv * a.j[i]; }
-}
-template <int N> __device__ __forceinline__ Dual<N> dtan(const Dual<N>& a)
-{
-    double sv, cv;
-    sincos(a.x, &sv, &cv);
-    Dual<N> y(sv / cv);
-#pragma unroll
-    for(int i = 0; i < N; i++) y.j[i] = a.j[i] / (cv * cv);
-    return y;
-}
-template <int N> __device__ __forceinline__ Dual<N> dacos(const Dual<N>& a)
-{
-    Dual<N> y(acos(a.x));
-    const double d = -1. / sqrt(1. - a.x * a.x);
-#pragma unroll
-    for(int i = 0; i < N; i++) y.j[i] = d * a.j[i];
-    return y;
-}
 
 // x rotated by r (by -r if inverted), the Rodrigues formula of rotate_point_r_core() (poseutils-uses-autodiff.cc:17-81),
 // with its small-angle limit for |r|^2 < 1e-10
@@ -279,7 +190,7 @@ __device__ __forceinline__ void compose_r_tinyr1_gradient(double Dr[9], const do
 // R from r (mrcal_R_from_r_full, poseutils-opencv.c:42-155), with J[i][j][k] = dR_ij/dr_k. Below |r| = DBL_EPSILON
 // the reference's exact branch: I and the constant gradient. Otherwise rodrigues(), whose series below |r| = 0.1 is
 // accurate where the reference's closed form loses digits to cancellation
-__device__ __forceinline__ void R_from_r(double R[9], double* J, const double r[3])
+__host__ __device__ __forceinline__ void R_from_r(double R[9], double* J, const double r[3])
 {
     const double n2 = r[0] * r[0] + r[1] * r[1] + r[2] * r[2];
     if(n2 < 2.220446049250313e-16 * 2.220446049250313e-16)
@@ -309,7 +220,7 @@ __device__ __forceinline__ void R_from_r(double R[9], double* J, const double r[
 // r from R (mrcal_r_from_R_full, poseutils.c:1140-1437): the axis from R - R', the angle from the trace, with the
 // reference's small-angle branch and its branch near a half-turn. J[k][i][j] = dr_k/dR_ij: the pseudo-inverse of
 // dR/dr at the result, the gradient within the manifold of rotations
-__device__ __forceinline__ void r_from_R(double r[3], double* J, const double R[9])
+__host__ __device__ __forceinline__ void r_from_R(double r[3], double* J, const double R[9])
 {
     const double tr = R[0] + R[4] + R[8];
     const double u[3] = {R[7] - R[5], R[2] - R[6], R[3] - R[1]};
@@ -374,6 +285,50 @@ __device__ __forceinline__ void r_from_R(double r[3], double* J, const double R[
         for(int k = 0; k < 3; k++)
             J[9 * k + ij] = (Mi[3 * k] * D[3 * ij] + Mi[3 * k + 1] * D[3 * ij + 1] + Mi[3 * k + 2] * D[3 * ij + 2]) *
                             inv_det;
+}
+
+// element (i,j) of R or, if transposed, of R'
+__host__ __device__ __forceinline__ double Rij(const double* R, bool transposed, int i, int j)
+{
+    return transposed ? R[3 * j + i] : R[3 * i + j];
+}
+
+__host__ __device__ __forceinline__ void invert_R(double out[9], const double R[9])
+{
+    for(int i = 0; i < 9; i++) out[i] = R[3 * (i % 3) + i / 3];
+}
+
+// (R', -R' t); out must not alias Rt
+__host__ __device__ __forceinline__ void invert_Rt(double out[12], const double Rt[12])
+{
+    invert_R(out, Rt);
+    for(int i = 0; i < 3; i++) out[9 + i] = -(out[3 * i] * Rt[9] + out[3 * i + 1] * Rt[10] + out[3 * i + 2] * Rt[11]);
+}
+
+// x -> Rt0(Rt1(x)), Rt0 and Rt1 taken inverted where asked: the four cases of mrcal_compose_Rt_full
+// (poseutils.c:603-738). out must not alias Rt0 or Rt1
+__host__ __device__ __forceinline__ void compose_Rt(double out[12], const double Rt0[12], const double Rt1[12],
+                                                    bool inverted0, bool inverted1)
+{
+    for(int i = 0; i < 3; i++)
+        for(int j = 0; j < 3; j++)
+            out[3 * i + j] = Rij(Rt0, inverted0, i, 0) * Rij(Rt1, inverted1, 0, j) +
+                             Rij(Rt0, inverted0, i, 1) * Rij(Rt1, inverted1, 1, j) +
+                             Rij(Rt0, inverted0, i, 2) * Rij(Rt1, inverted1, 2, j);
+    const double* t0 = &Rt0[9];
+    const double* t1 = &Rt1[9];
+    for(int i = 0; i < 3; i++)
+    {
+        if(!inverted0 && !inverted1)
+            out[9 + i] = Rt0[3 * i] * t1[0] + Rt0[3 * i + 1] * t1[1] + Rt0[3 * i + 2] * t1[2] + t0[i];
+        else if(inverted0 && !inverted1)
+            out[9 + i] = Rt0[i] * (t1[0] - t0[0]) + Rt0[3 + i] * (t1[1] - t0[1]) + Rt0[6 + i] * (t1[2] - t0[2]);
+        else
+        {
+            const double Rt = out[3 * i] * t1[0] + out[3 * i + 1] * t1[1] + out[3 * i + 2] * t1[2];
+            out[9 + i] = inverted0 ? -Rt - (Rt0[i] * t0[0] + Rt0[3 + i] * t0[1] + Rt0[6 + i] * t0[2]) : -Rt + t0[i];
+        }
+    }
 }
 
 __device__ __forceinline__ void skew_symmetric(double S[9], const double a[3])

@@ -62,12 +62,6 @@ struct PoseArgs
     double* out[3];                     // packed: element e's output k at out[k] + e * out_k
 };
 
-// element (i,j) of R or, if transposed, of R'
-__device__ __forceinline__ double Rij(const double* R, bool transposed, int i, int j)
-{
-    return transposed ? R[3 * j + i] : R[3 * i + j];
-}
-
 // compose_rt (mrcal_compose_rt_full, poseutils.c:745-1001, and _compose_rt_withgrad, poseutils-genpywrap.py): r by
 // compose_r(), t by the reference's four cases. d0, d1: the (6,6) drt/drt0, drt/drt1, or nullptr
 __device__ __forceinline__ void compose_rt(double out[6], double* d0, double* d1, const double rt0[6],
@@ -142,12 +136,10 @@ __device__ __forceinline__ void pose_op(double* y0, double* y1, double* y2, cons
         r_from_R(y0, G ? y1 : nullptr, x0);
         for(int i = 0; i < 3; i++) y0[3 + i] = x0[9 + i];
     }
-    else if constexpr(OP == MRCAL_B200_POSE_INVERT_R || OP == MRCAL_B200_POSE_INVERT_Rt)
-    {
-        for(int i = 0; i < 9; i++) y0[i] = x0[3 * (i % 3) + i / 3];
-        if constexpr(OP == MRCAL_B200_POSE_INVERT_Rt)
-            for(int i = 0; i < 3; i++) y0[9 + i] = -(y0[3 * i] * x0[9] + y0[3 * i + 1] * x0[10] + y0[3 * i + 2] * x0[11]);
-    }
+    else if constexpr(OP == MRCAL_B200_POSE_INVERT_R)
+        invert_R(y0, x0);
+    else if constexpr(OP == MRCAL_B200_POSE_INVERT_Rt)
+        invert_Rt(y0, x0);
     else if constexpr(OP == MRCAL_B200_POSE_INVERT_rt)
     {
         // r' = -r, t' = -rot(-r, t) (mrcal_invert_rt_full, poseutils.c:557-597)
@@ -166,27 +158,7 @@ __device__ __forceinline__ void pose_op(double* y0, double* y1, double* y2, cons
                 }
     }
     else if constexpr(OP == MRCAL_B200_POSE_COMPOSE_Rt)
-    {
-        // the four cases of mrcal_compose_Rt_full (poseutils.c:603-738)
-        for(int i = 0; i < 3; i++)
-            for(int j = 0; j < 3; j++)
-                y0[3 * i + j] = Rij(x0, inv0, i, 0) * Rij(x1, inv1, 0, j) + Rij(x0, inv0, i, 1) * Rij(x1, inv1, 1, j) +
-                                Rij(x0, inv0, i, 2) * Rij(x1, inv1, 2, j);
-        const double* t0 = &x0[9];
-        const double* t1 = &x1[9];
-        for(int i = 0; i < 3; i++)
-        {
-            if(!inv0 && !inv1)
-                y0[9 + i] = x0[3 * i] * t1[0] + x0[3 * i + 1] * t1[1] + x0[3 * i + 2] * t1[2] + t0[i];
-            else if(inv0 && !inv1)
-                y0[9 + i] = x0[i] * (t1[0] - t0[0]) + x0[3 + i] * (t1[1] - t0[1]) + x0[6 + i] * (t1[2] - t0[2]);
-            else
-            {
-                const double Rt1 = y0[3 * i] * t1[0] + y0[3 * i + 1] * t1[1] + y0[3 * i + 2] * t1[2];
-                y0[9 + i] = inv0 ? -Rt1 - (x0[i] * t0[0] + x0[3 + i] * t0[1] + x0[6 + i] * t0[2]) : -Rt1 + t0[i];
-            }
-        }
-    }
+        compose_Rt(y0, x0, x1, inv0, inv1);
     else if constexpr(OP == MRCAL_B200_POSE_COMPOSE_r)
         compose_r(y0, G ? y1 : nullptr, y2, x0, x1, inv0, inv1);
     else if constexpr(OP == MRCAL_B200_POSE_COMPOSE_rt)

@@ -12,6 +12,7 @@
 #include "device_call.h"
 #include "device_math.cuh"
 #include "lens_dispatch.cuh"
+#include "pose.cuh"
 
 namespace mb200 {
 namespace {
@@ -135,99 +136,6 @@ __global__ void stereo_range_kernel(RangeInput in, Fxycxy f, double baseline, lo
         rectified_ray<RECT>(v, qx, qy, f);
         const double s = r / sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
         p[3 * k] = v[0] * s; p[3 * k + 1] = v[1] * s; p[3 * k + 2] = v[2] * s;
-    }
-}
-
-////////////////////////////////////////////////////////////////////////////////
-// host: rotations (the reference's poseutils conventions: Rt is R (3x3, row-major) then t; r is Rodrigues)
-////////////////////////////////////////////////////////////////////////////////
-void R_from_r(double R[9], const double r[3])
-{
-    const double th2 = r[0] * r[0] + r[1] * r[1] + r[2] * r[2];
-    const double K[9] = {0., -r[2], r[1], r[2], 0., -r[0], -r[1], r[0], 0.};
-    double s, c;   // R = I + s K + c K^2
-    if(th2 < 1e-20) { s = 1.; c = 0.5; }
-    else
-    {
-        const double th = sqrt(th2);
-        s = sin(th) / th;
-        c = (1. - cos(th)) / th2;
-    }
-    for(int i = 0; i < 3; i++)
-        for(int j = 0; j < 3; j++)
-        {
-            double KK = 0.;
-            for(int k = 0; k < 3; k++) KK += K[3 * i + k] * K[3 * k + j];
-            R[3 * i + j] = (i == j ? 1. : 0.) + s * K[3 * i + j] + c * KK;
-        }
-}
-
-// th in [0, pi]: from the antisymmetric part u = 2 sin(th) axis and from trace(R) = 1 + 2 cos(th), whichever is
-// better conditioned (poseutils.c:1159-1228); near th = pi the axis comes from the symmetric part
-void r_from_R(double r[3], const double R[9])
-{
-    const double u[3] = {R[7] - R[5], R[2] - R[6], R[3] - R[1]};
-    const double costh = (R[0] + R[4] + R[8] - 1.) / 2.;
-    const double norm2u = u[0] * u[0] + u[1] * u[1] + u[2] * u[2];
-    const double eps = 1e-8;
-    if(norm2u > 4. * eps * eps && 1. - fabs(costh) > eps * eps / 2.)
-    {
-        const double sinth = sqrt(norm2u) / 2.;
-        const double th = sinth > sqrt(2.) / 2. ? acos(costh) : (costh > 0 ? asin(sinth) : M_PI - asin(sinth));
-        for(int i = 0; i < 3; i++) r[i] = u[i] / sqrt(norm2u) * th;
-    }
-    else if(costh > 0)
-        for(int i = 0; i < 3; i++) r[i] = u[i] / 2.;
-    else
-    {
-        // R ~ 2 v v' - I: the axis is the largest column of R + I, its sign from u
-        int imax = 0;
-        for(int i = 1; i < 3; i++) if(R[4 * i] > R[4 * imax]) imax = i;
-        double v[3], n = 0.;
-        for(int i = 0; i < 3; i++) { v[i] = R[3 * i + imax] + (i == imax ? 1. : 0.); n += v[i] * v[i]; }
-        n = sqrt(n);
-        double dot = 0.;
-        for(int i = 0; i < 3; i++) { v[i] /= n; dot += v[i] * u[i]; }
-        if(dot < 0) for(int i = 0; i < 3; i++) v[i] = -v[i];
-        const double th = M_PI - asin(fmin(1., sqrt(norm2u) / 2.));
-        for(int i = 0; i < 3; i++) r[i] = v[i] * th;
-    }
-}
-
-void Rt_from_rt(double Rt[12], const double rt[6])
-{
-    R_from_r(Rt, rt);
-    for(int i = 0; i < 3; i++) Rt[9 + i] = rt[3 + i];
-}
-
-// out = A B: x -> A(B(x))
-void compose_Rt(double out[12], const double A[12], const double B[12])
-{
-    double o[12];
-    for(int i = 0; i < 3; i++)
-    {
-        for(int j = 0; j < 3; j++)
-        {
-            double s = 0.;
-            for(int k = 0; k < 3; k++) s += A[3 * i + k] * B[3 * k + j];
-            o[3 * i + j] = s;
-        }
-        double t = A[9 + i];
-        for(int k = 0; k < 3; k++) t += A[3 * i + k] * B[9 + k];
-        o[9 + i] = t;
-    }
-    memcpy(out, o, sizeof(o));
-}
-
-void invert_Rt(double out[12], const double Rt[12])
-{
-    for(int i = 0; i < 3; i++)
-        for(int j = 0; j < 3; j++) out[3 * i + j] = Rt[3 * j + i];
-    for(int i = 0; i < 3; i++)
-    {
-        double t = 0.;
-        for(int k = 0; k < 3; k++) t -= Rt[3 * k + i] * Rt[9 + k];
-        out[9 + i] = t;
     }
 }
 
@@ -603,10 +511,11 @@ extern "C" bool mrcal_rectified_system2(unsigned int* imagersize_rectified, doub
     // The rectified frame, in camera-0 coordinates (stereo.c:488-550): x ("right") along the baseline towards camera
     // 1, z ("forward") the mean of the two optical axes without its component along x, y ("down") completing it
     double Rt_cam0_ref[12], Rt_cam1_ref[12], Rt_ref_cam1[12], Rt01[12];
-    Rt_from_rt(Rt_cam0_ref, rt_cam0_ref);
-    Rt_from_rt(Rt_cam1_ref, rt_cam1_ref);
+    R_from_r(Rt_cam0_ref, nullptr, rt_cam0_ref);
+    R_from_r(Rt_cam1_ref, nullptr, rt_cam1_ref);
+    for(int i = 0; i < 3; i++) { Rt_cam0_ref[9 + i] = rt_cam0_ref[3 + i]; Rt_cam1_ref[9 + i] = rt_cam1_ref[3 + i]; }
     invert_Rt(Rt_ref_cam1, Rt_cam1_ref);
-    compose_Rt(Rt01, Rt_cam0_ref, Rt_ref_cam1);
+    compose_Rt(Rt01, Rt_cam0_ref, Rt_ref_cam1, false, false);
 
     double Rt_rect0_cam0[12] = {};
     double* right = &Rt_rect0_cam0[0];
@@ -718,8 +627,8 @@ extern "C" bool mrcal_rectified_system2(unsigned int* imagersize_rectified, doub
     }
 
     double Rt_rect0_ref[12];
-    compose_Rt(Rt_rect0_ref, Rt_rect0_cam0, Rt_cam0_ref);
-    r_from_R(rt_rect0_ref, Rt_rect0_ref);
+    compose_Rt(Rt_rect0_ref, Rt_rect0_cam0, Rt_cam0_ref, false, false);
+    r_from_R(rt_rect0_ref, nullptr, Rt_rect0_ref);
     for(int i = 0; i < 3; i++) rt_rect0_ref[3 + i] = Rt_rect0_ref[9 + i];
     return true;
 }
@@ -763,12 +672,12 @@ extern "C" bool mrcal_rectification_maps(float* rectification_maps,
     if(Npix <= 0) return true;
     // R_cam_rect = R_cam_ref R_rect0_ref' (stereo.c:850-862)
     double R_rect0_ref[9];
-    R_from_r(R_rect0_ref, r_rect0_ref);
+    R_from_r(R_rect0_ref, nullptr, r_rect0_ref);
     Mat3 R[2];
     for(int c = 0; c < 2; c++)
     {
         double R_cam_ref[9];
-        R_from_r(R_cam_ref, r_cam_ref[c]);
+        R_from_r(R_cam_ref, nullptr, r_cam_ref[c]);
         for(int i = 0; i < 3; i++)
             for(int j = 0; j < 3; j++)
             {

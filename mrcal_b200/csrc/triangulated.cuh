@@ -5,120 +5,48 @@
 // for pairs that fail the cheirality test.
 //
 // The reference gets the gradients by forward-mode automatic differentiation over
-// 6 inputs; so does this file, with a dual-number type of its own: the function has
+// 6 inputs; so does this file, with the same dual-number type (dual.cuh): the function has
 // branches whose derivatives are defined by "whatever the operations taken produce",
 // and carrying the derivatives through the same operations is the one way to agree
 // with that to rounding everywhere, branch boundaries included.
 #pragma once
 #include <cuda_runtime.h>
 
+#include "dual.cuh"
+
 namespace mb200 {
 
-// value and gradient with respect to (a[0..2], t[0..2])
-struct Dual6
+__device__ __forceinline__ Dual<6> d6_dot(const Dual<6> a[3], const Dual<6> b[3])
 {
-    double x;
-    double g[6];
-};
-
-__device__ __forceinline__ Dual6 d6_const(double v)
-{
-    Dual6 r; r.x = v;
-#pragma unroll
-    for(int i = 0; i < 6; i++) r.g[i] = 0.;
-    return r;
+    return a[0] * b[0] + a[1] * b[1] + a[2] * b[2];
 }
-__device__ __forceinline__ Dual6 d6_var(double v, int i0)
+__device__ __forceinline__ Dual<6> d6_cross_norm2(const Dual<6> a[3], const Dual<6> b[3])
 {
-    Dual6 r = d6_const(v);
-    r.g[i0] = 1.;
-    return r;
-}
-__device__ __forceinline__ Dual6 operator+(const Dual6& a, const Dual6& b)
-{
-    Dual6 r; r.x = a.x + b.x;
-#pragma unroll
-    for(int i = 0; i < 6; i++) r.g[i] = a.g[i] + b.g[i];
-    return r;
-}
-__device__ __forceinline__ Dual6 operator-(const Dual6& a, const Dual6& b)
-{
-    Dual6 r; r.x = a.x - b.x;
-#pragma unroll
-    for(int i = 0; i < 6; i++) r.g[i] = a.g[i] - b.g[i];
-    return r;
-}
-__device__ __forceinline__ Dual6 operator-(const Dual6& a)
-{
-    Dual6 r; r.x = -a.x;
-#pragma unroll
-    for(int i = 0; i < 6; i++) r.g[i] = -a.g[i];
-    return r;
-}
-__device__ __forceinline__ Dual6 operator*(const Dual6& a, const Dual6& b)
-{
-    Dual6 r; r.x = a.x * b.x;
-#pragma unroll
-    for(int i = 0; i < 6; i++) r.g[i] = a.g[i] * b.x + a.x * b.g[i];
-    return r;
-}
-__device__ __forceinline__ Dual6 operator*(const Dual6& a, double s)
-{
-    Dual6 r; r.x = a.x * s;
-#pragma unroll
-    for(int i = 0; i < 6; i++) r.g[i] = a.g[i] * s;
-    return r;
-}
-__device__ __forceinline__ Dual6 operator+(const Dual6& a, double s) { Dual6 r = a; r.x += s; return r; }
-__device__ __forceinline__ Dual6 operator-(const Dual6& a, double s) { Dual6 r = a; r.x -= s; return r; }
-__device__ __forceinline__ Dual6 operator/(const Dual6& a, const Dual6& b)
-{
-    Dual6 r;
-    const double bi = 1. / b.x;
-    r.x = a.x * bi;
-#pragma unroll
-    for(int i = 0; i < 6; i++) r.g[i] = (a.g[i] - r.x * b.g[i]) * bi;
-    return r;
-}
-__device__ __forceinline__ Dual6 d6_sqrt(const Dual6& a)
-{
-    Dual6 r; r.x = sqrt(a.x);
-    const double h = 0.5 / r.x;
-#pragma unroll
-    for(int i = 0; i < 6; i++) r.g[i] = a.g[i] * h;
-    return r;
-}
-
-struct Vec6 { Dual6 v[3]; };
-
-__device__ __forceinline__ Dual6 d6_dot(const Vec6& a, const Vec6& b) { return a.v[0] * b.v[0] + a.v[1] * b.v[1] + a.v[2] * b.v[2]; }
-__device__ __forceinline__ Dual6 d6_cross_norm2(const Vec6& a, const Vec6& b)
-{
-    const Dual6 c0 = a.v[1] * b.v[2] - a.v[2] * b.v[1];
-    const Dual6 c1 = a.v[2] * b.v[0] - a.v[0] * b.v[2];
-    const Dual6 c2 = a.v[0] * b.v[1] - a.v[1] * b.v[0];
+    const Dual<6> c0 = a[1] * b[2] - a[2] * b[1];
+    const Dual<6> c1 = a[2] * b[0] - a[0] * b[2];
+    const Dual<6> c2 = a[0] * b[1] - a[1] * b[0];
     return c0 * c0 + c1 * c1 + c2 * c2;
 }
 
 // angle between two vectors, small-angle form th = sqrt(2 (1 - |cos|)); exactly 0 (value and gradient)
 // below 1e-21 (triangulation.cc:781-817)
-__device__ __forceinline__ Dual6 d6_angle_small(const Vec6& a, const Vec6& b)
+__device__ __forceinline__ Dual<6> d6_angle_small(const Dual<6> a[3], const Dual<6> b[3])
 {
-    Dual6 costh = d6_dot(a, b) / d6_sqrt(d6_dot(a, a) * d6_dot(b, b));
+    Dual<6> costh = d6_dot(a, b) / dsqrt(d6_dot(a, a) * d6_dot(b, b));
     if(costh.x < 0.) costh = -costh;
-    const Dual6 th_sq = costh * (-2.) + 2.;
-    if(th_sq.x < 1e-21) return d6_const(0.);
-    return d6_sqrt(th_sq);
+    const Dual<6> th_sq = costh * (-2.) + 2.;
+    if(th_sq.x < 1e-21) return Dual<6>(0.);
+    return dsqrt(th_sq);
 }
 
 // 0 below 0, 1 above the knee, two parabolas in between (triangulation.cc:893-947)
-__device__ __forceinline__ Dual6 d6_sigmoid(const Dual6& x, double knee)
+__device__ __forceinline__ Dual<6> d6_sigmoid(const Dual<6>& x, double knee)
 {
-    if(x.x <= 0.) return d6_const(0.);
-    if(knee <= x.x) return d6_const(1.);
+    if(x.x <= 0.) return Dual<6>(0.);
+    if(knee <= x.x) return Dual<6>(1.);
     const double b = 2. / knee;
     const double a = (x.x < knee / 2. ? 2. : -2.) / knee / knee;
-    const Dual6 dx = x - knee / 2.;
+    const Dual<6> dx = x - knee / 2.;
     return dx * (dx * a + b) + 0.5;
 }
 
@@ -127,44 +55,45 @@ __device__ __forceinline__ Dual6 d6_sigmoid(const Dual6& x, double knee)
 __device__ inline double triangulated_error(double derr_da[3], double derr_dt[3],
                                             const double v_fixed[3], const double a_in[3], const double t_in[3])
 {
-    Vec6 v0, v1, t01;
+    // values and gradients with respect to (a[0..2], t[0..2])
+    Dual<6> v0[3], v1[3], t01[3];
 #pragma unroll
     for(int i = 0; i < 3; i++)
     {
-        v0.v[i] = d6_const(v_fixed[i]);
-        v1.v[i] = d6_var(a_in[i], i);
-        t01.v[i] = d6_var(t_in[i], 3 + i);
+        v0[i] = Dual<6>(v_fixed[i]);
+        v1[i] = Dual<6>::var(a_in[i], i);
+        t01[i] = Dual<6>::var(t_in[i], 3 + i);
     }
-    const Dual6 p_norm2_recip = d6_const(1.) / d6_cross_norm2(v0, v1);
-    const Dual6 l0 = d6_sqrt(d6_cross_norm2(v1, t01) * p_norm2_recip);
-    const Dual6 l1 = d6_sqrt(d6_cross_norm2(v0, t01) * p_norm2_recip);
-    Vec6 m;
+    const Dual<6> p_norm2_recip = Dual<6>(1.) / d6_cross_norm2(v0, v1);
+    const Dual<6> l0 = dsqrt(d6_cross_norm2(v1, t01) * p_norm2_recip);
+    const Dual<6> l1 = dsqrt(d6_cross_norm2(v0, t01) * p_norm2_recip);
+    Dual<6> m[3];
 #pragma unroll
-    for(int i = 0; i < 3; i++) m.v[i] = (v0.v[i] * l0 + t01.v[i] + v1.v[i] * l1) * 0.5;
-    Dual6 err = d6_angle_small(v0, m) * 2.;
+    for(int i = 0; i < 3; i++) m[i] = (v0[i] * l0 + t01[i] + v1[i] * l1) * 0.5;
+    Dual<6> err = d6_angle_small(v0, m) * 2.;
 
     // cheirality: does flipping the sign of l0, l1 or both bring the two estimates of the point closer?
-    Dual6 w0 = d6_const(0.), w1 = d6_const(0.), w01 = d6_const(0.);
+    Dual<6> w0(0.), w1(0.), w01(0.);
 #pragma unroll
     for(int i = 0; i < 3; i++)
     {
-        const Dual6 far = l1 * v1.v[i], near = l0 * v0.v[i];
-        const Dual6 xn  = (far + t01.v[i]) - near;
-        const Dual6 x0  = (far + t01.v[i]) + near;
-        const Dual6 x1  = (t01.v[i] - far) - near;
-        const Dual6 x01 = (t01.v[i] - far) + near;
-        const Dual6 n2 = xn * xn;
+        const Dual<6> far = l1 * v1[i], near = l0 * v0[i];
+        const Dual<6> xn  = (far + t01[i]) - near;
+        const Dual<6> x0  = (far + t01[i]) + near;
+        const Dual<6> x1  = (t01[i] - far) - near;
+        const Dual<6> x01 = (t01[i] - far) + near;
+        const Dual<6> n2 = xn * xn;
         w0  = w0 + (x0 * x0 - n2);
         w1  = w1 + (x1 * x1 - n2);
         w01 = w01 + (x01 * x01 - n2);
     }
     if(!(w0.x > 0. && w1.x > 0. && w01.x > 0.))
     {
-        const Dual6 to_vanishing_point = d6_angle_small(v0, v1);
+        const Dual<6> to_vanishing_point = d6_angle_small(v0, v1);
         err = err + to_vanishing_point * (d6_sigmoid(-w0, 3.) + d6_sigmoid(-w1, 3.) + d6_sigmoid(-w01, 3.));
     }
 #pragma unroll
-    for(int i = 0; i < 3; i++) { derr_da[i] = err.g[i]; derr_dt[i] = err.g[3 + i]; }
+    for(int i = 0; i < 3; i++) { derr_da[i] = err.j[i]; derr_dt[i] = err.j[3 + i]; }
     return err.x;
 }
 

@@ -20,7 +20,8 @@ import numpy as np
 
 from . import _capi
 from ._capi import lib
-from .api import _compose_Rt, _lensmodel, _ptr, _require_gpu, lensmodel_metadata_and_config, unproject
+from ._poses_host import compose_Rt
+from .api import _lensmodel, _ptr, _require_gpu, lensmodel_metadata_and_config, unproject
 from .cameramodel import cameramodel
 
 INTER_NEAREST = 0
@@ -143,7 +144,7 @@ def image_transformation_map(model_from, model_to, *, intrinsics_only=False, dis
                                "valid_intrinsics_region")
         region = np.ascontiguousarray(region, np.float64)
     Rt_to_from = None if intrinsics_only else \
-        np.ascontiguousarray(_compose_Rt(model_to.Rt_cam_ref(), model_from.Rt_ref_cam()), np.float64)
+        np.ascontiguousarray(compose_Rt(model_to.Rt_cam_ref(), model_from.Rt_ref_cam()), np.float64)
     if plane_n is not None:
         plane_n = np.ascontiguousarray(plane_n, np.float64)
         if plane_n.shape != (3,):

@@ -28,68 +28,8 @@ import heapq
 
 import numpy as np
 
-
-# --------------------------------------------------------------------------- poses
-def R_from_r(r):
-    r = np.asarray(r, float)
-    th = np.linalg.norm(r)
-    if th < 1e-12:
-        K = np.array(((0, -r[2], r[1]), (r[2], 0, -r[0]), (-r[1], r[0], 0)))
-        return np.eye(3) + K
-    k = r / th
-    K = np.array(((0, -k[2], k[1]), (k[2], 0, -k[0]), (-k[1], k[0], 0)))
-    return np.eye(3) + np.sin(th) * K + (1 - np.cos(th)) * (K @ K)
-
-
-def r_from_R(R):
-    R = np.asarray(R, float)
-    c = (np.trace(R) - 1.) / 2.
-    c = min(1., max(-1., c))
-    th = np.arccos(c)
-    v = np.array((R[2, 1] - R[1, 2], R[0, 2] - R[2, 0], R[1, 0] - R[0, 1]))
-    if th < 1e-9:
-        return v / 2.
-    if np.pi - th < 1e-6:
-        # near pi: the axis from the symmetric part
-        A = (R + np.eye(3)) / 2.
-        k = np.sqrt(np.maximum(np.diag(A), 0.))
-        i = int(np.argmax(k))
-        k = A[i] / k[i]
-        if np.dot(k, v) < 0:
-            k = -k
-        return k * th
-    return v / (2. * np.sin(th)) * th
-
-
-def Rt_from_rt(rt):
-    rt = np.asarray(rt, float)
-    if rt.ndim > 1:
-        return np.array([Rt_from_rt(x) for x in rt])
-    return np.concatenate((R_from_r(rt[:3]), rt[None, 3:]), 0)
-
-
-def rt_from_Rt(Rt):
-    Rt = np.asarray(Rt, float)
-    if Rt.ndim > 2:
-        return np.array([rt_from_Rt(x) for x in Rt]).reshape(Rt.shape[:-2] + (6,))
-    return np.concatenate((r_from_R(Rt[:3]), Rt[3]))
-
-
-def invert_Rt(Rt):
-    Rt = np.asarray(Rt, float)
-    if Rt.ndim > 2:
-        return np.array([invert_Rt(x) for x in Rt]).reshape(Rt.shape)
-    R = Rt[:3]
-    return np.concatenate((R.T, (-R.T @ Rt[3])[None]), 0)
-
-
-def compose_Rt(Rt0, Rt1):
-    """x -> Rt0(Rt1(x))"""
-    return np.concatenate((Rt0[:3] @ Rt1[:3], (Rt0[:3] @ Rt1[3] + Rt0[3])[None]), 0)
-
-
-def transform_point_Rt(Rt, p):
-    return np.asarray(p, float) @ Rt[:3].T + Rt[3]
+# absolute, so that this file also runs when loaded by its path rather than as part of the package
+from mrcal_b200._poses_host import R_from_r, Rt_from_rt, compose_Rt, invert_Rt, r_from_R, rt_from_Rt, transform_point_Rt
 
 
 def ref_calibration_object(W, H, object_spacing, calobject_warp=None):

@@ -24,7 +24,8 @@ import numpy as np
 
 from . import _capi
 from ._capi import lib
-from .api import _compose_Rt, _lensmodel, _ptr, _require_gpu, lensmodel_metadata_and_config
+from ._poses_host import compose_Rt
+from .api import _lensmodel, _ptr, _require_gpu, lensmodel_metadata_and_config
 from .cameramodel import cameramodel
 from .image_transforms import _fail
 
@@ -121,7 +122,7 @@ def _validate_models_rectified(models_rectified):
     if len(models_rectified) != 2:
         raise RuntimeError(f"Must have received exactly two models. Got {len(models_rectified)} instead")
     intrinsics = [m.intrinsics() for m in models_rectified]
-    Rt01 = _compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())
+    Rt01 = compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())
     if not ((intrinsics[0][0] == "LENSMODEL_LATLON" and intrinsics[1][0] == "LENSMODEL_LATLON") or
             (intrinsics[0][0] == "LENSMODEL_PINHOLE" and intrinsics[1][0] == "LENSMODEL_PINHOLE")):
         raise RuntimeError(f"Expected two models with the same  'LENSMODEL_LATLON' or 'LENSMODEL_PINHOLE' but got "
@@ -188,7 +189,7 @@ def _range_arguments(disparity, models_rectified, disparity_scale, disparity_min
     is_scalar = np.ndim(disparity) == 0
     if is_scalar:
         disparity = np.array((disparity,))
-    Rt01 = _compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())
+    Rt01 = compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())
     rect, fxycxy = models_rectified[0].intrinsics()
     return dict(disparity=disparity, is_scalar=is_scalar, baseline=float(np.linalg.norm(Rt01[3, :])),
                 rect=_rectification_model_type(rect), fxycxy=np.ascontiguousarray(fxycxy, np.float64),
@@ -262,7 +263,7 @@ def stereo_unproject(disparity, models_rectified, *, ranges=None, disparity_scal
     fxycxy = np.ascontiguousarray(fxycxy, np.float64)
     if ranges is not None:
         _require_gpu()
-        Rt01 = _compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())
+        Rt01 = compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())
         baseline = float(np.linalg.norm(Rt01[3, :]))
         rg = np.asarray(ranges, np.float64)
         if qrect0 is None:

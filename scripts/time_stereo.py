@@ -11,7 +11,7 @@ import numpy as np
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
 sys.path.insert(0, ROOT)
 import mrcal_b200  # noqa: E402
-from mrcal_b200.seeding import rt_from_Rt  # noqa: E402
+from mrcal_b200._poses_host import Rt_from_rt, compose_Rt, rt_from_Rt  # noqa: E402
 from oracle import stereo_ref as ref  # noqa: E402
 import measure  # noqa: E402
 
@@ -19,10 +19,7 @@ import measure  # noqa: E402
 def pair(names, rt01=(0.1, 0.2, 0.05, 3.0, 0.2, 1.0)):
     gold = os.path.join(ROOT, "tests", "golden", "cameramodels")
     m0, m1 = (mrcal_b200.cameramodel(os.path.join(gold, n)) for n in names)
-    from mrcal_b200.cameramodel import _R_from_r
-    Rt = m0.Rt_ref_cam()
-    rt01 = np.array(rt01)
-    m1.rt_ref_cam(rt_from_Rt(np.vstack((Rt[:3] @ _R_from_r(rt01[:3]), Rt[:3] @ rt01[3:] + Rt[3]))))
+    m1.rt_ref_cam(rt_from_Rt(compose_Rt(m0.Rt_ref_cam(), Rt_from_rt(rt01))))
     return m0, m1
 
 

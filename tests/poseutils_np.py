@@ -175,6 +175,36 @@ def reference(fname, args, kw):
     return getattr(P, fname)(*args, **inv)
 
 
+ROTATION_VECTOR_RESULT = ("r_from_R", "rt_from_Rt", "compose_r", "compose_rt")
+
+
+def check_value(key, fname, got, want, R_from_r):
+    """Asserts that got, the value output of fname, matches want, the reference's, to 1e-12 of the largest |want|.
+    Returns the mask of the elements compared element by element, which is where gradients can be compared too"""
+    assert got.shape == want.shape, key
+    ok = np.ones(want.shape[:1], bool)
+    if fname in ROTATION_VECTOR_RESULT:
+        # Within ~1e-3 of a half-turn the reference takes the angle from acos() of a cosine near -1, or from
+        # sqrt((1 + R_ii)/2): it loses up to half its digits there, and r and the equivalent rotation of angle
+        # |r| - 2 pi are both valid answers. There the results are compared as rotations, to the ~1e-8 that
+        # conditioning allows, and the gradients of the rotation part (ill-conditioned) are not compared
+        r_ref = want[..., :3]
+        near = np.abs(np.linalg.norm(r_ref, axis=-1) - np.pi) < 1e-3
+        if near.any():
+            Rg = R_from_r(got[near][..., :3])
+            Rw = R_from_r(r_ref[near])
+            assert np.abs(Rg - Rw).max() < 1e-8, key
+            t_err = np.abs(got[near][..., 3:] - want[near][..., 3:])
+            assert t_err.size == 0 or t_err.max() <= 1e-8 * (1 + np.abs(want).max()), key
+        ok = ~near
+    g, w = got[ok], want[ok]
+    err = np.abs(g - w).reshape(len(g), -1).max(-1)
+    tol = 1e-12 * max(1., np.abs(w).max())
+    bad = np.nonzero(err > tol)[0]
+    assert len(bad) == 0, f"{key} output 0: element {bad[:3]} error {err[bad[:3]]} > {tol}"
+    return ok
+
+
 def load():
     """[(key, fname, inputs, kwargs, tags, answers)]: the answers from the compiled reference where it is built, from
     tests/golden/poseutils.npz otherwise"""

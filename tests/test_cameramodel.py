@@ -47,14 +47,6 @@ def test_roundtrip_explicit_model():
         cm.cameramodel(intrinsics=("LENSMODEL_OPENCV8", intr[:8]), imagersize=(10, 10))
 
 
-def test_inverse_pose_matches_reference(ref):
-    rng = np.random.default_rng(0)
-    for _ in range(5):
-        rt = rng.normal(size=6)
-        assert np.allclose(cm.invert_rt(rt), ref.invert_rt(rt), atol=1e-12)
-    assert np.allclose(cm.invert_rt(np.array((0., 0., 0., 1., 2., 3.))), (0., 0., 0., -1., -2., -3.))
-
-
 def test_model_from_a_solve_roundtrips_its_inputs(tmp_path):
     kw = dict(problems.golden_cases())["opencv8_points_fixed"]   # 3 cameras, camera 0 at the reference
     m = cm.cameramodel(optimization_inputs=kw, icam_intrinsics=2)

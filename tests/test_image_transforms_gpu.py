@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 import mrcal_b200
-from mrcal_b200.seeding import rt_from_Rt
+from mrcal_b200._poses_host import rt_from_Rt
 
 import remap_np
 

@@ -4,37 +4,10 @@ CPU: the pieces against known answers (an exact pinhole/stereographic camera giv
 through true stereographic lenses seeds close to the truth). GPU: the reference's own end-to-end flow,
 test/test-basic-calibration.py:45-209 -- seed_stereographic(), then optimize() in stages with a growing set of
 unknowns, noise and gross outliers in the data -- judged by that test's tolerances."""
-import importlib.util
-import os
-
 import numpy as np
 import pytest
 
-ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
-
-
-def _load(name):
-    # by path: the CPU tests must not need the CUDA library
-    spec = importlib.util.spec_from_file_location(f"_mb200_{name}", os.path.join(ROOT, "mrcal_b200", f"{name}.py"))
-    m = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(m)
-    return m
-
-
-S = _load("seeding")
-synthetic = _load("synthetic")
-
-
-def test_pose_utilities_roundtrip():
-    rng = np.random.default_rng(0)
-    for _ in range(20):
-        rt = np.concatenate((rng.uniform(-1.7, 1.7, 3), rng.uniform(-3, 3, 3)))   # |r| < pi
-        Rt = S.Rt_from_rt(rt)
-        assert np.allclose(S.rt_from_Rt(Rt), rt, atol=1e-12)
-        assert np.allclose(S.compose_Rt(Rt, S.invert_Rt(Rt)), np.concatenate((np.eye(3), np.zeros((1, 3)))), atol=1e-12)
-    # rotation by almost pi
-    r = np.array((0.3, -0.2, 0.9)); r *= (np.pi - 1e-8) / np.linalg.norm(r)
-    assert np.allclose(S.R_from_r(S.r_from_R(S.R_from_r(r))), S.R_from_r(r), atol=1e-7)
+from mrcal_b200 import seeding as S, synthetic
 
 
 def test_procrustes_known_answer():

@@ -9,6 +9,7 @@ import pytest
 
 import mrcal_b200
 from mrcal_b200 import _capi, stereo
+from mrcal_b200._poses_host import Rt_from_rt, compose_Rt, rt_from_Rt
 
 MODELS = os.path.join(os.path.dirname(__file__), "golden", "cameramodels")
 
@@ -23,21 +24,11 @@ def stereo_oracle():
     return stereo_ref
 
 
-def _R_from_r(r):
-    from mrcal_b200.cameramodel import _R_from_r
-    return _R_from_r(np.asarray(r, float))
-
-
 def _pair(rt01=(0., 0., 0., 3., 0., 0.), name="cam0.opencv8.cameramodel"):
     """camera 1 at rt01 from camera 0 (rt01 maps camera-1 coordinates to camera 0)"""
     m0 = mrcal_b200.cameramodel(os.path.join(MODELS, name))
     m1 = mrcal_b200.cameramodel(m0)
-    rt01 = np.array(rt01, float)
-    Rt_ref_cam0 = m0.Rt_ref_cam()
-    R01, t01 = _R_from_r(rt01[:3]), rt01[3:]
-    Rt_ref_cam1 = np.vstack((Rt_ref_cam0[:3] @ R01, Rt_ref_cam0[:3] @ t01 + Rt_ref_cam0[3]))
-    from mrcal_b200.seeding import rt_from_Rt
-    m1.rt_ref_cam(rt_from_Rt(Rt_ref_cam1))
+    m1.rt_ref_cam(rt_from_Rt(compose_Rt(m0.Rt_ref_cam(), Rt_from_rt(rt01))))
     return m0, m1
 
 

@@ -10,7 +10,7 @@ import scipy.interpolate
 
 import mrcal_b200
 from mrcal_b200 import _capi, stereo
-from mrcal_b200.seeding import rt_from_Rt
+from mrcal_b200._poses_host import R_from_r, Rt_from_rt, compose_Rt, invert_Rt, rt_from_Rt, transform_point_Rt
 
 pytestmark = pytest.mark.gpu
 
@@ -28,34 +28,13 @@ def stereo_oracle():
     return stereo_ref
 
 
-def _R_from_r(r):
-    from mrcal_b200.cameramodel import _R_from_r
-    return _R_from_r(np.asarray(r, float))
-
-
-def _Rt(rt):
-    return np.vstack((_R_from_r(rt[:3]), rt[3:]))
-
-
-def _compose_Rt(A, B):
-    return np.vstack((A[:3] @ B[:3], A[:3] @ B[3] + A[3]))
-
-
-def _invert_Rt(Rt):
-    return np.vstack((Rt[:3].T, -Rt[:3].T @ Rt[3]))
-
-
-def _transform(Rt, p):
-    return p @ Rt[:3].T + Rt[3]
-
-
 def _model(name):
     return mrcal_b200.cameramodel(os.path.join(MODELS, name))
 
 
 def _place(m0, m1, rt01):
     """camera 1 at rt01 from camera 0 (rt01 maps camera-1 coordinates to camera-0 coordinates)"""
-    m1.rt_ref_cam(rt_from_Rt(_compose_Rt(m0.Rt_ref_cam(), _Rt(np.asarray(rt01, float)))))
+    m1.rt_ref_cam(rt_from_Rt(compose_Rt(m0.Rt_ref_cam(), Rt_from_rt(np.asarray(rt01, float)))))
 
 
 def _unit(v):
@@ -101,15 +80,15 @@ def test_reference_stereo(stereo_oracle, rect):
         _check_against_reference((model0, model1), models_rectified, meta, stereo_oracle, rect, el0_deg=el0_deg, **kw)
         stereo._validate_models_rectified(models_rectified)
         assert models_rectified[0].intrinsics()[0] == rect and models_rectified[1].intrinsics()[0] == rect
-        Rt_cam0_rect = _compose_Rt(model0.Rt_cam_ref(), models_rectified[0].Rt_ref_cam())
-        Rt01_rectified = _compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())
+        Rt_cam0_rect = compose_Rt(model0.Rt_cam_ref(), models_rectified[0].Rt_ref_cam())
+        Rt01_rectified = compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())
         if geometry == "vanilla":
             az0, el0 = 0., 0.
             assert np.abs(Rt_cam0_rect - np.vstack((np.eye(3), np.zeros(3)))).max() < 1e-6
         else:
             el0 = el0_deg * np.pi / 180.
             baseline = rt01[3:] / np.linalg.norm(rt01[3:])
-            forward01 = np.array((0, 0, 1.)) + _R_from_r(rt01[:3]) @ np.array((0, 0, 1.))
+            forward01 = np.array((0, 0, 1.)) + R_from_r(rt01[:3]) @ np.array((0, 0, 1.))
             az0 = np.arcsin(np.dot(forward01, baseline) / np.linalg.norm(forward01))
             # the geometry the reference pins (test-stereo.py:297-302)
             assert np.abs(Rt_cam0_rect - np.array([[0.9467916, -0.08500675, -0.31041828],
@@ -152,9 +131,9 @@ def test_reference_stereo(stereo_oracle, rect):
     # the rest on the complex geometry, as the reference: points seen by both cameras
     pcam0 = np.array(((1., 2., 12.), (-4., 3., 12.)))
     qcam0 = mrcal_b200.project(pcam0, *model0.intrinsics())
-    pcam1 = _transform(_invert_Rt(_Rt(rt01)), pcam0)
+    pcam1 = transform_point_Rt(invert_Rt(Rt_from_rt(rt01)), pcam0)
     qcam1 = mrcal_b200.project(pcam1, *model1.intrinsics())
-    prect0 = _transform(_invert_Rt(Rt_cam0_rect), pcam0)
+    prect0 = transform_point_Rt(invert_Rt(Rt_cam0_rect), pcam0)
     prect1 = prect0 - Rt01_rectified[3, :]
     qrect0 = mrcal_b200.project(prect0, *models_rectified[0].intrinsics())
     qrect1 = mrcal_b200.project(prect1, *models_rectified[1].intrinsics())
@@ -289,7 +268,7 @@ def _disparity_image(rng, H, W, pad):
 
 
 def _baseline(models_rectified):
-    return float(np.linalg.norm(_compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())[3]))
+    return float(np.linalg.norm(compose_Rt(models_rectified[0].Rt_cam_ref(), models_rectified[1].Rt_ref_cam())[3]))
 
 
 # 3. the ranges against the reference's C functions
