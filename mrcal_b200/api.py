@@ -22,7 +22,7 @@ import numpy as np
 import scipy.sparse
 
 from . import _capi
-from ._capi import lib
+from ._capi import checked
 from ._poses_host import compose_Rt, invert_Rt
 
 _KNOWN_KWARGS = {
@@ -47,7 +47,7 @@ def _lensmodel(name):
     if not isinstance(name, str):
         raise RuntimeError("The lens model must be given as a string")
     lm = _capi.Lensmodel()
-    if not lib.mrcal_lensmodel_from_name(C.byref(lm), name.encode()):
+    if not checked.mrcal_lensmodel_from_name(C.byref(lm), name.encode()):
         t = lm.type
         if t == -1:
             raise RuntimeError(f"Couldn't parse the configuration of the given lens model '{name}'")
@@ -163,7 +163,7 @@ class _Inputs:
         if self.intrinsics.shape[0] != self.imagersizes.shape[0]:
             raise RuntimeError(f"Inconsistent Ncameras: 'intrinsics' says {self.intrinsics.shape[0]}, "
                                f"'imagersizes' says {self.imagersizes.shape[0]}")
-        Nintr = lib.mrcal_lensmodel_num_params(C.byref(self.lensmodel))
+        Nintr = checked.mrcal_lensmodel_num_params(C.byref(self.lensmodel))
         if self.intrinsics.shape[0] and self.intrinsics.shape[1] != Nintr:
             raise RuntimeError(f"intrinsics.shape[-1] MUST be {Nintr} for {self.lensmodel_name}. "
                                f"Instead got {self.intrinsics.shape[1]}")
@@ -270,8 +270,7 @@ class _Inputs:
                     q = np.ascontiguousarray(self.observations_tri[sel, :2])
                     v = np.zeros((len(sel), 3))
                     intr = np.ascontiguousarray(self.intrinsics[icam])
-                    if not lib.mrcal_unproject(_ptr(v), _ptr(q), len(sel), self.lm_ref(), _ptr(intr)):
-                        raise RuntimeError("mrcal_unproject() failed: " + _capi.last_error())
+                    checked.mrcal_unproject(_ptr(v), _ptr(q), len(sel), self.lm_ref(), _ptr(intr))
                     rays[sel] = v
             arr = (_capi.ObservationPointTriangulated * self.Nobs_tri)()
             last = np.concatenate((np.diff(it[:, 0]) != 0, [True]))
@@ -284,6 +283,18 @@ class _Inputs:
             self._tri_has_rays = bool(want)
         return self._tri, self.Nobs_tri
 
+    def c_problem(self):
+        """The arguments intrinsics .. problem_selections that mrcal_optimizer_callback(), mrcal_optimize() and
+        mrcal_b200_problem_create_triangulated() share, with the triangulated observations as rays. The pointers keep
+        their arrays alive"""
+        ob, op = self.c_observations()
+        tri, ntri = self.c_triangulated(rays=True)
+        return (_ptr(self.intrinsics), _ptr(self.rt_cam_ref), _ptr(self.rt_ref_frame), _ptr(self.points),
+                _ptr(self.calobject_warp), self.Ncam_i, self.Ncam_e, self.Nframes, self.Npoints, self.Npoints_fixed,
+                _ptr(ob), _ptr(op), self.Nobs_board, self.Nobs_point, tri, ntri,
+                _ptr(self.observations_board), _ptr(self.observations_point), self.lm_ref(), _ptr(self.imagersizes),
+                self.selections)
+
     def counts(self):
         return (self.Ncam_i, self.Ncam_e, self.Nframes, self.Npoints, self.Npoints_fixed, self.Nobs_board)
 
@@ -293,24 +304,24 @@ class _Inputs:
         return C.byref(self.lensmodel)
 
     def num_states(self):
-        return lib.mrcal_num_states(*self.counts(), self.selections, self.lm_ref())
+        return checked.mrcal_num_states(*self.counts(), self.selections, self.lm_ref())
 
     def num_measurements(self):
         tri, ntri = self.c_triangulated()
-        return lib.mrcal_num_measurements(self.Nobs_board, self.Nobs_point, tri, ntri, self.W, self.H,
-                                          self.Ncam_i, self.Ncam_e, self.Nframes, self.Npoints, self.Npoints_fixed,
-                                          self.selections, self.lm_ref())
+        return checked.mrcal_num_measurements(self.Nobs_board, self.Nobs_point, tri, ntri, self.W, self.H,
+                                              self.Ncam_i, self.Ncam_e, self.Nframes, self.Npoints, self.Npoints_fixed,
+                                              self.selections, self.lm_ref())
 
     def num_j_nonzero(self):
         ob, op = self.c_observations()
         tri, ntri = self.c_triangulated()
-        return lib._mrcal_num_j_nonzero(self.Nobs_board, self.Nobs_point, tri, ntri, self.W, self.H,
-                                        self.Ncam_i, self.Ncam_e, self.Nframes, self.Npoints, self.Npoints_fixed,
-                                        _ptr(ob), _ptr(op), self.selections, self.lm_ref())
+        return checked._mrcal_num_j_nonzero(self.Nobs_board, self.Nobs_point, tri, ntri, self.W, self.H,
+                                            self.Ncam_i, self.Ncam_e, self.Nframes, self.Npoints, self.Npoints_fixed,
+                                            _ptr(ob), _ptr(op), self.selections, self.lm_ref())
 
 
 def _require_gpu():
-    if lib.mrcal_b200_device_count() <= 0:
+    if checked.mrcal_b200_device_count() <= 0:
         raise RuntimeError("mrcal_b200: no usable CUDA device. This backend has no CPU fallback")
 
 
@@ -433,10 +444,8 @@ def implied_Rt10__from_unprojections(q0, p0, v1, *, weights=None, atinfinity=Tru
             raise RuntimeError(f"weights must have the shape of p0 without its last dimension; got {weights.shape}")
     fc = np.ascontiguousarray(focus_center, np.float64).reshape(2)
     Rt = np.zeros((4, 3))
-    if not lib.mrcal_b200_implied_Rt10__from_unprojections(_ptr(Rt), _ptr(q0), N, _ptr(p0), M, _ptr(v1),
-                                                           _ptr(weights) if weights is not None else None,
-                                                           bool(atinfinity), _ptr(fc), float(focus_radius)):
-        raise RuntimeError(_capi.last_error())
+    checked.mrcal_b200_implied_Rt10__from_unprojections(_ptr(Rt), _ptr(q0), N, _ptr(p0), M, _ptr(v1), _ptr(weights),
+                                                        bool(atinfinity), _ptr(fc), float(focus_radius))
     return Rt
 
 
@@ -522,11 +531,9 @@ def projection_diff(models, *, implied_Rt10=None, gridn_width=60, gridn_height=N
     diff = np.zeros((Nd, N, 2)) if Nmodels == 2 else None
     fc = np.ascontiguousarray(focus_center, np.float64).reshape(2)
     U = np.ascontiguousarray(uncertainties.reshape(Nmodels, Nd, N)) if uncertainties is not None and fit else None
-    if not lib.mrcal_b200_projection_diff(_ptr(Rt10), _ptr(difflen), _ptr(diff) if diff is not None else None,
-                                          _ptr(qq), N, _ptr(vv), Nmodels, None if atinfinity else _ptr(dist), Nd,
-                                          lms, _ptr(intr), _ptr(U) if U is not None else None, _ptr(fc),
-                                          float(focus_radius), fit):
-        raise RuntimeError(_capi.last_error())
+    checked.mrcal_b200_projection_diff(_ptr(Rt10), _ptr(difflen), _ptr(diff), _ptr(qq), N, _ptr(vv), Nmodels,
+                                       None if atinfinity else _ptr(dist), Nd, lms, _ptr(intr), _ptr(U), _ptr(fc),
+                                       float(focus_radius), fit)
 
     difflen = difflen.reshape((Nd,) + q0.shape[:2])
     if diff is not None:
@@ -559,9 +566,8 @@ def model_resolution__deg_pixel(q, model, *, mode="mean"):
     intr = np.ascontiguousarray(intrinsics, dtype=np.float64)
     flat = q.reshape(-1, 2)
     out = np.zeros(flat.shape[0])
-    if not lib.mrcal_b200_model_resolution__deg_pixel(_ptr(out), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr),
-                                                      _RESOLUTION_MODES[mode]):
-        raise RuntimeError("model_resolution__deg_pixel() failed: " + _capi.last_error())
+    checked.mrcal_b200_model_resolution__deg_pixel(_ptr(out), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr),
+                                                   _RESOLUTION_MODES[mode])
     return out.reshape(q.shape[:-1])
 
 
@@ -577,9 +583,8 @@ def _stereo_pair_reproject(q, models, Rts, distance):
     Rt = np.ascontiguousarray(Rts, np.float64)
     out = np.zeros(flat.shape)
     outlen = np.zeros(flat.shape[0])
-    if not lib.mrcal_b200_stereo_pair_reproject(_ptr(out), _ptr(outlen), _ptr(flat), flat.shape[0], len(models) // 2,
-                                                lms, _ptr(intr), _ptr(Rt), float(distance)):
-        raise RuntimeError("stereo_pair_diff() failed: " + _capi.last_error())
+    checked.mrcal_b200_stereo_pair_reproject(_ptr(out), _ptr(outlen), _ptr(flat), flat.shape[0], len(models) // 2, lms,
+                                             _ptr(intr), _ptr(Rt), float(distance))
     return out.reshape(q.shape), outlen.reshape(q.shape[:-1])
 
 
@@ -655,20 +660,8 @@ def optimizer_callback(no_jacobian=False, no_factorization=False, **kwargs):
         Jt = _capi.Sparse(nrow=Nstate, ncol=Nmeas, nzmax=nnz, p=P.ctypes.data, i=Ii.ctypes.data, x=X.ctypes.data,
                           sorted=1, packed=1)
         keep = (P, Ii, X)
-    ob, op = I.c_observations()
-    tri, ntri = I.c_triangulated(rays=True)
-    ok = lib.mrcal_optimizer_callback(
-        _ptr(b), C.c_int(b.nbytes), _ptr(x), C.c_int(x.nbytes),
-        C.byref(Jt) if Jt is not None else None,
-        _ptr(I.intrinsics), _ptr(I.rt_cam_ref), _ptr(I.rt_ref_frame), _ptr(I.points),
-        _ptr(I.calobject_warp) if I.calobject_warp is not None else None,
-        I.Ncam_i, I.Ncam_e, I.Nframes, I.Npoints, I.Npoints_fixed,
-        _ptr(ob), _ptr(op), I.Nobs_board, I.Nobs_point, tri, ntri,
-        _ptr(I.observations_board), _ptr(I.observations_point),
-        I.lm_ref(), _ptr(I.imagersizes), I.selections, None,
-        C.c_double(I.spacing), max(I.W, 0), max(I.H, 0), C.c_bool(I.verbose))
-    if not ok:
-        raise RuntimeError("mrcal_optimizer_callback() failed: " + _capi.last_error())
+    checked.mrcal_optimizer_callback(_ptr(b), b.nbytes, _ptr(x), x.nbytes, C.byref(Jt) if Jt is not None else None,
+                                     *I.c_problem(), None, I.spacing, max(I.W, 0), max(I.H, 0), I.verbose)
     J = None
     factorization = None
     if keep is not None:
@@ -687,7 +680,7 @@ def optimizer_callback(no_jacobian=False, no_factorization=False, **kwargs):
                         raise
                     factorization = None
             else:
-                h = lib.mrcal_b200_factorization_create_from_last_callback()   # NULL comes back as None
+                h = checked.mrcal_b200_factorization_create_from_last_callback()   # NULL comes back as None
                 if h:
                     factorization = CHOLMOD_factorization._from_handle(h, J.shape)
                 elif "not positive definite" not in _capi.last_error():
@@ -710,17 +703,8 @@ def optimize(**kwargs):
     Nstate, Nmeas = I.num_states(), I.num_measurements()
     b = np.zeros(Nstate)
     x = np.zeros(Nmeas)
-    ob, op = I.c_observations()
-    tri, ntri = I.c_triangulated(rays=True)
-    stats = lib.mrcal_optimize(
-        _ptr(b), C.c_int(b.nbytes), _ptr(x), C.c_int(x.nbytes),
-        _ptr(I.intrinsics), _ptr(I.rt_cam_ref), _ptr(I.rt_ref_frame), _ptr(I.points),
-        _ptr(I.calobject_warp) if I.calobject_warp is not None else None,
-        I.Ncam_i, I.Ncam_e, I.Nframes, I.Npoints, I.Npoints_fixed,
-        _ptr(ob), _ptr(op), I.Nobs_board, I.Nobs_point, tri, ntri,
-        _ptr(I.observations_board), _ptr(I.observations_point),
-        I.lm_ref(), _ptr(I.imagersizes), I.selections, None,
-        C.c_double(I.spacing), max(I.W, 0), max(I.H, 0), C.c_bool(I.verbose), C.c_bool(False))
+    stats = checked.mrcal_optimize(_ptr(b), b.nbytes, _ptr(x), x.nbytes, *I.c_problem(), None, I.spacing, max(I.W, 0),
+                                   max(I.H, 0), I.verbose, False)
     if stats.rms_reproj_error__pixels < 0.0:
         raise RuntimeError("mrcal.optimize() failed! " + _capi.last_error())
     return dict(rms_reproj_error__pixels=stats.rms_reproj_error__pixels,
@@ -738,8 +722,7 @@ def check_gradient(**kwargs):
     import tempfile
     _require_gpu()
     I = _Inputs(kwargs)
-    ob, op = I.c_observations()
-    tri, ntri = I.c_triangulated(rays=True)
+    problem = I.c_problem()
     sys_stdout_fd = 1
     with tempfile.TemporaryFile(mode="w+b") as tmp:
         import sys as _sys
@@ -747,15 +730,7 @@ def check_gradient(**kwargs):
         saved = os.dup(sys_stdout_fd)
         os.dup2(tmp.fileno(), sys_stdout_fd)
         try:
-            lib.mrcal_optimize(
-                None, C.c_int(0), None, C.c_int(0),
-                _ptr(I.intrinsics), _ptr(I.rt_cam_ref), _ptr(I.rt_ref_frame), _ptr(I.points),
-                _ptr(I.calobject_warp) if I.calobject_warp is not None else None,
-                I.Ncam_i, I.Ncam_e, I.Nframes, I.Npoints, I.Npoints_fixed,
-                _ptr(ob), _ptr(op), I.Nobs_board, I.Nobs_point, tri, ntri,
-                _ptr(I.observations_board), _ptr(I.observations_point),
-                I.lm_ref(), _ptr(I.imagersizes), I.selections, None,
-                C.c_double(I.spacing), max(I.W, 0), max(I.H, 0), C.c_bool(False), C.c_bool(True))
+            checked.mrcal_optimize(None, 0, None, 0, *problem, None, I.spacing, max(I.W, 0), max(I.H, 0), False, True)
         finally:
             os.dup2(saved, sys_stdout_fd)
             os.close(saved)
@@ -773,26 +748,15 @@ class Problem:
     def __init__(self, **kwargs):
         _require_gpu()
         I = self._I = _Inputs(kwargs)
-        ob, op = I.c_observations()
-        tri, ntri = I.c_triangulated(rays=True)
-        self._h = lib.mrcal_b200_problem_create_triangulated(
-            _ptr(I.intrinsics), _ptr(I.rt_cam_ref), _ptr(I.rt_ref_frame), _ptr(I.points),
-            _ptr(I.calobject_warp) if I.calobject_warp is not None else None,
-            I.Ncam_i, I.Ncam_e, I.Nframes, I.Npoints, I.Npoints_fixed,
-            _ptr(ob), _ptr(op), I.Nobs_board, I.Nobs_point, tri, ntri,
-            _ptr(I.observations_board), _ptr(I.observations_point),
-            I.lm_ref(), _ptr(I.imagersizes), I.selections,
-            C.c_double(I.spacing), max(I.W, 0), max(I.H, 0))
-        if not self._h:
-            raise RuntimeError("mrcal_b200_problem_create() failed: " + _capi.last_error())
-        self._h = C.c_void_p(self._h)
-        self.Nstate = lib.mrcal_b200_problem_num_states(self._h)
-        self.Nmeasurements = lib.mrcal_b200_problem_num_measurements(self._h)
-        self.N_j_nonzero = lib.mrcal_b200_problem_num_j_nonzero(self._h)
+        self._h = C.c_void_p(checked.mrcal_b200_problem_create_triangulated(*I.c_problem(), I.spacing, max(I.W, 0),
+                                                                            max(I.H, 0)))
+        self.Nstate = checked.mrcal_b200_problem_num_states(self._h)
+        self.Nmeasurements = checked.mrcal_b200_problem_num_measurements(self._h)
+        self.N_j_nonzero = checked.mrcal_b200_problem_num_j_nonzero(self._h)
 
     def close(self):
         if getattr(self, "_h", None):
-            lib.mrcal_b200_problem_destroy(self._h)
+            checked.mrcal_b200_problem_destroy(self._h)
             self._h = None
 
     __del__ = close
@@ -801,23 +765,19 @@ class Problem:
         if b_packed is not None:
             b_packed = np.ascontiguousarray(b_packed, np.float64)
             assert b_packed.shape == (self.Nstate,)
-        if not lib.mrcal_b200_problem_reset(self._h, _ptr(b_packed) if b_packed is not None else None):
-            raise RuntimeError(_capi.last_error())
+        checked.mrcal_b200_problem_reset(self._h, _ptr(b_packed))
 
     def upload(self):
         """Re-send the seed and the observation pool from the host arrays given at construction."""
         I = self._I
-        if not lib.mrcal_b200_problem_upload(self._h, _ptr(I.intrinsics), _ptr(I.rt_cam_ref), _ptr(I.rt_ref_frame),
-                                             _ptr(I.points),
-                                             _ptr(I.calobject_warp) if I.calobject_warp is not None else None,
-                                             _ptr(I.observations_board), _ptr(I.observations_point)):
-            raise RuntimeError(_capi.last_error())
+        checked.mrcal_b200_problem_upload(self._h, _ptr(I.intrinsics), _ptr(I.rt_cam_ref), _ptr(I.rt_ref_frame),
+                                          _ptr(I.points), _ptr(I.calobject_warp), _ptr(I.observations_board),
+                                          _ptr(I.observations_point))
 
     def drt_cross_reprojection__dbpacked(self, icam_intrinsics=-1):
         """K (6, Nstate) at the problem's current state: see the module-level function."""
         K = np.zeros((6, self.Nstate))
-        if not lib.mrcal_b200_problem_drt_cross_reprojection__dbpacked(self._h, int(icam_intrinsics), _ptr(K)):
-            raise RuntimeError("_mrcal_drt_cross_reprojection__dbpacked() failed: " + _capi.last_error())
+        checked.mrcal_b200_problem_drt_cross_reprojection__dbpacked(self._h, int(icam_intrinsics), _ptr(K))
         return K
 
     def projection_uncertainty(self, p_cam, icam_intrinsics, method="cross-reprojection-ccp", atinfinity=False,
@@ -835,10 +795,9 @@ class Problem:
         s = -1.0 if observed_pixel_uncertainty is None else float(observed_pixel_uncertainty)
         if observed_pixel_uncertainty is not None and not s > 0:
             raise RuntimeError("observed_pixel_uncertainty must be > 0 (or None to estimate it)")
-        if not lib.mrcal_b200_problem_projection_uncertainty(self._h, int(icam_intrinsics), _UNCERTAINTY_METHODS[method],
-                                                            bool(atinfinity), _ptr(p), p.shape[0], s, _ptr(Var),
-                                                            C.byref(sigma)):
-            raise RuntimeError("projection_uncertainty: " + _capi.last_error())
+        checked.mrcal_b200_problem_projection_uncertainty(self._h, int(icam_intrinsics), _UNCERTAINTY_METHODS[method],
+                                                         bool(atinfinity), _ptr(p), p.shape[0], s, _ptr(Var),
+                                                         C.byref(sigma))
         return Var, sigma.value
 
     def projection_uncertainty_cameras(self, p_cams, icams_intrinsics, method="cross-reprojection-ccp", atinfinity=False,
@@ -862,10 +821,9 @@ class Problem:
         s = -1.0 if observed_pixel_uncertainty is None else float(observed_pixel_uncertainty)
         if observed_pixel_uncertainty is not None and not s > 0:
             raise RuntimeError("observed_pixel_uncertainty must be > 0 (or None to estimate it)")
-        if not lib.mrcal_b200_problem_projection_uncertainty_cameras(self._h, _ptr(icams), _ptr(N), len(ps),
-                                                                    _UNCERTAINTY_METHODS[method], bool(atinfinity),
-                                                                    _ptr(p_all), s, _ptr(Var), C.byref(sigma)):
-            raise RuntimeError("projection_uncertainty: " + _capi.last_error())
+        checked.mrcal_b200_problem_projection_uncertainty_cameras(self._h, _ptr(icams), _ptr(N), len(ps),
+                                                                 _UNCERTAINTY_METHODS[method], bool(atinfinity),
+                                                                 _ptr(p_all), s, _ptr(Var), C.byref(sigma))
         return np.split(Var, np.cumsum(N)[:-1]), sigma.value
 
     def regional_statistics(self, icams_intrinsics, q_cell_center, rcell, evaluate=True):
@@ -881,9 +839,8 @@ class Problem:
                                f"{q.shape} and {r.shape} for {icams.size} cameras")
         stats = np.zeros(q.shape[:-1] + (3,))
         x = np.zeros(self.Nmeasurements)
-        if not lib.mrcal_b200_problem_regional_statistics(self._h, _ptr(icams), icams.size, q.shape[2], q.shape[1],
-                                                          _ptr(q), _ptr(r), bool(evaluate), _ptr(stats), _ptr(x)):
-            raise RuntimeError("regional_statistics: " + _capi.last_error())
+        checked.mrcal_b200_problem_regional_statistics(self._h, _ptr(icams), icams.size, q.shape[2], q.shape[1],
+                                                       _ptr(q), _ptr(r), bool(evaluate), _ptr(stats), _ptr(x))
         return stats, x
 
     def callback(self, jacobian=True):
@@ -893,26 +850,23 @@ class Problem:
             P = np.zeros(self.Nmeasurements + 1, np.int32)
             Ii = np.zeros(self.N_j_nonzero, np.int32)
             X = np.zeros(self.N_j_nonzero)
-            ok = lib.mrcal_b200_problem_callback(self._h, _ptr(b), _ptr(x), _ptr(P), _ptr(Ii), _ptr(X))
+            checked.mrcal_b200_problem_callback(self._h, _ptr(b), _ptr(x), _ptr(P), _ptr(Ii), _ptr(X))
         else:
-            ok = lib.mrcal_b200_problem_callback(self._h, _ptr(b), _ptr(x), None, None, None)
-        if not ok:
-            raise RuntimeError(_capi.last_error())
+            checked.mrcal_b200_problem_callback(self._h, _ptr(b), _ptr(x), None, None, None)
         if not jacobian:
             return b, x, None
         return b, x, scipy.sparse.csr_matrix((X, Ii, P), shape=(self.Nmeasurements, self.Nstate))
 
     def optimize(self, **parameters):
         p = _capi.SolverParameters()
-        lib.mrcal_b200_default_solver_parameters(C.byref(p))
+        checked.mrcal_b200_default_solver_parameters(C.byref(p))
         for k, v in parameters.items():
             if not hasattr(p, k):
                 raise RuntimeError(f"unknown solver parameter '{k}'")
             setattr(p, k, v)
         stats = _capi.Stats()
         info = _capi.SolveInfo()
-        if not lib.mrcal_b200_problem_optimize(self._h, C.byref(p), C.byref(stats), C.byref(info)):
-            raise RuntimeError("mrcal_b200_problem_optimize() failed: " + _capi.last_error())
+        checked.mrcal_b200_problem_optimize(self._h, C.byref(p), C.byref(stats), C.byref(info))
         out = dict(rms_reproj_error__pixels=stats.rms_reproj_error__pixels,
                    Noutliers_board=stats.Noutliers_board,
                    Noutliers_triangulated_point=stats.Noutliers_triangulated_point)
@@ -929,10 +883,8 @@ class Problem:
         if not into_inputs:
             tgt = tuple(None if a is None else a.copy() for a in tgt)
         intr, rtc, rtf, pts, warp, obs = tgt
-        ok = lib.mrcal_b200_problem_download(self._h, _ptr(b), _ptr(x), _ptr(intr), _ptr(rtc), _ptr(rtf), _ptr(pts),
-                                             _ptr(warp) if warp is not None else None, _ptr(obs))
-        if not ok:
-            raise RuntimeError(_capi.last_error())
+        checked.mrcal_b200_problem_download(self._h, _ptr(b), _ptr(x), _ptr(intr), _ptr(rtc), _ptr(rtf), _ptr(pts),
+                                            _ptr(warp), _ptr(obs))
         return dict(b_packed=b, x=x, intrinsics=intr, rt_cam_ref=rtc, rt_ref_frame=rtf, points=pts,
                     calobject_warp=warp, observations_board=obs)
 
@@ -940,20 +892,18 @@ class Problem:
         """(S, g_reduced, g_full): the Schur-reduced normal equations at the current state (introspection).
         fused: the board observations' blocks come from the fused evaluation that optimize() uses for splined models
         with the core locked, not from the stored Jacobian (RuntimeError if this problem does not take that path)."""
-        fn = lib.mrcal_b200_problem_reduced_system_fused if fused else lib.mrcal_b200_problem_reduced_system
+        fn = checked.mrcal_b200_problem_reduced_system_fused if fused else checked.mrcal_b200_problem_reduced_system
         n = C.c_int(0)
-        if not fn(self._h, C.c_double(lambda_), C.byref(n), None, None, None):
-            raise RuntimeError(_capi.last_error())
+        fn(self._h, lambda_, C.byref(n), None, None, None)
         S = np.zeros((n.value, n.value))
         g = np.zeros(n.value)
         gf = np.zeros(self.Nstate)
-        if not fn(self._h, C.c_double(lambda_), C.byref(n), _ptr(S), _ptr(g), _ptr(gf)):
-            raise RuntimeError(_capi.last_error())
+        fn(self._h, lambda_, C.byref(n), _ptr(S), _ptr(g), _ptr(gf))
         S = np.tril(S) + np.tril(S, -1).T
         return S, g, gf
 
     def time_callback(self, N=10, jacobian=True):
-        ms = lib.mrcal_b200_problem_time_callback(self._h, int(N), C.c_bool(jacobian))
+        ms = checked.mrcal_b200_problem_time_callback(self._h, int(N), jacobian)
         if ms < 0:
             raise RuntimeError(_capi.last_error())
         return ms
@@ -974,11 +924,8 @@ class CHOLMOD_factorization:
         Ii = np.ascontiguousarray(J.indices, np.int32)
         X = np.ascontiguousarray(J.data, np.float64)
         self.shape = J.shape
-        self._h = lib.mrcal_b200_factorization_create(_ptr(P) or P.ctypes.data_as(C.c_void_p), _ptr(Ii), _ptr(X),
-                                                      J.shape[0], J.shape[1])
-        if not self._h:
-            raise RuntimeError("CHOLMOD_factorization: " + _capi.last_error())
-        self._h = C.c_void_p(self._h)
+        self._h = C.c_void_p(checked.mrcal_b200_factorization_create(_ptr(P) or P.ctypes.data_as(C.c_void_p), _ptr(Ii),
+                                                                     _ptr(X), J.shape[0], J.shape[1]))
 
     @classmethod
     def _from_handle(cls, h, shape):
@@ -989,7 +936,7 @@ class CHOLMOD_factorization:
 
     def __del__(self):
         if getattr(self, "_h", None):
-            lib.mrcal_b200_factorization_destroy(self._h)
+            checked.mrcal_b200_factorization_destroy(self._h)
             self._h = None
 
     _SYS = ("A", "LDLt", "LD", "DLt", "L", "Lt", "D", "P", "Pt")   # mrcal-pywrap.c:467-476; codes of mrcal_b200.h
@@ -1008,12 +955,11 @@ class CHOLMOD_factorization:
         flat = np.ascontiguousarray(bt.reshape(-1, self.shape[1]))
         out = np.empty_like(flat)
         if flat.shape[0]:
-            if not lib.mrcal_b200_factorization_solve_sys(self._h, _ptr(out), _ptr(flat), flat.shape[0], code):
-                raise RuntimeError("solve_xt_JtJ_bt: " + _capi.last_error())
+            checked.mrcal_b200_factorization_solve_sys(self._h, _ptr(out), _ptr(flat), flat.shape[0], code)
         return out.reshape(bt.shape)
 
     def rcond(self):
-        return lib.mrcal_b200_factorization_rcond(self._h)
+        return checked.mrcal_b200_factorization_rcond(self._h)
 
 
 ####################################################################################################
@@ -1027,14 +973,12 @@ class _DeviceCSR:
     def __init__(self, Jp, Ji, Jx, Ncols):
         self.key = (Jp.ctypes.data, Ji.ctypes.data, Jx.ctypes.data, Jp.size, Ji.size, Ncols)
         self.Nrows, self.Ncols = Jp.size - 1, Ncols
-        h = lib.mrcal_b200_csr_create(_ptr(Jp) or Jp.ctypes.data_as(C.c_void_p), _ptr(Ji), _ptr(Jx), self.Nrows, Ncols)
-        if not h:
-            raise RuntimeError(_capi.last_error())
-        self._h = C.c_void_p(h)
+        self._h = C.c_void_p(checked.mrcal_b200_csr_create(_ptr(Jp) or Jp.ctypes.data_as(C.c_void_p), _ptr(Ji),
+                                                           _ptr(Jx), self.Nrows, Ncols))
 
     def __del__(self):
         if getattr(self, "_h", None):
-            lib.mrcal_b200_csr_destroy(self._h)
+            checked.mrcal_b200_csr_destroy(self._h)
             self._h = None
 
     @classmethod
@@ -1061,8 +1005,7 @@ def _Jt_x(Jp, Ji, Jx, xt, out=None):
     if out.dtype != np.float64 or not out.flags.c_contiguous or out.ndim != 1:
         raise RuntimeError("out must be a contiguous 1-dimensional float64 array")
     J = _DeviceCSR.get(Jp, Ji, Jx, out.shape[0])
-    if not lib.mrcal_b200_csr_Jt_x(J._h, _ptr(out), _ptr(xt)):
-        raise RuntimeError(_capi.last_error())
+    checked.mrcal_b200_csr_Jt_x(J._h, _ptr(out), _ptr(xt))
     return out
 
 
@@ -1079,8 +1022,7 @@ def _A_Jt_J_At(A, Jp, Ji, Jx, Nleading_rows_J=-1, out=None):
     flat = np.ascontiguousarray(A.reshape(-1, Nx, Nstate))
     res = np.zeros((flat.shape[0], Nx, Nx))
     for k in range(flat.shape[0]):
-        if not lib.mrcal_b200_csr_A_Jt_J_At(J._h, _ptr(res[k]), _ptr(flat[k]), Nx, int(Nleading_rows_J)):
-            raise RuntimeError(_capi.last_error())
+        checked.mrcal_b200_csr_A_Jt_J_At(J._h, _ptr(res[k]), _ptr(flat[k]), Nx, int(Nleading_rows_J))
     res = res.reshape(A.shape[:-2] + (Nx, Nx))
     if out is not None:
         out[...] = res
@@ -1099,11 +1041,11 @@ def _A_Jt_J_At__2(A, Jp, Ji, Jx, Nleading_rows_J=-1, out=None):
 # lens models
 ####################################################################################################
 def lensmodel_num_params(lensmodel):
-    return lib.mrcal_lensmodel_num_params(C.byref(_lensmodel(lensmodel)))
+    return checked.mrcal_lensmodel_num_params(C.byref(_lensmodel(lensmodel)))
 
 
 def supported_lensmodels():
-    names = lib.mrcal_supported_lensmodel_names()
+    names = checked.mrcal_supported_lensmodel_names()
     out, i = [], 0
     while names[i]:
         out.append(names[i].decode())
@@ -1113,7 +1055,7 @@ def supported_lensmodels():
 
 def lensmodel_metadata_and_config(lensmodel):
     lm = _lensmodel(lensmodel)
-    m = lib.mrcal_lensmodel_metadata(C.byref(lm)).bits
+    m = checked.mrcal_lensmodel_metadata(C.byref(lm)).bits
     out = dict(has_core=(m >> 0) & 1, can_project_behind_camera=(m >> 1) & 1,
                has_gradients=(m >> 2) & 1, noncentral=(m >> 3) & 1)
     if lm.type == 10:
@@ -1131,8 +1073,7 @@ def knots_for_splined_models(lensmodel):
                            f"'{lensmodel}' passed in")
     cfg = np.frombuffer(bytes(lm.config), np.uint16)
     ux, uy = np.zeros(int(cfg[1])), np.zeros(int(cfg[2]))
-    if not lib.mrcal_knots_for_splined_models(_ptr(ux), _ptr(uy), C.byref(lm)):
-        raise RuntimeError(_capi.last_error())
+    checked.mrcal_knots_for_splined_models(_ptr(ux), _ptr(uy), C.byref(lm))
     return ux, uy
 
 
@@ -1154,52 +1095,54 @@ def _none_if_negative(i):
 
 def state_index_intrinsics(icam_intrinsics, **kwargs):
     I = _layout_inputs(kwargs)
-    return _none_if_negative(lib.mrcal_state_index_intrinsics(int(icam_intrinsics), *I.counts(), I.selections, I.lm_ref()))
+    return _none_if_negative(checked.mrcal_state_index_intrinsics(int(icam_intrinsics), *I.counts(), I.selections,
+                                                                  I.lm_ref()))
 
 
 def state_index_extrinsics(icam_extrinsics, **kwargs):
     I = _layout_inputs(kwargs)
-    return _none_if_negative(lib.mrcal_state_index_extrinsics(int(icam_extrinsics), *I.counts(), I.selections, I.lm_ref()))
+    return _none_if_negative(checked.mrcal_state_index_extrinsics(int(icam_extrinsics), *I.counts(), I.selections,
+                                                                  I.lm_ref()))
 
 
 def state_index_frames(iframe, **kwargs):
     I = _layout_inputs(kwargs)
-    return _none_if_negative(lib.mrcal_state_index_frames(int(iframe), *I.counts(), I.selections, I.lm_ref()))
+    return _none_if_negative(checked.mrcal_state_index_frames(int(iframe), *I.counts(), I.selections, I.lm_ref()))
 
 
 def state_index_points(i_point, **kwargs):
     I = _layout_inputs(kwargs)
-    return _none_if_negative(lib.mrcal_state_index_points(int(i_point), *I.counts(), I.selections, I.lm_ref()))
+    return _none_if_negative(checked.mrcal_state_index_points(int(i_point), *I.counts(), I.selections, I.lm_ref()))
 
 
 def state_index_calobject_warp(**kwargs):
     I = _layout_inputs(kwargs)
-    return _none_if_negative(lib.mrcal_state_index_calobject_warp(*I.counts(), I.selections, I.lm_ref()))
+    return _none_if_negative(checked.mrcal_state_index_calobject_warp(*I.counts(), I.selections, I.lm_ref()))
 
 
 def num_states_intrinsics(**kwargs):
     I = _layout_inputs(kwargs)
-    return lib.mrcal_num_states_intrinsics(I.Ncam_i, I.selections, I.lm_ref())
+    return checked.mrcal_num_states_intrinsics(I.Ncam_i, I.selections, I.lm_ref())
 
 
 def num_states_extrinsics(**kwargs):
     I = _layout_inputs(kwargs)
-    return lib.mrcal_num_states_extrinsics(I.Ncam_e, I.selections)
+    return checked.mrcal_num_states_extrinsics(I.Ncam_e, I.selections)
 
 
 def num_states_frames(**kwargs):
     I = _layout_inputs(kwargs)
-    return lib.mrcal_num_states_frames(I.Nframes, I.selections)
+    return checked.mrcal_num_states_frames(I.Nframes, I.selections)
 
 
 def num_states_points(**kwargs):
     I = _layout_inputs(kwargs)
-    return lib.mrcal_num_states_points(I.Npoints, I.Npoints_fixed, I.selections)
+    return checked.mrcal_num_states_points(I.Npoints, I.Npoints_fixed, I.selections)
 
 
 def num_states_calobject_warp(**kwargs):
     I = _layout_inputs(kwargs)
-    return lib.mrcal_num_states_calobject_warp(I.selections, I.Nobs_board)
+    return checked.mrcal_num_states_calobject_warp(I.selections, I.Nobs_board)
 
 
 def num_states(**kwargs):
@@ -1208,29 +1151,29 @@ def num_states(**kwargs):
 
 def num_intrinsics_optimization_params(**kwargs):
     I = _layout_inputs(kwargs)
-    return lib.mrcal_num_intrinsics_optimization_params(I.selections, I.lm_ref())
+    return checked.mrcal_num_intrinsics_optimization_params(I.selections, I.lm_ref())
 
 
 def measurement_index_boards(i_observation_board, **kwargs):
     I = _layout_inputs(kwargs)
-    return _none_if_negative(lib.mrcal_measurement_index_boards(int(i_observation_board), I.Nobs_board, I.Nobs_point,
-                                                                I.W, I.H))
+    return _none_if_negative(checked.mrcal_measurement_index_boards(int(i_observation_board), I.Nobs_board,
+                                                                    I.Nobs_point, I.W, I.H))
 
 
 def num_measurements_boards(**kwargs):
     I = _layout_inputs(kwargs)
-    return lib.mrcal_num_measurements_boards(I.Nobs_board, I.W, I.H)
+    return checked.mrcal_num_measurements_boards(I.Nobs_board, I.W, I.H)
 
 
 def measurement_index_points(i_observation_point, **kwargs):
     I = _layout_inputs(kwargs)
-    return _none_if_negative(lib.mrcal_measurement_index_points(int(i_observation_point), I.Nobs_board, I.Nobs_point,
-                                                                I.W, I.H))
+    return _none_if_negative(checked.mrcal_measurement_index_points(int(i_observation_point), I.Nobs_board,
+                                                                    I.Nobs_point, I.W, I.H))
 
 
 def num_measurements_points(**kwargs):
     I = _layout_inputs(kwargs)
-    return lib.mrcal_num_measurements_points(I.Nobs_point)
+    return checked.mrcal_num_measurements_points(I.Nobs_point)
 
 
 def measurement_index_points_triangulated(i_point_triangulated, **kwargs):
@@ -1238,27 +1181,27 @@ def measurement_index_points_triangulated(i_point_triangulated, **kwargs):
     tri, ntri = I.c_triangulated()
     if ntri == 0:
         return None
-    return _none_if_negative(lib.mrcal_measurement_index_points_triangulated(
-        int(i_point_triangulated), I.Nobs_board, I.Nobs_point, tri, ntri, max(I.W, 0), max(I.H, 0)))
+    return _none_if_negative(checked.mrcal_measurement_index_points_triangulated(
+            int(i_point_triangulated), I.Nobs_board, I.Nobs_point, tri, ntri, max(I.W, 0), max(I.H, 0)))
 
 
 def num_measurements_points_triangulated(**kwargs):
     I = _layout_inputs(kwargs)
     tri, ntri = I.c_triangulated()
-    return lib.mrcal_num_measurements_points_triangulated(tri, ntri)
+    return checked.mrcal_num_measurements_points_triangulated(tri, ntri)
 
 
 def measurement_index_regularization(**kwargs):
     I = _layout_inputs(kwargs)
     tri, ntri = I.c_triangulated()
-    return _none_if_negative(lib.mrcal_measurement_index_regularization(
-        tri, ntri, I.W, I.H, I.Ncam_i, I.Ncam_e, I.Nframes, I.Npoints, I.Npoints_fixed, I.Nobs_board, I.Nobs_point,
-        I.selections, I.lm_ref()))
+    return _none_if_negative(checked.mrcal_measurement_index_regularization(
+            tri, ntri, I.W, I.H, I.Ncam_i, I.Ncam_e, I.Nframes, I.Npoints, I.Npoints_fixed, I.Nobs_board, I.Nobs_point,
+            I.selections, I.lm_ref()))
 
 
 def num_measurements_regularization(**kwargs):
     I = _layout_inputs(kwargs)
-    return lib.mrcal_num_measurements_regularization(*I.counts(), I.selections, I.lm_ref())
+    return checked.mrcal_num_measurements_regularization(*I.counts(), I.selections, I.lm_ref())
 
 
 def num_measurements(**kwargs):
@@ -1269,9 +1212,8 @@ def corresponding_icam_extrinsics(icam_intrinsics, **kwargs):
     I = _layout_inputs(kwargs)
     ob, op = I.c_observations()
     out = C.c_int(-100)
-    if not lib.mrcal_corresponding_icam_extrinsics(C.byref(out), int(icam_intrinsics), I.Ncam_i, I.Ncam_e,
-                                                   ob.shape[0], _ptr(ob), op.shape[0], _ptr(op)):
-        raise RuntimeError("Error calling mrcal_corresponding_icam_extrinsics(): " + _capi.last_error())
+    checked.mrcal_corresponding_icam_extrinsics(C.byref(out), int(icam_intrinsics), I.Ncam_i, I.Ncam_e, ob.shape[0],
+                                                _ptr(ob), op.shape[0], _ptr(op))
     return out.value
 
 
@@ -1286,10 +1228,10 @@ def _pack_unpack(b, pack, kwargs):
     if b.shape[-1] != Nstate:
         raise RuntimeError(f"The given array MUST have last dimension of size Nstate={Nstate}; "
                            f"instead got {b.shape[-1]}")
-    f = lib.mrcal_pack_solver_state_vector if pack else lib.mrcal_unpack_solver_state_vector
+    f = checked.mrcal_pack_solver_state_vector if pack else checked.mrcal_unpack_solver_state_vector
     flat = b.reshape(-1, Nstate)
     for i in range(flat.shape[0]):
-        f(C.c_void_p(flat[i].ctypes.data), *I.counts(), I.selections, I.lm_ref())
+        f(flat[i].ctypes.data, *I.counts(), I.selections, I.lm_ref())
     return None
 
 
@@ -1311,15 +1253,14 @@ def project(v, lensmodel, intrinsics_data, get_gradients=False):
         raise RuntimeError("project(): the last dimension of v must be 3")
     lm = _lensmodel(lensmodel)
     intr = np.ascontiguousarray(intrinsics_data, dtype=np.float64)
-    if intr.shape != (lib.mrcal_lensmodel_num_params(C.byref(lm)),):
-        raise RuntimeError(f"project(): intrinsics_data must have shape ({lib.mrcal_lensmodel_num_params(C.byref(lm))},)")
+    Nintr = checked.mrcal_lensmodel_num_params(C.byref(lm))
+    if intr.shape != (Nintr,):
+        raise RuntimeError(f"project(): intrinsics_data must have shape ({Nintr},)")
     flat = v.reshape(-1, 3)
     q = np.zeros((flat.shape[0], 2))
     g = np.zeros((flat.shape[0], 2, 3)) if get_gradients else None
     gi = np.zeros((flat.shape[0], 2, intr.shape[0])) if get_gradients else None
-    if not lib.mrcal_project(_ptr(q), _ptr(g) if g is not None else None, _ptr(gi) if gi is not None else None,
-                             _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr)):
-        raise RuntimeError("mrcal_project() failed: " + _capi.last_error())
+    checked.mrcal_project(_ptr(q), _ptr(g), _ptr(gi), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr))
     q = q.reshape(v.shape[:-1] + (2,))
     if not get_gradients:
         return q
@@ -1342,17 +1283,15 @@ def unproject(q, lensmodel, intrinsics_data, *, normalize=False, get_gradients=F
     flat = q.reshape(-1, 2)
     v = np.zeros((flat.shape[0], 3))
     if not normalize and not get_gradients:
-        if not lib.mrcal_unproject(_ptr(v), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr)):
-            raise RuntimeError("mrcal_unproject() failed: " + _capi.last_error())
+        checked.mrcal_unproject(_ptr(v), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr))
         return v.reshape(q.shape[:-1] + (3,))
-    Nintr = lib.mrcal_lensmodel_num_params(C.byref(lm))
+    Nintr = checked.mrcal_lensmodel_num_params(C.byref(lm))
     if intr.shape != (Nintr,):
         raise RuntimeError(f"unproject(): intrinsics_data must have shape ({Nintr},)")
     g = np.zeros((flat.shape[0], 3, 2)) if get_gradients else None
     gi = np.zeros((flat.shape[0], 3, Nintr)) if get_gradients else None
-    if not lib.mrcal_b200_unproject_with_gradients(_ptr(v), _ptr(g), _ptr(gi), _ptr(flat), flat.shape[0], C.byref(lm),
-                                                   _ptr(intr), bool(normalize)):
-        raise RuntimeError("unproject() failed: " + _capi.last_error())
+    checked.mrcal_b200_unproject_with_gradients(_ptr(v), _ptr(g), _ptr(gi), _ptr(flat), flat.shape[0], C.byref(lm),
+                                                _ptr(intr), bool(normalize))
     v = v.reshape(q.shape[:-1] + (3,))
     if not get_gradients:
         return v

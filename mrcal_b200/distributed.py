@@ -22,8 +22,7 @@ import os
 
 import numpy as np
 
-from . import _capi
-from ._capi import lib
+from ._capi import checked
 
 
 def _frame_ranges(Nframes, world):
@@ -121,19 +120,17 @@ def init_comm(rank, world, local_rank):
             os.environ["MRCAL_B200_NCCL_LIB"] = p
     buf = (C.c_char * 128)()
     if rank == 0:
-        if not lib.mrcal_b200_nccl_get_unique_id(buf):
-            raise RuntimeError(_capi.last_error())
+        checked.mrcal_b200_nccl_get_unique_id(buf)
     dev = torch.device("cuda", local_rank) if dist.get_backend() == "nccl" else torch.device("cpu")
     t = torch.frombuffer(bytearray(bytes(buf)), dtype=torch.uint8).clone().to(dev)
     dist.broadcast(t, src=0)
     raw = bytes(t.cpu().numpy().tobytes())
-    if not lib.mrcal_b200_nccl_comm_init(raw, rank, world, local_rank):
-        raise RuntimeError(_capi.last_error())
+    checked.mrcal_b200_nccl_comm_init(raw, rank, world, local_rank)
 
 
 def attach(problem, shard):
-    if not lib.mrcal_b200_problem_set_sharding(problem._h, shard["f0"], shard["Nframes"], shard["p0"], shard.get("Npoints", 0)):
-        raise RuntimeError(_capi.last_error())
+    checked.mrcal_b200_problem_set_sharding(problem._h, shard["f0"], shard["Nframes"], shard["p0"],
+                                            shard.get("Npoints", 0))
 
 
 def gather_solution(problem, shard):

@@ -18,8 +18,7 @@ import sys
 
 import numpy as np
 
-from . import _capi
-from ._capi import lib
+from ._capi import checked
 from ._poses_host import compose_Rt
 from .api import _lensmodel, _ptr, _require_gpu, lensmodel_metadata_and_config, unproject
 from .cameramodel import cameramodel
@@ -32,10 +31,6 @@ BORDER_TRANSPARENT = 5
 _FITS = ("corners", "centers-horizontal", "centers-vertical")
 # element type codes of include/mrcal_b200.h (MRCAL_B200_IMAGE_*)
 _NUMPY_TYPES = {np.dtype(np.uint8): 0, np.dtype(np.uint16): 1, np.dtype(np.float32): 2}
-
-
-def _fail(what):
-    raise RuntimeError(f"{what} failed: {_capi.last_error()}")
 
 
 def _require_core(lensmodel):
@@ -154,12 +149,11 @@ def image_transformation_map(model_from, model_to, *, intrinsics_only=False, dis
 
     W, H = (int(x) for x in model_to.imagersize())
     mapxy = np.empty((H, W, 2), dtype=np.float32)
-    if not lib.mrcal_b200_image_transformation_map(
-            _ptr(mapxy), W, H, C.byref(lm_from), _ptr(np.ascontiguousarray(intrinsics_from, np.float64)),
-            C.byref(lm_to), _ptr(np.ascontiguousarray(intrinsics_to, np.float64)), _ptr(Rt_to_from), _ptr(d),
-            _ptr(plane_n), 0. if plane_d is None else float(plane_d), _ptr(region),
-            0 if region is None else region.shape[0]):
-        _fail("mrcal_b200_image_transformation_map()")
+    checked.mrcal_b200_image_transformation_map(_ptr(mapxy), W, H, C.byref(lm_from),
+                                                _ptr(np.ascontiguousarray(intrinsics_from, np.float64)), C.byref(lm_to),
+                                                _ptr(np.ascontiguousarray(intrinsics_to, np.float64)), _ptr(Rt_to_from),
+                                                _ptr(d), _ptr(plane_n), 0. if plane_d is None else float(plane_d),
+                                                _ptr(region), 0 if region is None else region.shape[0])
     return mapxy
 
 
@@ -243,10 +237,9 @@ def transform_image(image, mapxy, *, out=None, borderMode=None, borderValue=0, i
         image = np.ascontiguousarray(image)
     mapxy = np.ascontiguousarray(mapxy)
     _require_gpu()
-    if not lib.mrcal_b200_transform_image(out.ctypes.data, image.ctypes.data, W, H, image.strides[0],
-                                          _NUMPY_TYPES[image.dtype], channels, _ptr(mapxy), Wo, Ho, interpolation,
-                                          borderMode, _ptr(bv)):
-        _fail("mrcal_b200_transform_image()")
+    checked.mrcal_b200_transform_image(out.ctypes.data, image.ctypes.data, W, H, image.strides[0],
+                                       _NUMPY_TYPES[image.dtype], channels, _ptr(mapxy), Wo, Ho, interpolation,
+                                       borderMode, _ptr(bv))
     return out
 
 
@@ -275,9 +268,7 @@ def _transform_image_device(torch, image, mapxy, out, borderMode, bv, interpolat
     # the launch goes to the tensors' device, whichever device is current
     with torch.cuda.device(image.device):
         stream = torch.cuda.current_stream(image.device).cuda_stream
-        if not lib.mrcal_b200_transform_image_device(out.data_ptr(), image.data_ptr(), W, H,
-                                                     W * channels * image.element_size(), types[image.dtype], channels,
-                                                     mapxy.data_ptr(), Wo, Ho, interpolation, borderMode, _ptr(bv),
-                                                     stream):
-            _fail("mrcal_b200_transform_image_device()")
+        checked.mrcal_b200_transform_image_device(out.data_ptr(), image.data_ptr(), W, H,
+                                                  W * channels * image.element_size(), types[image.dtype], channels,
+                                                  mapxy.data_ptr(), Wo, Ho, interpolation, borderMode, _ptr(bv), stream)
     return out

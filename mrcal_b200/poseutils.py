@@ -12,13 +12,11 @@ torch.cuda.current_stream() without waiting for it. Leading dimensions broadcast
 broadcast is read in place, never expanded. out= writes the results into the given array(s) (a tuple with gradients)
 and returns them. identity_*() are host-only.
 """
-import ctypes as C
 from functools import reduce
 
 import numpy as np
 
-from . import _capi
-from ._capi import lib
+from ._capi import checked
 from .api import _ptr, _require_gpu
 from .image_transforms import _torch_if_tensors
 
@@ -118,13 +116,11 @@ def _pose(fname, args, protos_in, protos_out, out, get_gradients=False, inverted
         call = (_ptr(shape), ins[0], _ptr(st[0]), ins[1], _ptr(st[1]), *o)
         if torch is None:
             _require_gpu()
-            if not lib.mrcal_b200_poseutils(_OPS[fname], flags, len(lead), *call):
-                raise RuntimeError(f"{fname}() failed: {_capi.last_error()}")
+            checked.mrcal_b200_poseutils(_OPS[fname], flags, len(lead), *call)
         else:
             with torch.cuda.device(device):
                 stream = torch.cuda.current_stream(device).cuda_stream
-                if not lib.mrcal_b200_poseutils_device(_OPS[fname], flags, len(lead), *call, C.c_void_p(stream)):
-                    raise RuntimeError(f"{fname}() failed: {_capi.last_error()}")
+                checked.mrcal_b200_poseutils_device(_OPS[fname], flags, len(lead), *call, stream)
     if outs is not None:
         for k in range(len(res)):
             if not direct[k]:

@@ -7,14 +7,13 @@ cell, the projection uncertainty of every camera's grid from one factorization o
 point-in-region test. What stays here is a few hundred cells of host arithmetic: the thresholds, the mask, and the
 mask's outer contour, which is cv2.findContours(RETR_EXTERNAL, CHAIN_APPROX_SIMPLE) restated so that the package
 needs no OpenCV at run time."""
-import ctypes as C
 import re
 import sys
 
 import numpy as np
 
-from . import _capi, api
-from ._capi import lib
+from . import api
+from ._capi import checked
 from .api import _ptr, _require_gpu
 
 
@@ -383,7 +382,6 @@ def is_within_valid_intrinsics_region(q, model):
         raise RuntimeError(f"q must have shape (...,2); got {q.shape}")
     r = np.ascontiguousarray(r, np.float64).reshape(-1, 2)
     mask = np.zeros(q.shape[:-1], dtype=bool)
-    if mask.size and not lib.mrcal_b200_is_within_region(mask.ctypes.data_as(C.c_void_p), _ptr(q), mask.size, _ptr(r),
-                                                         r.shape[0]):
-        raise RuntimeError("is_within_valid_intrinsics_region: " + _capi.last_error())
+    if mask.size:
+        checked.mrcal_b200_is_within_region(mask.ctypes.data, _ptr(q), mask.size, _ptr(r), r.shape[0])
     return mask

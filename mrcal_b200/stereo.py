@@ -23,11 +23,10 @@ import sys
 import numpy as np
 
 from . import _capi
-from ._capi import lib
+from ._capi import checked
 from ._poses_host import compose_Rt
 from .api import _lensmodel, _ptr, _require_gpu, lensmodel_metadata_and_config
 from .cameramodel import cameramodel
-from .image_transforms import _fail
 
 # the reference's Python wrapper takes an az0_deg above this for "autodetect" (mrcal-pywrap.c:4029-4030)
 _AZ0_AUTODETECT = 1e7
@@ -58,9 +57,8 @@ def rectified_resolution(model0, *, az_fov_deg, el_fov_deg, az0_deg, el0_deg, R_
     az, el = C.c_double(pixels_per_deg_az), C.c_double(pixels_per_deg_el)
     azel_fov = (C.c_double * 2)(az_fov_deg, el_fov_deg)
     azel0 = (C.c_double * 2)(az0_deg, el0_deg)
-    if not lib.mrcal_rectified_resolution(C.byref(az), C.byref(el), C.byref(lm), _ptr(intr), azel_fov, azel0, _ptr(R),
-                                          _rectification_model_type(rectification_model)):
-        _fail("mrcal_rectified_resolution()")
+    checked.mrcal_rectified_resolution(C.byref(az), C.byref(el), C.byref(lm), _ptr(intr), azel_fov, azel0, _ptr(R),
+                                       _rectification_model_type(rectification_model))
     return az.value, el.value
 
 
@@ -98,11 +96,10 @@ def rectified_system(models, *, az_fov_deg, el_fov_deg, az0_deg=None, el0_deg=0,
     az, el = C.c_double(pixels_per_deg_az), C.c_double(pixels_per_deg_el)
     azel_fov = (C.c_double * 2)(az_fov_deg, el_fov_deg)
     azel0 = (C.c_double * 2)(az0_deg, el0_deg)
-    if not lib.mrcal_rectified_system2(imagersize, _ptr(fxycxy), _ptr(rt_rect0_ref), C.byref(baseline), C.byref(az),
-                                       C.byref(el), azel_fov, azel0, float(az_edge_margin_deg), C.byref(lm), _ptr(intr),
-                                       _ptr(rt0), _ptr(rt1), _rectification_model_type(rectification_model),
-                                       az0_deg > _AZ0_AUTODETECT / 10., False, False, False):
-        _fail("mrcal_rectified_system()")
+    checked.mrcal_rectified_system2(imagersize, _ptr(fxycxy), _ptr(rt_rect0_ref), C.byref(baseline), C.byref(az),
+                                    C.byref(el), azel_fov, azel0, float(az_edge_margin_deg), C.byref(lm), _ptr(intr),
+                                    _ptr(rt0), _ptr(rt1), _rectification_model_type(rectification_model),
+                                    az0_deg > _AZ0_AUTODETECT / 10., False, False, False)
     # rect1 has rect0's orientation, its origin at camera 1: rt_rect1_ref = (0,0,0, -baseline,0,0) rt_rect0_ref
     rt_rect1_ref = rt_rect0_ref.copy()
     rt_rect1_ref[3] -= baseline.value
@@ -155,10 +152,9 @@ def rectification_maps(models, models_rectified):
     fxycxy = np.ascontiguousarray(fxycxy, np.float64)
     r = [np.ascontiguousarray(m.rt_cam_ref()[:3]) for m in (models[0], models[1], models_rectified[0])]
     size = (C.c_uint * 2)(Naz, Nel)
-    if not lib.mrcal_rectification_maps(_ptr(maps), C.byref(lms[0]), _ptr(intr[0]), _ptr(r[0]),
-                                        C.byref(lms[1]), _ptr(intr[1]), _ptr(r[1]),
-                                        _rectification_model_type(rect), _ptr(fxycxy), size, _ptr(r[2])):
-        _fail("mrcal_rectification_maps()")
+    checked.mrcal_rectification_maps(_ptr(maps), C.byref(lms[0]), _ptr(intr[0]), _ptr(r[0]), C.byref(lms[1]),
+                                     _ptr(intr[1]), _ptr(r[1]), _rectification_model_type(rect), _ptr(fxycxy), size,
+                                     _ptr(r[2]))
     return maps
 
 
@@ -234,16 +230,14 @@ def stereo_range(disparity, models_rectified, *, disparity_scale=1, disparity_mi
         _require_gpu()
         r = np.zeros(d16.shape)
         out = _capi.ImageDouble(img.w, img.h, int(r.strides[0]), r.ctypes.data)
-        if not lib.mrcal_stereo_range_dense(C.byref(out), C.byref(img), int(scale), int(smin), int(smax), a["rect"],
-                                            _ptr(a["fxycxy"]), a["baseline"]):
-            _fail("mrcal_stereo_range_dense()")
+        checked.mrcal_stereo_range_dense(C.byref(out), C.byref(img), int(scale), int(smin), int(smax), a["rect"],
+                                         _ptr(a["fxycxy"]), a["baseline"])
     else:
         d, q, shape = _sparse_inputs(a["disparity"], qrect0, disparity_scale)
         _require_gpu()
         r = np.zeros(d.shape)
-        if not lib.mrcal_stereo_range_sparse(_ptr(r), _ptr(d), _ptr(q), d.size, float(a["dmin"]), float(a["dmax"]),
-                                             a["rect"], _ptr(a["fxycxy"]), a["baseline"]):
-            _fail("mrcal_stereo_range_sparse()")
+        checked.mrcal_stereo_range_sparse(_ptr(r), _ptr(d), _ptr(q), d.size, float(a["dmin"]), float(a["dmax"]),
+                                          a["rect"], _ptr(a["fxycxy"]), a["baseline"])
         r = r.reshape(shape)
     if a["is_scalar"]:
         r = r[0]
@@ -275,24 +269,21 @@ def stereo_unproject(disparity, models_rectified, *, ranges=None, disparity_scal
         else:
             rg, q, shape = _sparse_inputs(rg, qrect0, 1.)
         p = np.zeros((rg.size, 3))
-        if not lib.mrcal_b200_stereo_unproject(_ptr(p), None, None, 0, 0, 0, None, _ptr(rg), _ptr(q) if q is not None else None,
-                                               rg.size, W, 0., 0., rect, _ptr(fxycxy), baseline):
-            _fail("mrcal_b200_stereo_unproject()")
+        checked.mrcal_b200_stereo_unproject(_ptr(p), None, None, 0, 0, 0, None, _ptr(rg), _ptr(q), rg.size, W, 0., 0.,
+                                            rect, _ptr(fxycxy), baseline)
         return p.reshape(shape + (3,))
     a = _range_arguments(disparity, models_rectified, disparity_scale, None, None, None, None, qrect0)
     _require_gpu()
     if qrect0 is None:
         img, d16, (scale, smin, smax) = _dense_image(a, models_rectified, disparity_scale)
         p = np.zeros((H, W, 3))
-        if not lib.mrcal_b200_stereo_unproject(_ptr(p), None, C.byref(img), int(scale), int(smin), int(smax), None, None,
-                                               None, 0, 0, 0., 0., rect, _ptr(fxycxy), a["baseline"]):
-            _fail("mrcal_b200_stereo_unproject()")
+        checked.mrcal_b200_stereo_unproject(_ptr(p), None, C.byref(img), int(scale), int(smin), int(smax), None, None,
+                                            None, 0, 0, 0., 0., rect, _ptr(fxycxy), a["baseline"])
         return p
     d, q, shape = _sparse_inputs(a["disparity"], qrect0, disparity_scale)
     p = np.zeros((d.size, 3))
-    if not lib.mrcal_b200_stereo_unproject(_ptr(p), None, None, 0, 0, 0, _ptr(d), None, _ptr(q), d.size, 0,
-                                           float(a["dmin"]), float(a["dmax"]), rect, _ptr(fxycxy), a["baseline"]):
-        _fail("mrcal_b200_stereo_unproject()")
+    checked.mrcal_b200_stereo_unproject(_ptr(p), None, None, 0, 0, 0, _ptr(d), None, _ptr(q), d.size, 0,
+                                        float(a["dmin"]), float(a["dmax"]), rect, _ptr(fxycxy), a["baseline"])
     p = p.reshape(shape + (3,))
     if a["is_scalar"] and np.ndim(qrect0) == 1:
         p = p[0]
@@ -496,18 +487,16 @@ def _match_features(image0, image1, q0, search_radius1, template_size1, q1_estim
         if torch is None:
             image0, image1 = _packed_rows(image0), _packed_rows(image1)
             _require_gpu()
-            ok = lib.mrcal_b200_match_feature(buf.ctypes.data, _ptr(templates), image0.ctypes.data, W0, H0,
-                                              image0.strides[0], image1.ctypes.data, W1, H1, image1.strides[0],
-                                              type_code, *args)
+            checked.mrcal_b200_match_feature(buf.ctypes.data, _ptr(templates), image0.ctypes.data, W0, H0,
+                                             image0.strides[0], image1.ctypes.data, W1, H1, image1.strides[0],
+                                             type_code, *args)
         else:
             es = image0.element_size()
             with torch.cuda.device(image0.device):
                 stream = torch.cuda.current_stream(image0.device).cuda_stream
-                ok = lib.mrcal_b200_match_feature_device(buf.ctypes.data, _ptr(templates), image0.data_ptr(), W0, H0,
-                                                         W0 * es, image1.data_ptr(), W1, H1, W1 * es, type_code,
-                                                         *args, stream)
-        if not ok:
-            _fail("mrcal_b200_match_feature()")
+                checked.mrcal_b200_match_feature_device(buf.ctypes.data, _ptr(templates), image0.data_ptr(), W0, H0,
+                                                        W0 * es, image1.data_ptr(), W1, H1, W1 * es, type_code, *args,
+                                                        stream)
     res = buf[:4 * M].reshape(M, 4)
     slots = buf[4 * M:].view(np.float32)[:M * slot_w * slot_h].reshape(M, slot_w * slot_h)
 

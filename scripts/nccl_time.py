@@ -1,6 +1,5 @@
 #!/usr/bin/env python3
 """Device time of the library's all-reduce at the sizes the sharded solve uses. Run under torchrun."""
-import ctypes as C
 import os
 import sys
 sys.path.insert(0, ".")
@@ -12,8 +11,6 @@ dist.init_process_group("nccl", device_id=torch.device("cuda", local))
 from mrcal_b200 import _capi, distributed
 distributed.init_comm(rank, world, local)
 f = _capi.lib.mrcal_b200_debug_time_allreduce
-f.restype = C.c_double
-f.argtypes = [C.c_size_t, C.c_int]
 for count in (8, 4821, 231 * 4096 + 8, 1035 * 4096 + 8):
     ms = f(count, 50)
     if rank == 0:

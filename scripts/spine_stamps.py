@@ -1,6 +1,5 @@
 #!/usr/bin/env python3
 """Where the spine of the persistent Cholesky (chol_dataflow.cu:chol_spine_kernel) spends its time, per 64-column step."""
-import ctypes as C
 import sys
 sys.path.insert(0, ".")
 import numpy as np
@@ -8,10 +7,7 @@ from mrcal_b200 import _capi
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 1270
 nb = (n + 63) // 64
 out = np.zeros(8 * nb, np.int64)
-f = _capi.lib.mrcal_b200_debug_spine_stamps
-f.restype = C.c_bool
-f.argtypes = [C.c_int, C.c_void_p, C.c_int]
-assert f(n, out.ctypes.data_as(C.c_void_p), out.size)
+assert _capi.lib.mrcal_b200_debug_spine_stamps(n, out.ctypes.data, out.size)
 st = out.reshape(nb, 8)
 t0 = st[0, 0]
 print("step  start   trsm  diag-ready  potrf  loads-issued  written  step-end | next ready   (cycles; deltas)")

@@ -3,14 +3,11 @@
 needs; the persistent kernel up to n = 8192, the multi-kernel chain above) and the persistent backward substitution of
 one right-hand side. One line per size, then one JSON line
 with the card's name, power limit and SM clocks, read in the same run. usage: time_cholesky.py n [n...]"""
-import ctypes as C
 import sys
 sys.path.insert(0, ".")
 from mrcal_b200 import _capi
 import measure
 f = _capi.lib.mrcal_b200_debug_time_cholesky
-f.argtypes = [C.c_int, C.c_int, C.c_int]
-f.restype = C.c_double
 
 
 res = {}

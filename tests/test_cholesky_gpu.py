@@ -33,11 +33,7 @@ LD = np.longdouble
 SMALL = 1300          # up to here the longdouble reference factor is computed
 
 _fac = _capi.lib.mrcal_b200_debug_cholesky
-_fac.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_int), C.c_void_p]
-_fac.restype = C.c_bool
 _solve = _capi.lib.mrcal_b200_debug_chol_solve
-_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int]
-_solve.restype = C.c_bool
 
 
 class Factor:

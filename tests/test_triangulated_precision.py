@@ -106,11 +106,10 @@ def test_reference_gradient_precision(ref, truth):
 def test_device_gradient_precision(ref, truth):
     from mrcal_b200 import _capi
     cases, tr = truth
-    f = _capi.lib.mrcal_b200_debug_triangulated_error
-    f.restype = C.c_bool
     out = np.zeros((len(cases), 7))
     inp = np.ascontiguousarray(cases)
-    assert f(inp.ctypes.data_as(C.c_void_p), len(cases), out.ctypes.data_as(C.c_void_p)), _capi.last_error()
+    assert _capi.lib.mrcal_b200_debug_triangulated_error(inp.ctypes.data, len(cases), out.ctypes.data), \
+        _capi.last_error()
     for k, (c, (e_true, g_true)) in enumerate(zip(cases, tr)):
         # our device function is as close to the exact value and gradient as double precision allows -- the same
         # bound the reference meets
