@@ -827,6 +827,38 @@ bool mrcal_b200_poseutils_device(int op, int flags, int ndim, const int64_t* sha
                                  const int64_t* strides0, const double* in1, const int64_t* strides1, double* out0,
                                  double* out1, double* out2, void* stream);
 
+/* The two-view triangulation routines of mrcal.triangulation, element-wise over a broadcast shape: one method
+   (MRCAL_B200_TRIANGULATE_*) applied to every element of the ndim-dimensional shape `shape`, with the reference's
+   inputs and output layouts (mrcal/triangulation.py, triangulation-genpywrap.py):
+
+     method                        inputs                            value    gradients
+     GEOMETRIC, LEECIVERA_L1,      v0, v1, t01 (camera-0 coords)     p (3,)   dp/dv0 (3,3), dp/dv1 (3,3), dp/dt01 (3,3)
+     LEECIVERA_LINF, _MID2, _WMID2
+     LINDSTROM                     v0, v1 (local), Rt01 (4,3)        p (3,)   dp/dv0 (3,3), dp/dv1 (3,3), dp/dRt01 (3,4,3)
+     TRIANGULATED_ERROR            v0, v1, t01 (camera-0 coords)     err ()   derr/dv1 (3,), derr/dt01 (3,)
+
+   In each gradient, entry [i, j] is dp_i/dx_j. TRIANGULATED_ERROR is the solver's measurement of a triangulated
+   point (_mrcal_triangulated_error()); it has no gradient in v0 and no fourth output. Where a method fails (parallel
+   or divergent rays, a point behind a camera) p is (0,0,0), as in the reference, and its gradients are written as
+   zeros: the reference leaves them unwritten. Input k's element at broadcast index (i_0 .. i_ndim-1) starts at
+   in_k + sum_d i_d strides_k[d] (in doubles; 0 where input k is repeated along d, so no input needs to be expanded)
+   and is packed. Outputs are packed: output k of element e starts at out_k + e * (its size). NULL for an output
+   the call does not have. ndim <= 8. False + mrcal_b200_last_error() on refusal or failure */
+enum { MRCAL_B200_TRIANGULATE_GEOMETRIC = 0, MRCAL_B200_TRIANGULATE_LEECIVERA_L1, MRCAL_B200_TRIANGULATE_LEECIVERA_LINF,
+       MRCAL_B200_TRIANGULATE_LEECIVERA_MID2, MRCAL_B200_TRIANGULATE_LEECIVERA_WMID2, MRCAL_B200_TRIANGULATE_LINDSTROM,
+       MRCAL_B200_TRIANGULATE_TRIANGULATED_ERROR, MRCAL_B200_TRIANGULATE_NUM_METHODS };
+enum { MRCAL_B200_TRIANGULATE_GET_GRADIENTS = 1 };
+bool mrcal_b200_triangulate(int method, int flags, int ndim, const int64_t* shape, const double* v0,
+                            const int64_t* strides0, const double* v1, const int64_t* strides1,
+                            const double* t01_or_Rt01, const int64_t* strides2, double* out0, double* out1,
+                            double* out2, double* out3);
+/* The same with every buffer on the device: the kernel is enqueued on stream (a cudaStream_t; NULL: the default
+   stream) and the call returns without waiting for it. shape and the strides stay on the host */
+bool mrcal_b200_triangulate_device(int method, int flags, int ndim, const int64_t* shape, const double* v0,
+                                   const int64_t* strides0, const double* v1, const int64_t* strides1,
+                                   const double* t01_or_Rt01, const int64_t* strides2, double* out0, double* out1,
+                                   double* out2, double* out3, void* stream);
+
 // Timing hook for benchmarks: run N cost-function evaluations (residuals +
 // Jacobian) at the current state back to back, return the mean device time per
 // evaluation in milliseconds (CUDA events on the library's stream); <0 on error

@@ -41,6 +41,10 @@ from .poseutils import (  # noqa: F401
     skew_symmetric, R_from_quat, quat_from_R, qt_from_Rt, Rt_from_qt, R_aligned_to_vector,
     identity_R, identity_r, identity_Rt, identity_rt,
 )
+from .triangulation import (  # noqa: F401
+    triangulate_geometric, triangulate_leecivera_l1, triangulate_leecivera_linf, triangulate_leecivera_mid2,
+    triangulate_leecivera_wmid2, triangulate_lindstrom, _triangulated_error,
+)
 from .cameramodel import cameramodel, CameramodelParseException  # noqa: F401
 from .regions import (  # noqa: F401
     measurements_board, measurements_point, residuals_board, residuals_chessboard, residuals_point,

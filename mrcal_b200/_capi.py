@@ -215,6 +215,8 @@ SIGNATURES = {
     "mrcal_b200_match_feature_device": (OK, [P, P, P, I, I, I, P] + [I] * 4 + [P, P] + [I] * 6 + [P]),
     "mrcal_b200_poseutils": (OK, [I] * 3 + [P] * 8),
     "mrcal_b200_poseutils_device": (OK, [I] * 3 + [P] * 9),
+    "mrcal_b200_triangulate": (OK, [I] * 3 + [P] * 11),
+    "mrcal_b200_triangulate_device": (OK, [I] * 3 + [P] * 12),
     # failure is a negative time
     "mrcal_b200_problem_time_callback": (D, [P, I, B]),
     "mrcal_b200_nccl_get_unique_id": (OK, [P]),

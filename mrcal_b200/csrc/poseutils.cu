@@ -2,14 +2,13 @@
 // Each thread takes one element of the broadcast shape: it decodes the element's offset into every operand (an
 // operand repeated along a dimension has stride 0 there, so it is never expanded in memory), computes in fp64 registers
 // (pose.cuh) and writes the value and any gradients, packed. All indexing is 64-bit.
-#include "device_call.h"
+#include "broadcast.cuh"
 #include "pose.cuh"
 
 namespace mb200 {
 
 namespace {
 
-constexpr int MAX_DIMS = 8;
 enum { F_GRAD = MRCAL_B200_POSE_GET_GRADIENTS, F_INV0 = MRCAL_B200_POSE_INVERTED0, F_INV1 = MRCAL_B200_POSE_INVERTED1 };
 
 // doubles per element of each operand; grad: whether the operation has gradients; ninv: how many inverted flags it takes
@@ -52,13 +51,8 @@ __host__ __device__ constexpr OpShape op_shape(int op)
     }
 }
 
-struct PoseArgs
+struct PoseArgs : Broadcast<2>
 {
-    int64_t N;                          // elements of the broadcast shape
-    int ndim, flags;
-    int64_t shape[MAX_DIMS];
-    const double* in[2];
-    int64_t stride[2][MAX_DIMS];        // in doubles, per broadcast dimension; 0 where the operand is repeated
     double* out[3];                     // packed: element e's output k at out[k] + e * out_k
 };
 
@@ -260,16 +254,9 @@ template <int OP, bool G> __global__ void __launch_bounds__(256) poseutils_kerne
     constexpr OpShape S = op_shape(OP);
     const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if(e >= a.N) return;
-    int64_t rem = e, o0 = 0, o1 = 0;
-    for(int d = a.ndim - 1; d > 0; d--)
-    {
-        const int64_t n = a.shape[d], c = rem % n;
-        rem /= n;
-        o0 += c * a.stride[0][d];
-        o1 += c * a.stride[1][d];
-    }
-    o0 += rem * a.stride[0][0];
-    o1 += rem * a.stride[1][0];
+    int64_t o[2];
+    broadcast_offsets(a, e, o);
+    const int64_t o0 = o[0], o1 = o[1];
 
     double x0[S.in0], x1[S.in1 > 0 ? S.in1 : 1];
 #pragma unroll
@@ -314,8 +301,7 @@ template <int OP = 0> void dispatch(int op, const PoseArgs& a, cudaStream_t stre
     }
 }
 
-// The checks both flavours make, and the arguments of the launch: the broadcast shape with its unit dimensions
-// dropped and, where every operand allows it, neighbouring dimensions merged. Pointers are not filled in
+// The checks both flavours make, and the broadcast frame of the launch. Pointers are not filled in
 bool prepare(PoseArgs& a, int op, int flags, int ndim, const int64_t* shape, const int64_t* strides0,
              const int64_t* strides1)
 {
@@ -331,55 +317,10 @@ bool prepare(PoseArgs& a, int op, int flags, int ndim, const int64_t* shape, con
         set_error("poseutils: operation %d does not take flags 0x%x", op, flags);
         return false;
     }
-    if(ndim < 0 || ndim > MAX_DIMS)
-    {
-        set_error("poseutils: at most %d broadcast dimensions are supported; got %d", MAX_DIMS, ndim);
-        return false;
-    }
+    const int64_t* const st[2] = {strides0, strides1};
+    const int width[2] = {S.in0, S.in1};
     a = PoseArgs{};
-    a.flags = flags;
-    a.N = 1;
-    const int64_t* st[2] = {strides0, strides1};
-    for(int d = 0; d < ndim; d++)
-    {
-        if(shape[d] < 0 || (S.in0 && strides0[d] < 0) || (S.in1 && strides1[d] < 0))
-        {
-            set_error("poseutils: negative size or stride in broadcast dimension %d", d);
-            return false;
-        }
-        a.N *= shape[d];
-        if(shape[d] == 1) continue;
-        const int n = a.ndim;
-        int64_t s[2] = {0, 0};
-        for(int k = 0; k < 2; k++)
-            if(k == 0 ? S.in0 : S.in1) s[k] = st[k][d];
-        // dimension d continues the previous one if each operand steps over it as over one of its elements
-        if(n > 0 && a.stride[0][n - 1] == s[0] * shape[d] && a.stride[1][n - 1] == s[1] * shape[d])
-        {
-            a.shape[n - 1] *= shape[d];
-            a.stride[0][n - 1] = s[0];
-            a.stride[1][n - 1] = s[1];
-            continue;
-        }
-        a.shape[n] = shape[d];
-        a.stride[0][n] = s[0];
-        a.stride[1][n] = s[1];
-        a.ndim++;
-    }
-    if(a.ndim == 0)
-    {
-        a.ndim = 1;
-        a.shape[0] = 1;
-    }
-    return true;
-}
-
-// doubles an operand spans: its last element's offset plus one element
-size_t extent(const PoseArgs& a, int k, int width)
-{
-    int64_t last = 0;
-    for(int d = 0; d < a.ndim; d++) last += (a.shape[d] - 1) * a.stride[k][d];
-    return (size_t)(last + width);
+    return broadcast_prepare<2>(a, "poseutils", flags, ndim, shape, st, width);
 }
 
 }  // namespace
@@ -401,8 +342,8 @@ extern "C" bool mrcal_b200_poseutils(int op, int flags, int ndim, const int64_t*
     DeviceCall D;
     const double *d_in0 = nullptr, *d_in1 = nullptr;
     double *d_out0, *d_out1 = nullptr, *d_out2 = nullptr;
-    if(!D.start() || !D.upload((double**)&d_in0, in0, extent(a, 0, S.in0)) ||
-       (S.in1 && !D.upload((double**)&d_in1, in1, extent(a, 1, S.in1))) || !D.alloc(&d_out0, n0) ||
+    if(!D.start() || !D.upload((double**)&d_in0, in0, broadcast_extent(a, 0, S.in0)) ||
+       (S.in1 && !D.upload((double**)&d_in1, in1, broadcast_extent(a, 1, S.in1))) || !D.alloc(&d_out0, n0) ||
        (n1 && !D.alloc(&d_out1, n1)) || (n2 && !D.alloc(&d_out2, n2)))
         return false;
     a.in[0] = d_in0;

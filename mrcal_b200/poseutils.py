@@ -69,13 +69,16 @@ def _strides(x, lead, nproto, torch):
     return out
 
 
-def _pose(fname, args, protos_in, protos_out, out, get_gradients=False, inverted0=False, inverted1=False):
+def _pose(fname, args, protos_in, protos_out, out, get_gradients=False, inverted0=False, inverted1=False,
+          entry="poseutils", op=None):
     """The outputs of operation fname on args: each args[k] of shape (..., *protos_in[k]), the leading dimensions
-    broadcast together; the value, then (with get_gradients) the gradients, of shapes (broadcast, *protos_out[k])"""
+    broadcast together; the value, then (with get_gradients) the gradients, of shapes (broadcast, *protos_out[k]).
+    entry: the C entry point, mrcal_b200_<entry>() (two inputs, three outputs: the pose utilities) or its _device
+    flavour; "triangulate" has three inputs and four outputs. op: the operation code (default: fname's pose code)"""
     outs = tuple(out) if isinstance(out, (tuple, list)) else ((out,) if out is not None else None)
     torch = _torch_if_tensors(*args, *(outs or ()), what=f"{fname}(): the inputs and out")
     device = None if torch is None else args[0].device
-    names = ("the first input", "the second input")
+    names = ("the first input", "the second input", "the third input")
     args = [_operand(a, p, names[k], fname, torch, device) for k, (a, p) in enumerate(zip(args, protos_in))]
     leads = [tuple(a.shape)[:len(a.shape) - len(p)] for a, p in zip(args, protos_in)]
     try:
@@ -108,19 +111,21 @@ def _pose(fname, args, protos_in, protos_out, out, get_gradients=False, inverted
     if int(np.prod(lead)) > 0:
         flags = (_GET_GRADIENTS if get_gradients else 0) | (_INVERTED0 if inverted0 else 0) | \
             (_INVERTED1 if inverted1 else 0)
-        st = [_strides(a, lead, len(p), torch) for a, p in zip(args, protos_in)] + [None]
+        nin, nout = (2, 3) if entry == "poseutils" else (3, 4)
+        st = [_strides(a, lead, len(p), torch) for a, p in zip(args, protos_in)] + [None] * (nin - len(args))
         shape = np.array(lead, np.int64)
         ptr = (lambda a: a.ctypes.data) if torch is None else (lambda a: a.data_ptr())
-        ins = [ptr(a) for a in args] + [None]
-        o = [ptr(r) for r in res] + [None] * (3 - len(res))
-        call = (_ptr(shape), ins[0], _ptr(st[0]), ins[1], _ptr(st[1]), *o)
+        ins = [ptr(a) for a in args] + [None] * (nin - len(args))
+        o = [ptr(r) for r in res] + [None] * (nout - len(res))
+        call = (_ptr(shape), *(x for k in range(nin) for x in (ins[k], _ptr(st[k]))), *o)
+        code = _OPS[fname] if op is None else op
         if torch is None:
             _require_gpu()
-            checked.mrcal_b200_poseutils(_OPS[fname], flags, len(lead), *call)
+            getattr(checked, f"mrcal_b200_{entry}")(code, flags, len(lead), *call)
         else:
             with torch.cuda.device(device):
                 stream = torch.cuda.current_stream(device).cuda_stream
-                checked.mrcal_b200_poseutils_device(_OPS[fname], flags, len(lead), *call, stream)
+                getattr(checked, f"mrcal_b200_{entry}_device")(code, flags, len(lead), *call, stream)
     if outs is not None:
         for k in range(len(res)):
             if not direct[k]:
