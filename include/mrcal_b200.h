@@ -595,6 +595,12 @@ bool mrcal_b200_problem_reduced_system(mrcal_b200_problem_t* problem, double lam
 // locked) instead of the stored Jacobian. False if this problem does not take it
 bool mrcal_b200_problem_reduced_system_fused(mrcal_b200_problem_t* problem, double lambda, int* n_reduced,
                                              double* S_out, double* g_reduced, double* g_full);
+// Introspection: the two sums of the Cauchy step at the current state, out[0] = |g|^2 and
+// out[1] = |J g|^2 with g = J'x, from the kernels a step of mrcal_b200_problem_optimize()
+// runs: with fused, the board rows of J g from the fused evaluation's blocks and the other
+// rows from their Jacobian rows (false if this problem does not take that path); without,
+// every row from the stored Jacobian
+bool mrcal_b200_problem_cauchy_denominator(mrcal_b200_problem_t* problem, bool fused, double* out);
 
 // Copy results to the host: the packed state, the residuals, the unpacked
 // solution and the (possibly outlier-marked) board observation pool. Any may be NULL

@@ -197,6 +197,7 @@ SIGNATURES = {
     "mrcal_b200_problem_optimize": (OK, [P] * 4),
     "mrcal_b200_problem_reduced_system": (OK, [P, D, P, P, P, P]),
     "mrcal_b200_problem_reduced_system_fused": (OK, [P, D, P, P, P, P]),
+    "mrcal_b200_problem_cauchy_denominator": (OK, [P, B, P]),
     "mrcal_b200_problem_download": (OK, [P] * 9),
     "mrcal_b200_problem_triangulated_outliers": (I, [P, P, I]),
     "mrcal_b200_problem_drt_cross_reprojection__dbpacked": (OK, [P, I, P]),

@@ -902,6 +902,13 @@ class Problem:
         S = np.tril(S) + np.tril(S, -1).T
         return S, g, gf
 
+    def cauchy_denominator(self, fused=False):
+        """(|g|^2, |J g|^2), g = J'x at the current state, from the kernels an optimize() step runs (introspection).
+        fused: the board rows from the fused evaluation's blocks, as in reduced_system(fused=True)."""
+        out = np.zeros(2)
+        checked.mrcal_b200_problem_cauchy_denominator(self._h, bool(fused), _ptr(out))
+        return float(out[0]), float(out[1])
+
     def time_callback(self, N=10, jacobian=True):
         ms = checked.mrcal_b200_problem_time_callback(self._h, int(N), jacobian)
         if ms < 0:

@@ -35,6 +35,11 @@ constexpr int FLDK = 68;    // row stride of Dk [K][<=64 knots]: 4 (mod 16), con
 constexpr int FLDG = 36;    // row stride of G  [K][32]
 constexpr int FMAXK = kCompactMaxKnots;   // most knots of one observation's patch that are touched
 constexpr int FMAXPATCH = 400;   // bounding box of the patch (knots)
+constexpr int FMAXCORNERS = 128; // one thread per corner
+
+// the dynamic shared memory of fused_boards_kernel for K (= W*H rounded up to 4) rows: Dk, G, C, GG and gv (below).
+// 125 088 bytes at K = 128: one CTA per SM above 112 corners (two fit up to K = 112)
+constexpr size_t fused_smem_bytes(int K) { return ((size_t)K * (FLDK + FLDG) + FMAXK * 33 + 14 * 14 + 14 + 2) * sizeof(double); }
 
 }  // namespace
 
@@ -412,11 +417,12 @@ quadform_items_kernel(DevProblem P, NormalBuffers N, const double* __restrict__ 
 // N.active / N.stat for this evaluation and has unpacked the state (launch_unpack_state)
 bool launch_fused_boards(const DevProblem& dp, NormalBuffers& N, const EvalBuffers& out, double* norm_part, cudaStream_t s, int* nlaunch)
 {
-    if(!set_max_dynamic_smem<fused_boards_kernel<4>>(110 * 1024) || !set_max_dynamic_smem<fused_boards_kernel<3>>(110 * 1024)) return false;
+    constexpr size_t smem_max = fused_smem_bytes(FMAXCORNERS);
+    if(!set_max_dynamic_smem<fused_boards_kernel<4>>((int)smem_max) || !set_max_dynamic_smem<fused_boards_kernel<3>>((int)smem_max)) return false;
     const int NWH = dp.W * dp.H;
-    if(NWH > 128) { set_error("internal error: the fused path needs W*H <= 128"); return false; }
+    if(NWH > FMAXCORNERS) { set_error("internal error: the fused path needs W*H <= %d", FMAXCORNERS); return false; }
     const int K = (NWH + 3) & ~3;
-    const size_t smem = ((size_t)K * (FLDK + FLDG) + FMAXK * 33 + 14 * 14 + 14 + 2) * sizeof(double);
+    const size_t smem = fused_smem_bytes(K);
     if(dp.lens_kind == LENS_SPLINED3) fused_boards_kernel<4><<<dp.Nobs_board, 128, smem, s>>>(dp, N, out.x, norm_part, K);
     else                              fused_boards_kernel<3><<<dp.Nobs_board, 128, smem, s>>>(dp, N, out.x, norm_part, K);
     sum_partials_kernel<256><<<1, 256, 0, s>>>(norm_part, dp.Nobs_board, out.norm2);

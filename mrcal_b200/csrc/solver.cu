@@ -145,6 +145,30 @@ static bool count_negative_weights(mrcal_b200_problem* P, int* count)
     return true;
 }
 
+// The sums of the Cauchy step at the operating point `cur`, g = J'x (N.g_full, from the assembly that ran last), into the
+// scalars (slots below): |g|^2 by range in scal[0..8], x.(J g) in scal[9], |J g|^2 in scal[10]. When fused, the board rows
+// of J g come from the observations' blocks and the other rows (from m_point0 on) from their stored Jacobian rows;
+// otherwise every row from its stored row. Rows [0, Nrows) take part. scal[0..10] must be zero
+static bool launch_cauchy_sums(mrcal_b200_problem* P, const EvalBuffers& cur, bool fused, int Nrows, double* scal,
+                               cudaStream_t sc)
+{
+    NormalBuffers& N = P->ws->N;
+    int* nl = &P->launches;
+    dots_kernel<<<3, 1024, 0, sc>>>(N.g_full, nullptr, N.e0, N.e1, P->L.Nstate, scal + 0);
+    const int nsm = std::max(1, device_sm_count());
+    if(fused)
+    {
+        if(!launch_quadform_boards(P->dp, N, N.g_full, N.qf_part, scal + 10, sc, nl)) return false;
+        if(Nrows > P->dp.m_point0)
+            jv_kernel<<<nsm * 4, 256, 0, sc>>>(P->d_rowptr, cur.Jcol, cur.Jval, N.g_full, cur.x, P->dp.m_point0, Nrows, scal + 9);
+    }
+    else
+        jv_kernel<<<nsm * 16, 256, 0, sc>>>(P->d_rowptr, cur.Jcol, cur.Jval, N.g_full, cur.x, 0, Nrows, scal + 9);
+    *nl += 2;
+    MB200_CUDA_CHECK(cudaGetLastError());
+    return true;
+}
+
 ////////////////////////////////////////////////////////////////////////////////
 // one dogleg solve from the current state (the reference's dogleg_optimize2())
 ////////////////////////////////////////////////////////////////////////////////
@@ -397,18 +421,7 @@ static bool dogleg_pass(mrcal_b200_problem* P, const mrcal_b200_solver_parameter
                 cudaStream_t sc = N.s_side[0];
                 MB200_CUDA_CHECK(cudaEventRecord(N.ev_fork, s));
                 MB200_CUDA_CHECK(cudaStreamWaitEvent(sc, N.ev_fork, 0));
-                dots_kernel<<<3, 1024, 0, sc>>>(N.g_full, nullptr, e0, e1, Nstate, ws->scal + 0);
-                const int nsm = std::max(1, device_sm_count());
-                if(N.fused)
-                {
-                    // |J g|^2: the board rows from the observations' blocks, the others from their stored rows
-                    if(!launch_quadform_boards(P->dp, N, N.g_full, N.qf_part, ws->scal + 10, sc, nl)) return false;
-                    if(Nrows_mine > P->dp.m_point0)
-                        jv_kernel<<<nsm * 4, 256, 0, sc>>>(P->d_rowptr, cur.Jcol, cur.Jval, N.g_full, cur.x, P->dp.m_point0, Nrows_mine, ws->scal + 9);
-                }
-                else
-                    jv_kernel<<<nsm * 16, 256, 0, sc>>>(P->d_rowptr, cur.Jcol, cur.Jval, N.g_full, cur.x, 0, Nrows_mine, ws->scal + 9);
-                *nl += 2;
+                if(!launch_cauchy_sums(P, cur, N.fused, Nrows_mine, ws->scal, sc)) return false;
                 MB200_CUDA_CHECK(cudaEventRecord(N.ev_join[0], sc));
                 // eliminated-range dots and the row sums are per-rank partial sums. Sharded: they wait for the partial sums
                 // of the Gauss-Newton dots and go through ONE reduction with them (below)
@@ -639,15 +652,11 @@ extern "C" bool mrcal_b200_problem_reduced_system(mrcal_b200_problem_t* P, doubl
     return download_reduced_system(P, S_out, g_reduced, g_full);
 }
 
-extern "C" bool mrcal_b200_problem_reduced_system_fused(mrcal_b200_problem_t* P, double lambda, int* n_reduced,
-                                                        double* S_out, double* g_reduced, double* g_full)
+// What an optimize() step on the fused path assembles at the current state: the boards' blocks from the fused evaluation,
+// the other rows from their Jacobian. `who` names the caller in the errors
+static bool assemble_fused(mrcal_b200_problem_t* P, double lambda, const char* who)
 {
-    if(!build_workspace(P)) return false;
     NormalBuffers& N = P->ws->N;
-    if(n_reduced) *n_reduced = N.n_r;
-    if(!N.fused) { set_error("reduced_system_fused: this problem does not take the fused evaluation"); return false; }
-    if(S_out == nullptr && g_reduced == nullptr && g_full == nullptr) return true;
-    // what an optimize() step does: the boards' blocks from the fused evaluation, the other rows from their Jacobian
     cudaStream_t s = P->stream;
     int* nl = &P->launches;
     const EvalBuffers& o = P->op[P->cur];
@@ -656,11 +665,43 @@ extern "C" bool mrcal_b200_problem_reduced_system_fused(mrcal_b200_problem_t* P,
     if(!normal_adopt_sizes(N, s)) return false;
     if(N.h_stat[3] != 0)
     {
-        set_error("reduced_system_fused: the fused evaluation's blocks do not fit this problem");
+        set_error("%s: the fused evaluation's blocks do not fit this problem", who);
         return false;
     }
-    if(!normal_finish(P->dp, N, o, P->d_rowptr, lambda, s, nl, true)) return false;
+    return normal_finish(P->dp, N, o, P->d_rowptr, lambda, s, nl, true);
+}
+
+extern "C" bool mrcal_b200_problem_reduced_system_fused(mrcal_b200_problem_t* P, double lambda, int* n_reduced,
+                                                        double* S_out, double* g_reduced, double* g_full)
+{
+    if(!build_workspace(P)) return false;
+    NormalBuffers& N = P->ws->N;
+    if(n_reduced) *n_reduced = N.n_r;
+    if(!N.fused) { set_error("reduced_system_fused: this problem does not take the fused evaluation"); return false; }
+    if(S_out == nullptr && g_reduced == nullptr && g_full == nullptr) return true;
+    if(!assemble_fused(P, lambda, "reduced_system_fused")) return false;
     return download_reduced_system(P, S_out, g_reduced, g_full);
+}
+
+extern "C" bool mrcal_b200_problem_cauchy_denominator(mrcal_b200_problem_t* P, bool fused, double* out)
+{
+    if(!build_workspace(P)) return false;
+    NormalBuffers& N = P->ws->N;
+    if(fused && !N.fused) { set_error("cauchy_denominator: this problem does not take the fused evaluation"); return false; }
+    cudaStream_t s = P->stream;
+    // (the row pointers are analytic; jv_kernel reads them, and the fused evaluation does not write them)
+    if(!problem_evaluate(P, P->cur, !fused, true)) return false;
+    if(fused ? !assemble_fused(P, 0., "cauchy_denominator")
+             : !normal_assemble(P->dp, N, P->op[P->cur], P->d_rowptr, 0., s, &P->launches)) return false;
+    double* scal = P->ws->scal;
+    MB200_CUDA_CHECK(cudaMemsetAsync(scal, 0, 11 * sizeof(double), s));
+    if(!launch_cauchy_sums(P, P->op[P->cur], fused, P->L.Nmeas, scal, s)) return false;
+    double h[11];
+    MB200_CUDA_CHECK(cudaMemcpyAsync(h, scal, sizeof(h), cudaMemcpyDeviceToHost, s));
+    MB200_CUDA_CHECK(cudaStreamSynchronize(s));
+    out[0] = h[0] + h[3] + h[6];
+    out[1] = h[10];
+    return true;
 }
 
 extern "C" bool mrcal_b200_problem_optimize(mrcal_b200_problem_t* P, const mrcal_b200_solver_parameters_t* parameters,
