@@ -648,6 +648,12 @@ bool mrcal_b200_problem_projection_uncertainty_cameras(mrcal_b200_problem_t* pro
                                                        const mrcal_point3_t* p_cam, double observed_pixel_uncertainty,
                                                        double* Var, double* sigma_used);
 
+/* The observed-pixel uncertainty estimated from the residuals at the problem's current state
+   (mrcal.model_analysis._observed_pixel_uncertainty_from_inputs(), model_analysis.py:491-556): the estimate, and the
+   evaluation behind it, that mrcal_b200_problem_projection_uncertainty() makes, so *sigma is bit for bit the
+   *sigma_used it returns. False + mrcal_b200_last_error() without board or point observations, or on failure */
+bool mrcal_b200_problem_observed_pixel_uncertainty(mrcal_b200_problem_t* problem, double* sigma);
+
 /* Residual statistics binned by imager cell, as mrcal.calibration._report_regional_statistics() computes them
    (mrcal/calibration.py:1720-1866), for the cameras icam_intrinsics [Ncameras] in one launch. q_cell_center
    [Ncameras][gridn_height][gridn_width][2]: each camera's cell centres (mrcal.sample_imager()); rcell [Ncameras][2]:
@@ -864,6 +870,37 @@ bool mrcal_b200_triangulate_device(int method, int flags, int ndim, const int64_
                                    const int64_t* strides0, const double* v1, const int64_t* strides1,
                                    const double* t01_or_Rt01, const int64_t* strides2, double* out0, double* out1,
                                    double* out2, double* out3, void* stream);
+
+/* The projections behind mrcal.synthesize_board_observations() (mrcal/synthetic_data.py:236-554) for one chunk of
+   Nframes board poses: Rt_ref_boardref [Nframes][4][3] = Rt_from_rt(rt_ref_boardref [Nframes][6]); for every frame,
+   camera and corner of board [Npoints][3] (the centered board), q [Nframes][Ncameras][Npoints][2] =
+   project(transform_point_Rt(Rt_cam_ref[c], transform_point_Rt(Rt_ref_boardref[f], corner))), two transforms as
+   the reference makes them; Nvisible [Nframes][Ncameras] counts the corners with 0 <= q <= imagersize - 1 on both
+   axes. Camera c has the lens model lensmodels[c], its intrinsics packed one camera after the other in intrinsics,
+   Rt_cam_ref [Ncameras][4][3] and imagersizes [Ncameras][2] (width, height). The random poses, the culling and the
+   selection of frames are the caller's. False + mrcal_b200_last_error() on refusal or failure */
+bool mrcal_b200_synthesize_board_observations(double* q, int* Nvisible, double* Rt_ref_boardref,
+                                              const double* rt_ref_boardref, int Nframes, const double* board,
+                                              int Npoints, int Ncameras, const mrcal_lensmodel_t* lensmodels,
+                                              const double* intrinsics, const double* Rt_cam_ref,
+                                              const int* imagersizes);
+/* The camera-frame board corners and the perfect observations of a problem, as mrcal.hypothesis_board_corner_positions()
+   (mrcal/utils.py:440-584) and mrcal.make_perfect_observations() (mrcal/synthetic_data.py:594-750) compute them. For
+   each board observation o (indices in the Python order: iframe, icam_intrinsics, icam_extrinsics) and each corner of
+   board [Npoints_board][3] (ref_calibration_object() of the problem), pcam_board [o][corner][3] =
+   transform_point_Rt(compose_Rt(Rt_cam_ref, Rt_ref_frame), corner), Rt_cam_ref the identity for icam_extrinsics = -1,
+   and q_board [o][corner][2] its projection through the camera's intrinsics [Ncameras_intrinsics][Nintrinsics]. For
+   each point observation (i_point, icam_intrinsics, icam_extrinsics), q_point [o][2] = the projection of
+   transform_point_Rt(Rt_cam_ref, points[i_point]). Any of the three outputs may be NULL, but point observations need
+   q_point; lensmodel and intrinsics are needed only to project. False + mrcal_b200_last_error() on refusal (an index
+   out of range) or failure */
+bool mrcal_b200_problem_corners(double* pcam_board, double* q_board, double* q_point,
+                                const int32_t* indices_frame_camintrinsics_camextrinsics, int Nobservations_board,
+                                const double* board, int Npoints_board,
+                                const int32_t* indices_point_camintrinsics_camextrinsics, int Nobservations_point,
+                                const double* points, int Npoints, const double* rt_ref_frame, int Nframes,
+                                const double* rt_cam_ref, int Ncameras_extrinsics, const mrcal_lensmodel_t* lensmodel,
+                                const double* intrinsics, int Ncameras_intrinsics);
 
 // Timing hook for benchmarks: run N cost-function evaluations (residuals +
 // Jacobian) at the current state back to back, return the mean device time per

@@ -45,6 +45,9 @@ from .triangulation import (  # noqa: F401
     triangulate_geometric, triangulate_leecivera_l1, triangulate_leecivera_linf, triangulate_leecivera_mid2,
     triangulate_leecivera_wmid2, triangulate_lindstrom, _triangulated_error,
 )
+from .synthetic_data import (  # noqa: F401
+    ref_calibration_object, synthesize_board_observations, hypothesis_board_corner_positions, make_perfect_observations,
+)
 from .cameramodel import cameramodel, CameramodelParseException  # noqa: F401
 from .regions import (  # noqa: F401
     measurements_board, measurements_point, residuals_board, residuals_chessboard, residuals_point,

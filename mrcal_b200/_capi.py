@@ -203,6 +203,7 @@ SIGNATURES = {
     "mrcal_b200_problem_drt_cross_reprojection__dbpacked": (OK, [P, I, P]),
     "mrcal_b200_problem_projection_uncertainty": (OK, [P, I, I, B, P, I, D, P, P]),
     "mrcal_b200_problem_projection_uncertainty_cameras": (OK, [P, P, P, I, I, B, P, D, P, P]),
+    "mrcal_b200_problem_observed_pixel_uncertainty": (OK, [P, P]),
     "mrcal_b200_problem_regional_statistics": (OK, [P, P, I, I, I, P, P, B, P, P]),
     "mrcal_b200_implied_Rt10__from_unprojections": (OK, [P, P, I, P, I, P, P, B, P, D]),
     "mrcal_b200_projection_diff": (OK, [P, P, P, P, I, P, I, P, I, P, P, P, P, D, B]),
@@ -218,6 +219,8 @@ SIGNATURES = {
     "mrcal_b200_poseutils_device": (OK, [I] * 3 + [P] * 9),
     "mrcal_b200_triangulate": (OK, [I] * 3 + [P] * 11),
     "mrcal_b200_triangulate_device": (OK, [I] * 3 + [P] * 12),
+    "mrcal_b200_synthesize_board_observations": (OK, [P, P, P, P, I, P, I, I, P, P, P, P]),
+    "mrcal_b200_problem_corners": (OK, [P, P, P, P, I, P, I, P, I, P, I, P, I, P, I, P, P, I]),
     # failure is a negative time
     "mrcal_b200_problem_time_callback": (D, [P, I, B]),
     "mrcal_b200_nccl_get_unique_id": (OK, [P]),

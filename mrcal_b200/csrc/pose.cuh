@@ -305,6 +305,12 @@ __host__ __device__ __forceinline__ void invert_Rt(double out[12], const double 
     for(int i = 0; i < 3; i++) out[9 + i] = -(out[3 * i] * Rt[9] + out[3 * i + 1] * Rt[10] + out[3 * i + 2] * Rt[11]);
 }
 
+// R x + t (mrcal_transform_point_Rt_full, poseutils.c:271-424, not inverted). out must not alias x
+__host__ __device__ __forceinline__ void transform_point_Rt(double out[3], const double Rt[12], const double x[3])
+{
+    for(int i = 0; i < 3; i++) out[i] = Rt[3 * i] * x[0] + Rt[3 * i + 1] * x[1] + Rt[3 * i + 2] * x[2] + Rt[9 + i];
+}
+
 // x -> Rt0(Rt1(x)), Rt0 and Rt1 taken inverted where asked: the four cases of mrcal_compose_Rt_full
 // (poseutils.c:603-738). out must not alias Rt0 or Rt1
 __host__ __device__ __forceinline__ void compose_Rt(double out[12], const double Rt0[12], const double Rt1[12],

@@ -483,6 +483,27 @@ extern "C" bool mrcal_b200_problem_projection_uncertainty(mrcal_b200_problem_t* 
     return uncertainty_cameras(P, method, atinfinity, Q, p_cam, observed_pixel_uncertainty, Var, sigma_used);
 }
 
+extern "C" bool mrcal_b200_problem_observed_pixel_uncertainty(mrcal_b200_problem_t* P, double* sigma)
+{
+    if(mrcal_b200_device_count() <= 0) { set_error("no usable CUDA device: libmrcal_b200 has no CPU fallback"); return false; }
+    if(P == nullptr) { set_error("observed_pixel_uncertainty: no problem"); return false; }
+    const Layout& L = P->L;
+    if(L.Nmeas_board + L.Nmeas_point == 0)
+    { set_error("observed_pixel_uncertainty cannot be computed because we don't have any board or point observations"); return false; }
+    DeviceArena mem;
+    double* d_sigma;
+    if(!mem.alloc(&d_sigma, 1)) return false;
+    // the evaluation schur_factor_build() makes, so that the residuals, and sigma, are those projection_uncertainty() uses
+    if(!problem_evaluate(P, P->cur, true, true)) return false;
+    const EvalBuffers& op = P->op[P->cur];
+    sigma_kernel<<<1, 256, 0, P->stream>>>(op.x, L.m_board0, L.Nmeas_board, L.m_point0, L.Nmeas_point, L.Nstate, -1.,
+                                           d_sigma);
+    MB200_CUDA_CHECK(cudaGetLastError());
+    MB200_CUDA_CHECK(cudaMemcpyAsync(sigma, d_sigma, sizeof(double), cudaMemcpyDeviceToHost, P->stream));
+    MB200_CUDA_CHECK(cudaStreamSynchronize(P->stream));
+    return true;
+}
+
 extern "C" bool mrcal_b200_problem_projection_uncertainty_cameras(mrcal_b200_problem_t* P, const int* icam_intrinsics,
                                                                   const int* N, int Ncameras, int method, bool atinfinity,
                                                                   const mrcal_point3_t* p_cam,

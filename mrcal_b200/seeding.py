@@ -30,17 +30,7 @@ import numpy as np
 
 # absolute, so that this file also runs when loaded by its path rather than as part of the package
 from mrcal_b200._poses_host import R_from_r, Rt_from_rt, compose_Rt, invert_Rt, r_from_R, rt_from_Rt, transform_point_Rt
-
-
-def ref_calibration_object(W, H, object_spacing, calobject_warp=None):
-    """Board corners in the board's own coordinates, shape (H,W,3) (mrcal/synthetic_data.py:25)."""
-    xx, yy = np.meshgrid(np.arange(W, dtype=float), np.arange(H, dtype=float))
-    full = np.stack((xx * object_spacing, yy * object_spacing, np.zeros_like(xx)), -1)
-    if calobject_warp is not None:
-        xr = xx / (W - 1)
-        yr = yy / (H - 1)
-        full[..., 2] += calobject_warp[0] * 4. * xr * (1. - xr) + calobject_warp[1] * 4. * yr * (1. - yr)
-    return full
+from mrcal_b200.synthetic_data import ref_calibration_object
 
 
 def align_procrustes_points_Rt01(p0, p1):
