@@ -335,6 +335,30 @@ bool mrcal_unproject(mrcal_point3_t* out, const mrcal_point2_t* q, int N,
 bool mrcal_b200_unproject_with_gradients(mrcal_point3_t* v, double* dv_dq, double* dv_dintrinsics,
                                          const mrcal_point2_t* q, int N, const mrcal_lensmodel_t* lensmodel,
                                          const double* intrinsics, bool normalize);
+/* mrcal_project(), or with MRCAL_B200_PROJECT_UNPROJECT mrcal_b200_unproject_with_gradients(), element-wise over a
+   broadcast shape: each element of the ndim-dimensional shape `shape` projects its point `in` (3,) through its
+   intrinsics row (Nintrinsics,), or unprojects its pixel `in` (2,). Every row has one lens model, `lensmodel`.
+     flags: MRCAL_B200_PROJECT_GET_GRADIENTS   dout_din (2,3) or (3,2) and dout_dintrinsics (2 or 3,Nintrinsics; dense:
+                                               the entries the projection does not touch are 0). Either may be NULL
+            MRCAL_B200_PROJECT_UNPROJECT       unproject: out is the ray (3,)
+            MRCAL_B200_PROJECT_NORMALIZE       (with UNPROJECT) unit rays, as mrcal_b200_unproject_with_gradients()
+   The values, the NaN of a failed unprojection and the refusal of CAHVORE with E != 0 (in any row the call reads) are
+   those of the single-intrinsics entries. Operand element at broadcast index (i_0 .. i_ndim-1) starts at
+   in + sum_d i_d strides_in[d] (intrinsics + sum_d i_d strides_intrinsics[d]), in doubles; 0 where the operand is
+   repeated along d, so no operand needs to be expanded, and is packed. Outputs are packed: output k of element e
+   starts at out_k + e * (its size). ndim <= 8. False + mrcal_b200_last_error() on refusal or failure */
+enum { MRCAL_B200_PROJECT_GET_GRADIENTS = 1, MRCAL_B200_PROJECT_UNPROJECT = 2, MRCAL_B200_PROJECT_NORMALIZE = 4 };
+bool mrcal_b200_project(const mrcal_lensmodel_t* lensmodel, int flags, int ndim, const int64_t* shape,
+                        const double* in, const int64_t* strides_in, const double* intrinsics,
+                        const int64_t* strides_intrinsics, double* out, double* dout_din, double* dout_dintrinsics);
+/* The same with every buffer on the device: the kernel is enqueued on stream (a cudaStream_t; NULL: the default
+   stream) and the call returns without waiting for it, except when it unprojects with CAHVORE: then one flag per call
+   comes back to the host to check every intrinsics row's E terms, and the call waits for the stream. shape and the
+   strides stay on the host */
+bool mrcal_b200_project_device(const mrcal_lensmodel_t* lensmodel, int flags, int ndim, const int64_t* shape,
+                               const double* in, const int64_t* strides_in, const double* intrinsics,
+                               const int64_t* strides_intrinsics, double* out, double* dout_din,
+                               double* dout_dintrinsics, void* stream);
 /* The angular resolution of a camera in degrees per pixel at N pixels, as mrcal.model_resolution__deg_pixel()
    computes it (mrcal/model_analysis.py:2152-2246): from the eigenvalues of M'M, M = dq/dv [u0 u1] at the unit ray v
    of each pixel, [u0 u1] an orthonormal basis of the plane perpendicular to v, the smaller one clamped at 1e-6. mode:

@@ -170,6 +170,8 @@ SIGNATURES = {
     "mrcal_project": (OK, [P, P, P, P, I, P, P]),
     "mrcal_unproject": (OK, [P, P, I, P, P]),
     "mrcal_b200_unproject_with_gradients": (OK, [P] * 4 + [I, P, P, B]),
+    "mrcal_b200_project": (OK, [P, I, I] + [P] * 8),
+    "mrcal_b200_project_device": (OK, [P, I, I] + [P] * 9),
     "mrcal_b200_model_resolution__deg_pixel": (OK, [P, P, I, P, P, I]),
     "mrcal_rectified_resolution": (OK, [P] * 7 + [I]),
     "mrcal_rectified_system2": (OK, [P] * 8 + [D] + [P] * 4 + [I] + [B] * 4),

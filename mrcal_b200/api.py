@@ -1250,119 +1250,118 @@ def unpack_state(b, **kwargs):
     return _pack_unpack(b, False, kwargs)
 
 
-def project(v, lensmodel, intrinsics_data, get_gradients=False):
-    """q = project(v): the reference's mrcal.project() for one camera (mrcal-pywrap.c / mrcal.h:165-191).
-    v: (...,3) points in camera coordinates. Returns q (...,2); with get_gradients, as the reference,
-    (q, dq_dv (...,2,3), dq_dintrinsics (...,2,Nintrinsics))."""
-    _require_gpu()
-    v = np.ascontiguousarray(v, dtype=np.float64)
-    if v.shape[-1] != 3:
-        raise RuntimeError("project(): the last dimension of v must be 3")
+_PROJECT_UNPROJECT, _PROJECT_NORMALIZE = 2, 4   # MRCAL_B200_PROJECT_* of include/mrcal_b200.h
+
+
+def _projection(fname, x, lensmodel, intrinsics_data, flags, get_gradients, out, names, dintrinsics=True):
+    """The (un)projection of x through intrinsics_data in the pose utilities' call frame (poseutils._pose()):
+    mrcal_b200_project[_device](). dintrinsics: whether the gradients include the one in the intrinsics"""
+    from .poseutils import _pose
     lm = _lensmodel(lensmodel)
-    intr = np.ascontiguousarray(intrinsics_data, dtype=np.float64)
     Nintr = checked.mrcal_lensmodel_num_params(C.byref(lm))
-    if intr.shape != (Nintr,):
-        raise RuntimeError(f"project(): intrinsics_data must have shape ({Nintr},)")
-    flat = v.reshape(-1, 3)
-    q = np.zeros((flat.shape[0], 2))
-    g = np.zeros((flat.shape[0], 2, 3)) if get_gradients else None
-    gi = np.zeros((flat.shape[0], 2, intr.shape[0])) if get_gradients else None
-    checked.mrcal_project(_ptr(q), _ptr(g), _ptr(gi), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr))
-    q = q.reshape(v.shape[:-1] + (2,))
-    if not get_gradients:
-        return q
-    return q, g.reshape(v.shape[:-1] + (2, 3)), gi.reshape(v.shape[:-1] + (2, intr.shape[0]))
+    w_in, w_out = (2, 3) if flags & _PROJECT_UNPROJECT else (3, 2)
+    grads = ((w_out, w_in),) + (((w_out, Nintr),) if dintrinsics else ()) if get_gradients else ()
+    return _pose(fname, (x, intrinsics_data), ((w_in,), (Nintr,)), ((w_out,),) + grads, out, get_gradients,
+                 entry="project", op=flags, lensmodel=lm, names=names)
 
 
-def unproject(q, lensmodel, intrinsics_data, *, normalize=False, get_gradients=False):
+def project(v, lensmodel, intrinsics_data, get_gradients=False, *, out=None):
+    """q = project(v), as the reference's mrcal.project() (mrcal/projections.py, mrcal.h:165-191). v: (...,3) points
+    in camera coordinates; intrinsics_data: (...,Nintrinsics), one lens model for all. The leading dimensions
+    broadcast together (at most 8 of them); a broadcast operand is read in place, never expanded. Returns q
+    (...,2); with get_gradients, as the reference, (q, dq_dv (...,2,3), dq_dintrinsics (...,2,Nintrinsics): dense,
+    0 where the projection does not depend on an intrinsic). v and intrinsics_data (and out) are either numpy arrays
+    (or lists), converted to float64, or all torch CUDA float64 tensors on one device: the results are then tensors on
+    that device, and the kernel is enqueued on torch.cuda.current_stream() without waiting for it. out= writes the
+    results into the given array (a tuple of three with get_gradients) and returns it."""
+    return _projection("project", v, lensmodel, intrinsics_data, 0, get_gradients, out, ("v", "intrinsics_data"))
+
+
+def unproject(q, lensmodel, intrinsics_data, *, normalize=False, get_gradients=False, out=None):
     """Observation rays of pixels q (...,2), as the reference's mrcal.unproject() returns them
     (mrcal/projections.py:112-397). Returns v (...,3); with get_gradients, (v, dv_dq (...,3,2), dv_dintrinsics
     (...,3,Nintrinsics), dense). The rays are not normalised unless normalize; then the gradients are those of the unit
     rays. As in the reference, the magnitude of an unnormalised ray may change with get_gradients: the gradients are
     those of the ray returned with them. A pixel that cannot be unprojected gives NaN (the zero vector with normalize
-    and no gradients)."""
-    _require_gpu()
-    q = np.ascontiguousarray(q, dtype=np.float64)
-    if q.shape[-1] != 2:
-        raise RuntimeError("unproject(): the last dimension of q must be 2")
-    lm = _lensmodel(lensmodel)
-    intr = np.ascontiguousarray(intrinsics_data, dtype=np.float64)
-    flat = q.reshape(-1, 2)
-    v = np.zeros((flat.shape[0], 3))
-    if not normalize and not get_gradients:
-        checked.mrcal_unproject(_ptr(v), _ptr(flat), flat.shape[0], C.byref(lm), _ptr(intr))
-        return v.reshape(q.shape[:-1] + (3,))
-    Nintr = checked.mrcal_lensmodel_num_params(C.byref(lm))
-    if intr.shape != (Nintr,):
-        raise RuntimeError(f"unproject(): intrinsics_data must have shape ({Nintr},)")
-    g = np.zeros((flat.shape[0], 3, 2)) if get_gradients else None
-    gi = np.zeros((flat.shape[0], 3, Nintr)) if get_gradients else None
-    checked.mrcal_b200_unproject_with_gradients(_ptr(v), _ptr(g), _ptr(gi), _ptr(flat), flat.shape[0], C.byref(lm),
-                                                _ptr(intr), bool(normalize))
-    v = v.reshape(q.shape[:-1] + (3,))
-    if not get_gradients:
-        return v
-    return v, g.reshape(q.shape[:-1] + (3, 2)), gi.reshape(q.shape[:-1] + (3, Nintr))
+    and no gradients). intrinsics_data is (...,Nintrinsics); broadcasting, the torch CUDA tensors and out= are those of
+    project(). CAHVORE with E != 0 in any intrinsics row is refused; with tensors that check brings one flag back to the
+    host, so unprojecting through CAHVORE waits for the current stream."""
+    flags = _PROJECT_UNPROJECT | (_PROJECT_NORMALIZE if normalize else 0)
+    return _projection("unproject", q, lensmodel, intrinsics_data, flags, get_gradients, out, ("q", "intrinsics_data"))
 
 
 _FXYCXY_IDENTITY = np.array((1.0, 1.0, 0.0, 0.0))
 
 
-def _project_closed_form(lensmodel, points, fxycxy, get_gradients):
-    if not get_gradients:
-        return project(points, lensmodel, fxycxy)
-    q, dq_dp, _ = project(points, lensmodel, fxycxy, get_gradients=True)
-    return q, dq_dp
+def _fxycxy(points, fxycxy):
+    """fxycxy; the default core f = 1, c = 0 on the device of tensor points"""
+    torch = sys.modules.get("torch")
+    if fxycxy is _FXYCXY_IDENTITY and torch is not None and isinstance(points, torch.Tensor) and points.is_cuda:
+        # filled on the device, in stream order: no upload from the host
+        fxycxy = torch.zeros(4, dtype=torch.float64, device=points.device)
+        fxycxy[:2] = 1.
+    return fxycxy
 
 
-def _unproject_closed_form(lensmodel, points, fxycxy, get_gradients):
-    if not get_gradients:
-        return unproject(points, lensmodel, fxycxy)
-    v, dv_dq, _ = unproject(points, lensmodel, fxycxy, get_gradients=True)
-    return v, dv_dq
+def _project_closed_form(lensmodel, points, fxycxy, get_gradients, out):
+    return _projection(f"project_{lensmodel[10:].lower()}", points, lensmodel, _fxycxy(points, fxycxy), 0,
+                       get_gradients, out, ("points", "fxycxy"), dintrinsics=False)
 
 
-def project_pinhole(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
-    """q = (f x/z + c) of points (...,3), as mrcal.project_pinhole(); with get_gradients, (q, dq_dp (...,2,3))"""
-    return _project_closed_form("LENSMODEL_PINHOLE", points, fxycxy, get_gradients)
+def _unproject_closed_form(lensmodel, points, fxycxy, get_gradients, out):
+    return _projection(f"unproject_{lensmodel[10:].lower()}", points, lensmodel, _fxycxy(points, fxycxy),
+                       _PROJECT_UNPROJECT, get_gradients, out, ("points", "fxycxy"), dintrinsics=False)
 
 
-def unproject_pinhole(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
-    """v = ((q - c)/f, 1) of pixels (...,2), as mrcal.unproject_pinhole(); with get_gradients, (v, dv_dq (...,3,2))"""
-    return _unproject_closed_form("LENSMODEL_PINHOLE", points, fxycxy, get_gradients)
+def project_pinhole(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False, out=None):
+    """q = (f x/z + c) of points (...,3), as mrcal.project_pinhole(); with get_gradients, (q, dq_dp (...,2,3)).
+    fxycxy (...,4) broadcasts with the points; torch CUDA tensors and out= as in project()"""
+    return _project_closed_form("LENSMODEL_PINHOLE", points, fxycxy, get_gradients, out)
 
 
-def project_stereographic(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+def unproject_pinhole(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False, out=None):
+    """v = ((q - c)/f, 1) of pixels (...,2), as mrcal.unproject_pinhole(); with get_gradients, (v, dv_dq (...,3,2)).
+    fxycxy (...,4) broadcasts with the points; torch CUDA tensors and out= as in project()"""
+    return _unproject_closed_form("LENSMODEL_PINHOLE", points, fxycxy, get_gradients, out)
+
+
+def project_stereographic(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False, out=None):
     """The stereographic projection of points (...,3), as mrcal.project_stereographic(); with get_gradients,
-    (q, dq_dp (...,2,3))"""
-    return _project_closed_form("LENSMODEL_STEREOGRAPHIC", points, fxycxy, get_gradients)
+    (q, dq_dp (...,2,3)).
+    fxycxy (...,4) broadcasts with the points; torch CUDA tensors and out= as in project()"""
+    return _project_closed_form("LENSMODEL_STEREOGRAPHIC", points, fxycxy, get_gradients, out)
 
 
-def unproject_stereographic(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+def unproject_stereographic(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False, out=None):
     """The stereographic unprojection of pixels (...,2), as mrcal.unproject_stereographic(); with get_gradients,
-    (v, dv_dq (...,3,2))"""
-    return _unproject_closed_form("LENSMODEL_STEREOGRAPHIC", points, fxycxy, get_gradients)
+    (v, dv_dq (...,3,2)).
+    fxycxy (...,4) broadcasts with the points; torch CUDA tensors and out= as in project()"""
+    return _unproject_closed_form("LENSMODEL_STEREOGRAPHIC", points, fxycxy, get_gradients, out)
 
 
-def project_lonlat(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+def project_lonlat(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False, out=None):
     """The equirectangular (longitude, latitude) projection of points (...,3), as mrcal.project_lonlat(); with
-    get_gradients, (q, dq_dp (...,2,3))"""
-    return _project_closed_form("LENSMODEL_LONLAT", points, fxycxy, get_gradients)
+    get_gradients, (q, dq_dp (...,2,3)).
+    fxycxy (...,4) broadcasts with the points; torch CUDA tensors and out= as in project()"""
+    return _project_closed_form("LENSMODEL_LONLAT", points, fxycxy, get_gradients, out)
 
 
-def unproject_lonlat(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+def unproject_lonlat(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False, out=None):
     """Unit rays of equirectangular (longitude, latitude) pixels (...,2), as mrcal.unproject_lonlat(); with
-    get_gradients, (v, dv_dq (...,3,2))"""
-    return _unproject_closed_form("LENSMODEL_LONLAT", points, fxycxy, get_gradients)
+    get_gradients, (v, dv_dq (...,3,2)).
+    fxycxy (...,4) broadcasts with the points; torch CUDA tensors and out= as in project()"""
+    return _unproject_closed_form("LENSMODEL_LONLAT", points, fxycxy, get_gradients, out)
 
 
-def project_latlon(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+def project_latlon(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False, out=None):
     """The transverse equirectangular (latitude, longitude) projection of points (...,3), as mrcal.project_latlon();
-    with get_gradients, (q, dq_dp (...,2,3))"""
-    return _project_closed_form("LENSMODEL_LATLON", points, fxycxy, get_gradients)
+    with get_gradients, (q, dq_dp (...,2,3)).
+    fxycxy (...,4) broadcasts with the points; torch CUDA tensors and out= as in project()"""
+    return _project_closed_form("LENSMODEL_LATLON", points, fxycxy, get_gradients, out)
 
 
-def unproject_latlon(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False):
+def unproject_latlon(points, fxycxy=_FXYCXY_IDENTITY, *, get_gradients=False, out=None):
     """Unit rays of transverse equirectangular (latitude, longitude) pixels (...,2), as mrcal.unproject_latlon(); with
-    get_gradients, (v, dv_dq (...,3,2))"""
-    return _unproject_closed_form("LENSMODEL_LATLON", points, fxycxy, get_gradients)
+    get_gradients, (v, dv_dq (...,3,2)).
+    fxycxy (...,4) broadcasts with the points; torch CUDA tensors and out= as in project()"""
+    return _unproject_closed_form("LENSMODEL_LATLON", points, fxycxy, get_gradients, out)

@@ -1,5 +1,5 @@
-// The broadcast frame of the element-wise kernels (poseutils.cu, triangulation.cu): one thread per element of a
-// broadcast shape, K operands read through per-dimension strides (0 where an operand is repeated, so it is never
+// The broadcast frame of the element-wise kernels (poseutils.cu, triangulation.cu, project.cu): one thread per element
+// of a broadcast shape, K operands read through per-dimension strides (0 where an operand is repeated, so it is never
 // expanded in memory), every index 64-bit.
 #pragma once
 #include <cstdint>
@@ -20,7 +20,8 @@ template <int K> struct Broadcast
 };
 
 // o[k]: the offset of operand k's element e
-template <int K> __device__ __forceinline__ void broadcast_offsets(const Broadcast<K>& a, int64_t e, int64_t o[K])
+template <int K>
+__host__ __device__ __forceinline__ void broadcast_offsets(const Broadcast<K>& a, int64_t e, int64_t o[K])
 {
     int64_t rem = e;
     for(int k = 0; k < K; k++) o[k] = 0;
@@ -84,6 +85,29 @@ bool broadcast_prepare(Broadcast<K>& a, const char* who, int flags, int ndim, co
         a.shape[0] = 1;
     }
     return true;
+}
+
+// The rows of operand k that a broadcast reads, each once: a frame over a's dimensions where k is not repeated, its
+// operand 0 being a's operand k
+template <int K> Broadcast<1> broadcast_rows(const Broadcast<K>& a, int k)
+{
+    Broadcast<1> r{};
+    r.N = 1;
+    r.in[0] = a.in[k];
+    for(int d = 0; d < a.ndim; d++)
+        if(a.stride[k][d] != 0 && a.shape[d] != 1)
+        {
+            r.shape[r.ndim] = a.shape[d];
+            r.stride[0][r.ndim] = a.stride[k][d];
+            r.N *= a.shape[d];
+            r.ndim++;
+        }
+    if(r.ndim == 0)
+    {
+        r.ndim = 1;
+        r.shape[0] = 1;
+    }
+    return r;
 }
 
 // doubles operand k spans: its last element's offset plus one element

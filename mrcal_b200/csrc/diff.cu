@@ -508,17 +508,24 @@ extern "C" bool mrcal_b200_stereo_pair_reproject(double* out, double* outlen, co
     const unsigned blocks = (unsigned)((N + 127) / 128);
     for(int p = 0; p < Npairs; p++)
     {
-        LensArgs a0 = lens[2 * p].a, a1 = lens[2 * p + 1].a;
-        a0.intr = d_intr + off[2 * p];
+        // the unprojection: the pixels packed, camera 0's intrinsics repeated
+        const int64_t shape[1] = {N}, st_q[1] = {2}, st_intr[1] = {0};
+        const int64_t* const st[2] = {st_q, st_intr};
+        const int width[2] = {2, lens[2 * p].Nintr};
+        LensBroadcast u{};
+        if(!broadcast_prepare<2>(u, "stereo_pair_reproject", 0, 1, shape, st, width)) return false;
+        u.in[0] = d_q;
+        u.in[1] = d_intr + off[2 * p];
+        u.lens = lens[2 * p].a;
+        u.Nintr = lens[2 * p].Nintr;
+        u.behind_ok = mrcal_lensmodel_metadata(&lensmodels[2 * p]).can_project_behind_camera;
+        u.normalize = true;
+        u.out[0] = d_v;
+        LensArgs a1 = lens[2 * p + 1].a;
         a1.intr = d_intr + off[2 * p + 1];
-        const bool behind_ok = mrcal_lensmodel_metadata(&lensmodels[2 * p]).can_project_behind_camera;
         const double* ref = p == 0 ? d_zero : d_q1;
         double* dst = p == Npairs - 1 ? d_out : d_q1;
-        if(!dispatch_lens_kind(lens[2 * p].kind, [&](auto k)
-           {
-               unproject_kernel<decltype(k)::value><<<blocks, 128, 0, D.stream>>>(a0, d_q, N, d_v, nullptr, nullptr, 0,
-                                                                                  behind_ok, true);
-           }) ||
+        if(!dispatch_lens_kind(lens[2 * p].kind, [&](auto k) { launch_unproject<decltype(k)::value>(u, D.stream); }) ||
            !dispatch_lens_kind(lens[2 * p + 1].kind, [&](auto k)
            {
                reproject_diff_kernel<decltype(k)::value><<<blocks, 128, 0, D.stream>>>(a1, d_Rt + 12 * p, ref, d_v, d_dist,

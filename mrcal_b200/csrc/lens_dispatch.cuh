@@ -89,17 +89,19 @@ inline bool lens_setup(HostLens* L, const mrcal_lensmodel_t* lensmodel)
     return true;
 }
 
-// unproject() needs a central projection: false + set_error() for CAHVORE with E != 0, the reference's rule
-// (mrcal.c:3203-3214)
+// unproject() needs a central projection: the refusal of CAHVORE with E != 0, the reference's rule (mrcal.c:3203-3214)
+inline bool refuse_noncentral()
+{
+    set_error("unproject() currently only works with a central projection. So I cannot unproject(CAHVORE,E!=0)");
+    return false;
+}
+
+// false + refuse_noncentral() for CAHVORE with E != 0 in the (host) intrinsics
 inline bool central_projection(const HostLens& L, const double* intrinsics)
 {
     if(L.kind == LENS_CAHVORE)
         for(int i = L.Nintr - 3; i < L.Nintr; i++)
-            if(intrinsics[i] != 0.)
-            {
-                set_error("unproject() currently only works with a central projection. So I cannot unproject(CAHVORE,E!=0)");
-                return false;
-            }
+            if(intrinsics[i] != 0.) return refuse_noncentral();
     return true;
 }
 

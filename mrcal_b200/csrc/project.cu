@@ -1,10 +1,12 @@
-// mrcal_project() / mrcal_unproject(): the reference's point-wise entry points
-// (mrcal.h:165-224, mrcal.c:2866-3080 and :3082-3270), host buffers in and out,
-// one thread per point on the device. They use the same lens-model device functions
-// as the residual kernels (device_math.cuh); the unprojection is unproject.cuh's. With them, the unprojection with
-// gradients (mrcal/projections.py:112-397) and model_resolution__deg_pixel() (mrcal/model_analysis.py:2152-2246).
+// mrcal_project() / mrcal_unproject(): the reference's point-wise entry points (mrcal.h:165-224, mrcal.c:2866-3080
+// and :3082-3270), and mrcal_b200_project(): the same projections broadcast over stacked intrinsics, with host or device
+// buffers. One thread per element on the device, in the broadcast frame of unproject.cuh (LensBroadcast): the
+// entries for one intrinsics vector repeat it through stride 0. They use the same lens-model device functions as the
+// residual kernels (device_math.cuh); the unprojection is unproject.cuh's. With them, the unprojection with gradients
+// (mrcal/projections.py:112-397) and model_resolution__deg_pixel() (mrcal/model_analysis.py:2152-2246).
 #include <cuda_runtime.h>
 
+#include "broadcast.cuh"
 #include "common.h"
 #include "device_call.h"
 #include "device_math.cuh"
@@ -14,22 +16,31 @@
 namespace mb200 {
 namespace {
 
-// dq_di: dense (N,2,Nintr), zeroed by the caller, or NULL; IntrinsicsGradient::scatter() fills its nonzero entries
+enum { F_GRAD = MRCAL_B200_PROJECT_GET_GRADIENTS, F_UNPROJECT = MRCAL_B200_PROJECT_UNPROJECT,
+       F_NORMALIZE = MRCAL_B200_PROJECT_NORMALIZE };
+
+// One thread per point: q (2), and if given, dq_dp (2,3) = out[1] and dq_di (2,Nintr) = out[2] (zeroed by the caller;
+// IntrinsicsGradient::scatter() fills its nonzero entries)
 template <int KIND>
-__global__ void project_kernel(LensArgs a, const double* __restrict__ p, int N, double* __restrict__ q, double* __restrict__ dq_dp,
-                               double* __restrict__ dq_di, int Nintr)
+__global__ void project_kernel(const LensBroadcast b)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if(i >= N) return;
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(i >= b.N) return;
+    int64_t o[2];
+    const LensArgs a = lens_element(b, i, o);
+    double* __restrict__ q = b.out[0];
+    double* __restrict__ dq_dp = b.out[1];
+    double* __restrict__ dq_di = b.out[2];
+    const int Nintr = b.Nintr;
     double qq[2], g[2][3];
-    const double pp[3] = {p[3 * i], p[3 * i + 1], p[3 * i + 2]};
+    const double pp[3] = {b.in[0][o[0]], b.in[0][o[0] + 1], b.in[0][o[0] + 2]};
     if(dq_di == nullptr) project_any<KIND>(qq, g, pp, a);
     else
     {
         IntrinsicsGradient<KIND> G;
         G.project(g, pp, a);
         qq[0] = G.q[0]; qq[1] = G.q[1];
-        double* out = dq_di + (size_t)i * 2 * Nintr;
+        double* out = dq_di + i * 2 * Nintr;
         G.scatter(a, [&](int k, int col, double val) { out[k * Nintr + col] = val; });
     }
     q[2 * i] = qq[0]; q[2 * i + 1] = qq[1];
@@ -80,44 +91,82 @@ __global__ void resolution_kernel(LensArgs a, const double* __restrict__ q, int 
              mode == MB200_RESOLUTION_ECCENTRICITY ? rmax / rmin : (rmin + rmax) / 2.;
 }
 
-enum Call { PROJECT, UNPROJECT, RESOLUTION };
-
-// PROJECT: p [N][3] -> q [N][2], dq_dp [N][2][3], dq_di [N][2][Nintr]. UNPROJECT: q [N][2] -> v [N][3], dv_dq
-// [N][3][2], dv_di [N][3][Nintr], normalized if opt. RESOLUTION: q [N][2] -> [N] in mode opt. The gradients may be NULL
-bool run(Call call, double* out, double* grad, double* gi, const double* in, int N, const mrcal_lensmodel_t* lensmodel,
-         const double* intrinsics, int opt = 0)
+// flag = 1 if any intrinsics row of r (CAHVORE, Nintr) has E != 0. One thread per row
+__global__ void noncentral_kernel(const Broadcast<1> r, int Nintr, int* flag)
 {
-    DeviceCall D;
-    HostLens L;
-    if(!D.start() || !lens_setup(&L, lensmodel)) return false;
-    if(N <= 0) return true;
-    if(call != PROJECT && !central_projection(L, intrinsics)) return false;
-    const int Nintr = L.Nintr;
-    const size_t nin = (size_t)N * (call == PROJECT ? 3 : 2), nout = (size_t)N * (call == PROJECT ? 2 : call == UNPROJECT ? 3 : 1);
-    const size_t ngi = (size_t)N * (call == PROJECT ? 2 : 3) * Nintr;
-    double *d_intr, *d_in, *d_out, *d_grad = nullptr, *d_gi = nullptr;
-    if(!D.upload(&d_intr, intrinsics, (size_t)Nintr) || !D.upload(&d_in, in, nin) || !D.alloc(&d_out, nout) ||
-       (grad && !D.alloc(&d_grad, (size_t)N * 6)) || (gi && !D.alloc(&d_gi, ngi)))
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(i >= r.N) return;
+    int64_t o[1];
+    broadcast_offsets(r, i, o);
+    const double* E = r.in[0] + o[0] + Nintr - 3;
+    if(E[0] != 0. || E[1] != 0. || E[2] != 0.) *flag = 1;
+}
+
+// The checks both flavours of mrcal_b200_project() make, and the broadcast frame of the call; the operands and outputs
+// are not filled in
+bool prepare(LensBroadcast& b, HostLens& L, const mrcal_lensmodel_t* lensmodel, int flags, int ndim,
+             const int64_t* shape, const int64_t* strides_in, const int64_t* strides_intrinsics)
+{
+    if(flags & ~(F_GRAD | F_UNPROJECT | F_NORMALIZE) || ((flags & F_NORMALIZE) && !(flags & F_UNPROJECT)))
+    {
+        set_error("project: invalid flags 0x%x", flags);
         return false;
-    if(gi) MB200_CUDA_CHECK(cudaMemsetAsync(d_gi, 0, ngi * sizeof(double), D.stream));
-    L.a.intr = d_intr;
-    const mrcal_lensmodel_metadata_t meta = mrcal_lensmodel_metadata(lensmodel);
-    const int threads = 128, blocks = (N + threads - 1) / threads;
-    const bool ok = dispatch_lens_kind(L.kind, [&](auto k)
+    }
+    if(!lens_setup(&L, lensmodel)) return false;
+    const int64_t* const st[2] = {strides_in, strides_intrinsics};
+    const int width[2] = {flags & F_UNPROJECT ? 2 : 3, L.Nintr};
+    b = LensBroadcast{};
+    if(!broadcast_prepare<2>(b, "project", flags, ndim, shape, st, width)) return false;
+    b.lens = L.a;
+    b.Nintr = L.Nintr;
+    b.behind_ok = mrcal_lensmodel_metadata(lensmodel).can_project_behind_camera;
+    b.normalize = flags & F_NORMALIZE;
+    return true;
+}
+
+// The projection (or with F_UNPROJECT the unprojection) of every element of b on stream, b's operands and outputs on
+// the device. out[2], the dense intrinsics gradient, is zeroed first: the kernels write only its nonzero entries
+bool launch(const LensBroadcast& b, int kind, int flags, cudaStream_t stream)
+{
+    const size_t rows = flags & F_UNPROJECT ? 3 : 2;
+    if(b.out[2]) MB200_CUDA_CHECK(cudaMemsetAsync(b.out[2], 0, (size_t)b.N * rows * b.Nintr * sizeof(double), stream));
+    const bool ok = dispatch_lens_kind(kind, [&](auto k)
     {
         constexpr int K = decltype(k)::value;
-        if(call == UNPROJECT)
-            unproject_kernel<K><<<blocks, threads, 0, D.stream>>>(L.a, d_in, N, d_out, d_grad, d_gi, Nintr,
-                                                                  meta.can_project_behind_camera, opt != 0);
-        else if(call == PROJECT)
-            project_kernel<K><<<blocks, threads, 0, D.stream>>>(L.a, d_in, N, d_out, d_grad, d_gi, Nintr);
-        else
-            resolution_kernel<K><<<blocks, threads, 0, D.stream>>>(L.a, d_in, N, d_out, opt, meta.can_project_behind_camera);
+        if(flags & F_UNPROJECT) launch_unproject<K>(b, stream);
+        else project_kernel<K><<<(unsigned)((b.N + 127) / 128), 128, 0, stream>>>(b);
     });
     if(!ok) return false;
     MB200_CUDA_CHECK(cudaGetLastError());
-    return D.download(out, d_out, nout) && (!grad || D.download(grad, d_grad, (size_t)N * 6)) &&
-           (!gi || D.download(gi, d_gi, ngi)) && D.finish();
+    return true;
+}
+
+// mrcal_project(), mrcal_unproject(), mrcal_b200_unproject_with_gradients(): N points or pixels of one intrinsics
+// vector, host buffers. flags: F_*; the gradients may be NULL
+bool run(int flags, double* out, double* grad, double* gi, const double* in, int N, const mrcal_lensmodel_t* lensmodel,
+         const double* intrinsics)
+{
+    // shape (N,): the points packed, the intrinsics repeated
+    const int w_in = flags & F_UNPROJECT ? 2 : 3, w_out = 5 - w_in;
+    const int64_t shape[1] = {N > 0 ? N : 0}, st_in[1] = {w_in}, st_intr[1] = {0};
+    DeviceCall D;
+    HostLens L;
+    LensBroadcast b;
+    if(!D.start() || !prepare(b, L, lensmodel, flags, 1, shape, st_in, st_intr)) return false;
+    if(N <= 0) return true;
+    if((flags & F_UNPROJECT) && !central_projection(L, intrinsics)) return false;
+    const size_t nin = (size_t)N * w_in, nout = (size_t)N * w_out, ngi = (size_t)N * w_out * L.Nintr;
+    double *d_intr, *d_in, *d_out, *d_grad = nullptr, *d_gi = nullptr;
+    if(!D.upload(&d_intr, intrinsics, (size_t)L.Nintr) || !D.upload(&d_in, in, nin) || !D.alloc(&d_out, nout) ||
+       (grad && !D.alloc(&d_grad, (size_t)N * 6)) || (gi && !D.alloc(&d_gi, ngi)))
+        return false;
+    b.in[0] = d_in;
+    b.in[1] = d_intr;
+    b.out[0] = d_out;
+    b.out[1] = d_grad;
+    b.out[2] = d_gi;
+    return launch(b, L.kind, flags, D.stream) && D.download(out, d_out, nout) &&
+           (!grad || D.download(grad, d_grad, (size_t)N * 6)) && (!gi || D.download(gi, d_gi, ngi)) && D.finish();
 }
 
 }  // namespace
@@ -129,21 +178,94 @@ using namespace mb200;
 extern "C" bool mrcal_project(mrcal_point2_t* q, mrcal_point3_t* dq_dp, double* dq_dintrinsics,
                               const mrcal_point3_t* p, int N, const mrcal_lensmodel_t* lensmodel, const double* intrinsics)
 {
-    return run(PROJECT, (double*)q, (double*)dq_dp, dq_dintrinsics, (const double*)p, N, lensmodel, intrinsics);
+    return run(F_GRAD, (double*)q, (double*)dq_dp, dq_dintrinsics, (const double*)p, N, lensmodel, intrinsics);
 }
 
 // replaces mrcal.h:193-224
 extern "C" bool mrcal_unproject(mrcal_point3_t* out, const mrcal_point2_t* q, int N,
                                 const mrcal_lensmodel_t* lensmodel, const double* intrinsics)
 {
-    return run(UNPROJECT, (double*)out, nullptr, nullptr, (const double*)q, N, lensmodel, intrinsics);
+    return run(F_UNPROJECT, (double*)out, nullptr, nullptr, (const double*)q, N, lensmodel, intrinsics);
 }
 
 extern "C" bool mrcal_b200_unproject_with_gradients(mrcal_point3_t* v, double* dv_dq, double* dv_dintrinsics,
                                                     const mrcal_point2_t* q, int N, const mrcal_lensmodel_t* lensmodel,
                                                     const double* intrinsics, bool normalize)
 {
-    return run(UNPROJECT, (double*)v, dv_dq, dv_dintrinsics, (const double*)q, N, lensmodel, intrinsics, normalize);
+    return run(F_GRAD | F_UNPROJECT | (normalize ? F_NORMALIZE : 0), (double*)v, dv_dq, dv_dintrinsics,
+               (const double*)q, N, lensmodel, intrinsics);
+}
+
+extern "C" bool mrcal_b200_project(const mrcal_lensmodel_t* lensmodel, int flags, int ndim, const int64_t* shape,
+                                   const double* in, const int64_t* strides_in, const double* intrinsics,
+                                   const int64_t* strides_intrinsics, double* out, double* dout_din,
+                                   double* dout_dintrinsics)
+{
+    LensBroadcast b;
+    HostLens L;
+    if(!prepare(b, L, lensmodel, flags, ndim, shape, strides_in, strides_intrinsics)) return false;
+    if(b.N == 0) return true;
+    if(flags & F_UNPROJECT)
+    {
+        // every intrinsics row the call reads must be central
+        b.in[1] = intrinsics;
+        const Broadcast<1> rows = broadcast_rows(b, 1);
+        for(int64_t r = 0; r < rows.N; r++)
+        {
+            int64_t o[1];
+            broadcast_offsets(rows, r, o);
+            if(!central_projection(L, intrinsics + o[0])) return false;
+        }
+    }
+    const bool G = flags & F_GRAD;
+    const int w_in = flags & F_UNPROJECT ? 2 : 3, w_out = 5 - w_in;
+    const size_t n0 = b.N * w_out, n1 = G && dout_din ? b.N * 6 : 0, n2 = G && dout_dintrinsics ? b.N * w_out * L.Nintr : 0;
+    DeviceCall D;
+    const double *d_in, *d_intr;
+    double *d_out, *d_grad = nullptr, *d_gi = nullptr;
+    if(!D.start() || !D.upload((double**)&d_in, in, broadcast_extent(b, 0, w_in)) ||
+       !D.upload((double**)&d_intr, intrinsics, broadcast_extent(b, 1, L.Nintr)) || !D.alloc(&d_out, n0) ||
+       (n1 && !D.alloc(&d_grad, n1)) || (n2 && !D.alloc(&d_gi, n2)))
+        return false;
+    b.in[0] = d_in;
+    b.in[1] = d_intr;
+    b.out[0] = d_out;
+    b.out[1] = d_grad;
+    b.out[2] = d_gi;
+    return launch(b, L.kind, flags, D.stream) && D.download(out, d_out, n0) &&
+           (!n1 || D.download(dout_din, d_grad, n1)) && (!n2 || D.download(dout_dintrinsics, d_gi, n2)) && D.finish();
+}
+
+extern "C" bool mrcal_b200_project_device(const mrcal_lensmodel_t* lensmodel, int flags, int ndim, const int64_t* shape,
+                                          const double* in, const int64_t* strides_in, const double* intrinsics,
+                                          const int64_t* strides_intrinsics, double* out, double* dout_din,
+                                          double* dout_dintrinsics, void* stream)
+{
+    LensBroadcast b;
+    HostLens L;
+    if(!prepare(b, L, lensmodel, flags, ndim, shape, strides_in, strides_intrinsics)) return false;
+    if(b.N == 0) return true;
+    if(!have_device()) return false;
+    b.in[0] = in;
+    b.in[1] = intrinsics;
+    if((flags & F_UNPROJECT) && L.kind == LENS_CAHVORE)
+    {
+        // every intrinsics row the call reads must be central: one flag back to the host, so this call waits
+        DeviceCall D;
+        int *d_flag, flag = 0;
+        if(!D.start((cudaStream_t)stream) || !D.alloc(&d_flag, 1)) return false;
+        MB200_CUDA_CHECK(cudaMemsetAsync(d_flag, 0, sizeof(int), D.stream));
+        const Broadcast<1> rows = broadcast_rows(b, 1);
+        noncentral_kernel<<<(unsigned)((rows.N + 127) / 128), 128, 0, D.stream>>>(rows, L.Nintr, d_flag);
+        MB200_CUDA_CHECK(cudaGetLastError());
+        if(!D.download(&flag, d_flag, 1) || !D.finish()) return false;
+        if(flag) return refuse_noncentral();
+    }
+    const bool G = flags & F_GRAD;
+    b.out[0] = out;
+    b.out[1] = G ? dout_din : nullptr;
+    b.out[2] = G ? dout_dintrinsics : nullptr;
+    return launch(b, L.kind, flags, (cudaStream_t)stream);
 }
 
 extern "C" bool mrcal_b200_model_resolution__deg_pixel(double* resolution, const mrcal_point2_t* q, int N,
@@ -155,5 +277,23 @@ extern "C" bool mrcal_b200_model_resolution__deg_pixel(double* resolution, const
         set_error("Mode must be one of ('min','max','mean','eccentricity')");
         return false;
     }
-    return run(RESOLUTION, resolution, nullptr, nullptr, (const double*)q, N, lensmodel, intrinsics, mode);
+    DeviceCall D;
+    HostLens L;
+    if(!D.start() || !lens_setup(&L, lensmodel)) return false;
+    if(N <= 0) return true;
+    if(!central_projection(L, intrinsics)) return false;
+    double *d_intr, *d_q, *d_out;
+    if(!D.upload(&d_intr, intrinsics, (size_t)L.Nintr) || !D.upload(&d_q, (const double*)q, 2 * (size_t)N) ||
+       !D.alloc(&d_out, (size_t)N))
+        return false;
+    L.a.intr = d_intr;
+    const bool behind_ok = mrcal_lensmodel_metadata(lensmodel).can_project_behind_camera;
+    const int threads = 128, blocks = (N + threads - 1) / threads;
+    if(!dispatch_lens_kind(L.kind, [&](auto k)
+       {
+           resolution_kernel<decltype(k)::value><<<blocks, threads, 0, D.stream>>>(L.a, d_q, N, d_out, mode, behind_ok);
+       }))
+        return false;
+    MB200_CUDA_CHECK(cudaGetLastError());
+    return D.download(resolution, d_out, (size_t)N) && D.finish();
 }

@@ -1,13 +1,14 @@
 // The per-point unprojection of every lens kind: unproject_any(), used by the reprojection maps (image_transforms.cu)
-// and model_resolution__deg_pixel() (project.cu); its gradients, unproject_gradient(); the normalizations; and
-// unproject_kernel, which runs mrcal_unproject() and mrcal_b200_unproject_with_gradients() (project.cu) and the
-// unprojections of mrcal_b200_stereo_pair_reproject() (diff.cu).
+// and model_resolution__deg_pixel() (project.cu); its gradients, unproject_gradient(); the normalizations; the
+// broadcast frame of the point-wise lens kernels, LensBroadcast; and unproject_kernel, which runs every unprojection
+// entry of project.cu and the unprojections of mrcal_b200_stereo_pair_reproject() (diff.cu).
 //
 // Unprojection of the models without a closed form follows the reference's scheme (mrcal.c:3106-3270): search the 2D
 // stereographic coordinates u of the ray so that project(unproject_stereographic(u)) = q, seeded from the pinhole
 // ray. The reference hands that 2x2 problem to libdogleg; here it is a damped Newton iteration. Same fixed point,
 // same failure rule (residual^2/2 > 1e-4 -> NaN).
 #pragma once
+#include "broadcast.cuh"
 #include "device_math.cuh"
 #include "lens_dispatch.cuh"
 
@@ -179,28 +180,56 @@ __device__ __forceinline__ void normalize_with_gradient(double v[3], double dv_d
     }
 }
 
-// One thread per pixel: v [N][3], and if dv_dq [N][3][2] or dv_di [N][3][Nintr] is given, the gradients of
+// The frame of project_kernel (project.cu) and unproject_kernel: one thread per element of the broadcast shape, two
+// operands read in place through Broadcast<2> -- in[0] the point (3) or pixel (2), in[1] the intrinsics row (Nintr),
+// repeated through stride 0 where one row serves many elements. Every row shares one lens model: lens holds its spline
+// grid and configuration, and each thread points its own copy's intr at its row. out[0] the value, out[1] its gradient
+// in the point or pixel, out[2] its gradient in the intrinsics (dense, zeroed by the caller: only its nonzero entries
+// are written); packed, element e's at out[k] + e * (its size). The gradients may be NULL
+struct LensBroadcast : Broadcast<2>
+{
+    LensArgs lens;
+    int Nintr;
+    bool behind_ok, normalize;   // unprojection only
+    double* out[3];
+};
+
+// The lens arguments of element e: the call's, pointed at e's intrinsics row. o: e's offsets into the two operands
+__device__ __forceinline__ LensArgs lens_element(const LensBroadcast& b, int64_t e, int64_t o[2])
+{
+    broadcast_offsets(b, e, o);
+    LensArgs a = b.lens;
+    a.intr = b.in[1] + o[1];
+    return a;
+}
+
+// One thread per pixel: v (3), and if dv_dq (3,2) = out[1] or dv_di (3,Nintr) = out[2] is given, the gradients of
 // unproject_gradient() (dv_di zeroed by the caller: only its nonzero columns are written). normalize: unit rays, and
 // the gradients of the unit rays. A ray or dv/dq that is not finite gives NaN gradients
 template <int KIND>
-__global__ void unproject_kernel(LensArgs a, const double* __restrict__ q, int N, double* __restrict__ v,
-                                 double* __restrict__ dv_dq, double* __restrict__ dv_di, int Nintr, bool behind_ok,
-                                 bool normalize)
+__global__ void unproject_kernel(const LensBroadcast b)
 {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if(i >= N) return;
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if(i >= b.N) return;
+    int64_t o[2];
+    const LensArgs a = lens_element(b, i, o);
+    const double qx = b.in[0][o[0]], qy = b.in[0][o[0] + 1];
+    double* __restrict__ v = b.out[0];
+    double* __restrict__ dv_dq = b.out[1];
+    double* __restrict__ dv_di = b.out[2];
+    const int Nintr = b.Nintr;
     double out[3];
     if(dv_dq == nullptr && dv_di == nullptr)
     {
-        unproject_any<KIND>(out, q[2 * i], q[2 * i + 1], a, behind_ok);
-        if(normalize) normalize_or_zero<KIND>(out);
+        unproject_any<KIND>(out, qx, qy, a, b.behind_ok);
+        if(b.normalize) normalize_or_zero<KIND>(out);
         v[3 * i] = out[0]; v[3 * i + 1] = out[1]; v[3 * i + 2] = out[2];
         return;
     }
     double D[3][2];
     IntrinsicsGradient<KIND> G;
-    unproject_gradient<KIND>(out, D, G, q[2 * i], q[2 * i + 1], a, behind_ok);
-    if(normalize && !unit_rays<KIND>) normalize_with_gradient(out, D);
+    unproject_gradient<KIND>(out, D, G, qx, qy, a, b.behind_ok);
+    if(b.normalize && !unit_rays<KIND>) normalize_with_gradient(out, D);
     bool ok = isfinite(out[0]) && isfinite(out[1]) && isfinite(out[2]);
     for(int r = 0; r < 3; r++)
         for(int c = 0; c < 2; c++) ok = ok && isfinite(D[r][c]);
@@ -211,15 +240,21 @@ __global__ void unproject_kernel(LensArgs a, const double* __restrict__ q, int N
         for(int r = 0; r < 3; r++) { dv_dq[6 * i + 2 * r] = D[r][0]; dv_dq[6 * i + 2 * r + 1] = D[r][1]; }
     if(dv_di)
     {
-        double* o = dv_di + (size_t)i * 3 * Nintr;
+        double* row = dv_di + i * 3 * Nintr;
         if(!ok)
-            for(int j = 0; j < 3 * Nintr; j++) o[j] = nan("");
+            for(int j = 0; j < 3 * Nintr; j++) row[j] = nan("");
         else
             G.scatter(a, [&](int k, int col, double val)
             {
-                for(int r = 0; r < 3; r++) o[r * Nintr + col] -= D[r][k] * val;
+                for(int r = 0; r < 3; r++) row[r * Nintr + col] -= D[r][k] * val;
             });
     }
+}
+
+// The launch of unproject_kernel over b on stream: 128 threads per block
+template <int KIND> void launch_unproject(const LensBroadcast& b, cudaStream_t stream)
+{
+    unproject_kernel<KIND><<<(unsigned)((b.N + 127) / 128), 128, 0, stream>>>(b);
 }
 
 }  // namespace mb200

@@ -12,6 +12,7 @@ torch.cuda.current_stream() without waiting for it. Leading dimensions broadcast
 broadcast is read in place, never expanded. out= writes the results into the given array(s) (a tuple with gradients)
 and returns them. identity_*() are host-only.
 """
+import ctypes as C
 from functools import reduce
 
 import numpy as np
@@ -70,15 +71,18 @@ def _strides(x, lead, nproto, torch):
 
 
 def _pose(fname, args, protos_in, protos_out, out, get_gradients=False, inverted0=False, inverted1=False,
-          entry="poseutils", op=None):
+          entry="poseutils", op=None, lensmodel=None,
+          names=("the first input", "the second input", "the third input")):
     """The outputs of operation fname on args: each args[k] of shape (..., *protos_in[k]), the leading dimensions
     broadcast together; the value, then (with get_gradients) the gradients, of shapes (broadcast, *protos_out[k]).
     entry: the C entry point, mrcal_b200_<entry>() (two inputs, three outputs: the pose utilities) or its _device
-    flavour; "triangulate" has three inputs and four outputs. op: the operation code (default: fname's pose code)"""
+    flavour; "triangulate" has three inputs and four outputs. op: the operation code (default: fname's pose code).
+    lensmodel (a parsed lens model, with entry "project"): the call is mrcal_b200_project[_device]() of that model,
+    args the points or pixels and the intrinsics, op its MRCAL_B200_PROJECT_* flags other than the gradients; the
+    outputs it is not given are not computed. names: the inputs' names in the messages"""
     outs = tuple(out) if isinstance(out, (tuple, list)) else ((out,) if out is not None else None)
     torch = _torch_if_tensors(*args, *(outs or ()), what=f"{fname}(): the inputs and out")
     device = None if torch is None else args[0].device
-    names = ("the first input", "the second input", "the third input")
     args = [_operand(a, p, names[k], fname, torch, device) for k, (a, p) in enumerate(zip(args, protos_in))]
     leads = [tuple(a.shape)[:len(a.shape) - len(p)] for a, p in zip(args, protos_in)]
     try:
@@ -111,14 +115,17 @@ def _pose(fname, args, protos_in, protos_out, out, get_gradients=False, inverted
     if int(np.prod(lead)) > 0:
         flags = (_GET_GRADIENTS if get_gradients else 0) | (_INVERTED0 if inverted0 else 0) | \
             (_INVERTED1 if inverted1 else 0)
-        nin, nout = (2, 3) if entry == "poseutils" else (3, 4)
+        nin, nout = (3, 4) if entry == "triangulate" else (2, 3)
         st = [_strides(a, lead, len(p), torch) for a, p in zip(args, protos_in)] + [None] * (nin - len(args))
         shape = np.array(lead, np.int64)
         ptr = (lambda a: a.ctypes.data) if torch is None else (lambda a: a.data_ptr())
         ins = [ptr(a) for a in args] + [None] * (nin - len(args))
         o = [ptr(r) for r in res] + [None] * (nout - len(res))
         call = (_ptr(shape), *(x for k in range(nin) for x in (ins[k], _ptr(st[k]))), *o)
-        code = _OPS[fname] if op is None else op
+        if lensmodel is None:
+            code = _OPS[fname] if op is None else op
+        else:
+            code, flags = C.byref(lensmodel), flags | op
         if torch is None:
             _require_gpu()
             getattr(checked, f"mrcal_b200_{entry}")(code, flags, len(lead), *call)
