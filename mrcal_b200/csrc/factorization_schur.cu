@@ -123,15 +123,16 @@ __global__ void groups_tri_kernel(NormalBuffers N, double* __restrict__ Bf, int 
 }
 
 // Forward panels: Bs[r][64 blk + col] -= sum over the groups g that reach block blk of  Zf[r][g] Y_g[blk][:, col].
-// One CTA per (block, tile of kSolveTile right-hand sides); the groups in index order, 8 per stage, each padded to 8
-// unknowns. (The panels carry the solver's right-hand-side column at compact index n_c: not part of the factor)
+// One CTA per (tile of kSolveTile right-hand sides, block): the tiles on gridDim.x, which takes any count of right-hand
+// sides (gridDim.y stops at 65535 tiles); the groups in index order, 8 per stage, each padded to 8 unknowns. (The panels
+// carry the solver's right-hand-side column at compact index n_c: not part of the factor)
 __global__ void __launch_bounds__(256)
 panels_forward_tiled_kernel(NormalBuffers N, const double* __restrict__ Bf, int Nelim, double* __restrict__ Bs, int Nrhs)
 {
     extern __shared__ __align__(16) double dsm[];
     double (*sA)[kSolveTileLd] = reinterpret_cast<double (*)[kSolveTileLd]>(dsm);
     double (*sM)[kSolveTileLd] = reinterpret_cast<double (*)[kSolveTileLd]>(dsm + kSolveTile * kSolveTileLd);
-    const int blk = blockIdx.x, r0 = blockIdx.y * kSolveTile;
+    const int blk = blockIdx.y, r0 = blockIdx.x * kSolveTile;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g8 = lane >> 2, t4 = lane & 3;
     const int mt = warp >> 1, nt0 = (warp & 1) * 4;   // warp: rows mt*8.., n-tiles nt0..nt0+3
@@ -275,7 +276,8 @@ bool schur_solve_pieces(const mrcal_b200_factorization* F, double* Bf, double* B
         if(N.Ngroups > 0)
         {
             groups_tri_kernel<<<(unsigned)((gr + 127) / 128), 128, 0, s>>>(N, Bf, Nelim, Nrhs, true);
-            panels_forward_tiled_kernel<<<dim3(nblk, (Nrhs + kSolveTile - 1) / kSolveTile), 256, kSolveTileSmem, s>>>(N, Bf, Nelim, Bs, Nrhs);
+            panels_forward_tiled_kernel<<<dim3((Nrhs + kSolveTile - 1) / kSolveTile, nblk), 256, kSolveTileSmem, s>>>(N, Bf, Nelim, Bs, Nrhs);
+            MB200_CUDA_CHECK(cudaGetLastError());   // here: chol_solve() may configure its kernels, which clears it
         }
         if(N.n_c > 0 && !chol_solve(N.S, N.ldS, N.n_c, ws->invL, Bs, N.ldS, Nrhs, s, nullptr, 1)) return false;
         if(N.n_r > N.n_c) inactive_tri_kernel<<<(unsigned)((ir + 255) / 256), 256, 0, s>>>(N, F->ia_L, F->ia_first, Bi, Nrhs, true);

@@ -19,7 +19,9 @@ namespace mb200 {
 
 constexpr int kMaxDevices = 64;   // per-device one-time kernel configuration flags
 
-// Raises the limit of `kernel`'s dynamic shared memory to `bytes`, once per device (the attribute is per device)
+// Raises the limit of `kernel`'s dynamic shared memory to `bytes`, once per device (the attribute is per device).
+// A successful cudaFuncSetAttribute() clears the thread's last error, so a launch error still pending (an invalid launch
+// configuration just before) is reported here instead of being lost
 template <auto kernel>
 bool set_max_dynamic_smem(int bytes)
 {
@@ -29,6 +31,7 @@ bool set_max_dynamic_smem(int bytes)
     if(dev < 0 || dev >= kMaxDevices) { set_error("device index %d out of range", dev); return false; }
     if(!configured[dev])
     {
+        MB200_CUDA_CHECK(cudaGetLastError());
         MB200_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
         configured[dev] = true;
     }
